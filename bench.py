@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- image-pairs matched(+verified)/s on N B200s (BASELINE.json metric).
+"""bench.py -- image-pairs matched(+verified)/s on N H100s (BASELINE.json metric).
 
     python bench.py --gpus 1 --steps 2 --warmup 3
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 \
@@ -8,6 +8,9 @@
 
 A "step" is one pass of the hot path (exhaustive matching [+ two-view verification]) over every
 image pair of the synthetic scene.  Prints ONE JSON line (rank 0).
+
+--dump-outputs DIR writes what the last timed step returned to rank 0's caller as DIR/<name>.npy (a fixed sample of
+the pairs, see dump_outputs), so that two builds can be compared output for output on identical, seeded inputs.
 """
 import argparse
 import json
@@ -56,11 +59,13 @@ def parse_args():
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--pair-batch", type=int, default=0)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last step's results (sampled pairs) as DIR/<name>.npy")
     return ap.parse_args()
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,"
          "clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -160,6 +165,55 @@ def cpu_baseline(desc_np, n_feat, pairs, budget_s, verify, kpts_np=None, cam=Non
             out["sample"] += (f"; + oracle/ransac_seq.cpp (scalar fp64 sequential LO-RANSAC, E/F/H + decision) on {len(idx)} "
                               f"of the sampled pairs with >= 15 matches ({min(cores, len(idx))} threads, {wall:.1f} s)")
     return out, sample, res
+
+
+DUMP_BUDGET_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, res, pairs, verify):
+    """The results of one match_pairs call as .npy files: per sampled pair the image pair, its matches and (with
+    verification) its two-view geometry.  The sample is the first 256 pairs of the list (dense in overlapping images)
+    plus 256 more drawn with a fixed seed, so it is the same for every run with the same arguments; pairs are dropped
+    from the end until everything fits DUMP_BUDGET_BYTES."""
+    n = len(pairs)
+    rng = np.random.default_rng(20240601)
+    rest = rng.choice(np.arange(min(n, 256), n), size=min(256, max(n - 256, 0)), replace=False) if n > 256 else []
+    idx = np.unique(np.concatenate([np.arange(min(n, 256)), np.asarray(rest, np.int64)])).astype(np.int64)
+    rows = []
+    size = 0
+    for k in idx:
+        m = res.matches(int(k))
+        row = {"matches": m}
+        if verify:
+            g = res.two_view_geometry(int(k))
+            row.update(config=int(g.config), inliers=np.asarray(g.inlier_matches), F=g.F, E=g.E, H=g.H)
+        nbytes = 8 * len(m) + (8 * len(row["inliers"]) + 3 * 9 * 8 + 16 if verify else 0) + 24
+        if size + nbytes > DUMP_BUDGET_BYTES:
+            break
+        size += nbytes
+        rows.append((k, row))
+    os.makedirs(out_dir, exist_ok=True)
+    ks = np.array([k for k, _ in rows], np.int64)
+    arrays = {
+        "pair_index": ks.astype(np.float64),
+        "image_pairs": pairs[ks].astype(np.float32).reshape(-1, 2),
+        "num_matches": np.array([len(r["matches"]) for _, r in rows], np.float32),
+        "matches": np.concatenate([r["matches"] for _, r in rows] + [np.zeros((0, 2))]).astype(np.float32).reshape(-1, 2),
+        "total_matches": np.array([res.total_matches], np.float64),
+    }
+    if verify:
+        arrays.update(
+            config=np.array([r["config"] for _, r in rows], np.float32),
+            num_inliers=np.array([len(r["inliers"]) for _, r in rows], np.float32),
+            inlier_matches=np.concatenate([r["inliers"].reshape(-1, 2) for _, r in rows] + [np.zeros((0, 2))]
+                                          ).astype(np.float32).reshape(-1, 2),
+            F=np.array([np.asarray(r["F"], np.float64).reshape(9) for _, r in rows]).reshape(-1, 9),
+            E=np.array([np.asarray(r["E"], np.float64).reshape(9) for _, r in rows]).reshape(-1, 9),
+            H=np.array([np.asarray(r["H"], np.float64).reshape(9) for _, r in rows]).reshape(-1, 9),
+            num_verified=np.array([res.num_verified], np.float64))
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
+    return {"dir": out_dir, "pairs_sampled": int(len(ks)), "bytes": int(sum(a.nbytes for a in arrays.values()))}
 
 
 def resolve_config(args):
@@ -291,9 +345,10 @@ def main():
             dist.barrier()
         torch.cuda.synchronize()
 
-    def one_step(host=None):
+    def one_step(host=None, keep=False):
         """One pass of the hot path: shard -> whole set resident on this GPU (copy + ONE all-gather) -> match
-        (+ verify) this rank's pairs.  `host`: (desc, kpts) pinned host arrays of the local shard (e2e leg)."""
+        (+ verify) this rank's pairs.  `host`: (desc, kpts) pinned host arrays of the local shard (e2e leg).
+        `keep`: the results are returned as out["res"] instead of being freed."""
         w0 = time.perf_counter()
         if host is None:
             ctx.set_images_sharded(nfeat, first, count, d_desc.data_ptr(), d_kpts.data_ptr() if verify else None, cams,
@@ -312,7 +367,10 @@ def main():
             _ = res.matches(len(my_pairs) - 1)
             if verify:
                 _ = res.two_view_geometry(len(my_pairs) - 1)
-        res.free()
+        if keep:
+            out["res"] = res
+        else:
+            res.free()
         out["wall_ms"] = dict(upload=(w1 - w0) * 1e3, match_pairs=(w2 - w1) * 1e3, read_and_free=(time.perf_counter() - w2) * 1e3)
         return out
 
@@ -328,12 +386,17 @@ def main():
     t_wall0 = time.perf_counter()
     acc = dict(dev_ms=0.0, k1_ms=0.0, k1_n=0, ver_ms=0.0, ag_ms=0.0, up_ms=0.0)
     last = None
-    for _ in range(args.steps):
-        last = one_step()
+    for step in range(args.steps):
+        last = one_step(keep=bool(args.dump_outputs) and step == args.steps - 1)
         for k in acc:
             acc[k] += last[k]
     barrier()
     wall_ms = (time.perf_counter() - t_wall0) * 1e3
+    dumped = None
+    if last is not None and "res" in last:
+        if rank == 0:
+            dumped = dump_outputs(args.dump_outputs, last["res"], my_pairs, bool(verify))
+        last["res"].free()
     if rank == 0:
         log(f"timed region done: {wall_ms / max(args.steps, 1):.0f} ms/step")
     clk = clocks.stop() if rank == 0 else None
@@ -390,39 +453,11 @@ def main():
             dist.destroy_process_group()
         return
 
-    # ---- roofline of the dominant kernel (K1: int8 GEMM + fused top-2), tensor-bound
-    peaks = {}
-    try:
-        peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-    except Exception:
-        pass
-    bf16 = peaks.get("bf16_tflops_sustained")
-    peak_src = "2 x MEASURED_PEAKS.json bf16_tflops_sustained (derived int8 peak: kind::i8 runs at twice the bf16 rate)"
-    if not bf16:
-        bf16, peak_src = 1400.0, "2 x fallback sustained bf16 1.4 PFLOP/s (B200_PROFILING.md), derived int8 peak"
-    peak = 2.0 * bf16
-    try:
-        # measured on this pool's B200 by tools/microbench.cu (tcgen05.mma.kind::i8 issue loop, all SMs)
-        mb = json.load(open(os.path.join(ROOT, "profiles", "r01_microbench_tmem_i8mma.json")))
-        peak = float(mb["i8_mma_n256_chip_TOPS"])
-        peak_src = ("measured int8 tcgen05 peak, tools/microbench.cu on this pool's B200 "
-                    "(profiles/r01_microbench_tmem_i8mma.json, burst, 1965 MHz)")
-    except Exception:
-        pass
-    # K1 is timed INSIDE a long step (the board sits at its power cap): the applicable peak is the SUSTAINED one
-    # (B200_PROFILING.md: burst for a kernel timed alone, sustained for a kernel inside a long step) -- the same MMA
-    # loop back to back for 4 s, tools/microbench.cu.  The burst figure and the fraction against it are kept beside it
-    # (round 1 quoted the burst fraction).
-    peak_burst, peak_burst_src = peak, peak_src
-    try:
-        mb = json.load(open(os.path.join(ROOT, "profiles", "r02_microbench_sustained.json")))
-        peak = float(mb["i8_mma_n256_chip_TOPS_sustained"])
-        peak_burst = float(mb["i8_mma_n256_chip_TOPS"])
-        peak_src = ("measured SUSTAINED int8 tcgen05 peak: tools/microbench.cu MMA loop back to back for 4 s on this pool's "
-                    "B200, last second timed (profiles/r02_microbench_sustained.json; 1725-1760 MHz at the 1 kW power cap); "
-                    "burst in the same run %.1f TOP/s at 1965 MHz" % peak_burst)
-    except Exception:
-        pass
+    # ---- roofline of the dominant kernel (K1: int8 GEMM + fused top-2), tensor-bound.  The peak is NVIDIA's data sheet
+    # figure for the H100 SXM (dense int8, card allowed 700 W), not a measured one: "clocks" beside it shows what the
+    # card ran at.
+    peak = 1979.0
+    peak_src = "H100 SXM data sheet: 1979 TOP/s dense int8 at up to 700 W (not measured)"
     ops_per_pair = 2.0 * K * K * 128
     k1_avg_ms = acc["k1_ms"] / max(acc["k1_n"], 1)
     pairs_per_launch = len(my_pairs) * args.steps / max(acc["k1_n"], 1)
@@ -433,15 +468,7 @@ def main():
     # api.cu match_pairs_impl: resolve + gather of batch b next to the RANSAC kernels of batch b - 1
     overlapped = (gathered and bool(verify) and not guided and "B2M_NO_OVERLAP" not in os.environ
                   and len(my_pairs) > pairs_per_launch)
-    traffic = None
-    try:   # dram__bytes_read.sum + dram__bytes_write.sum per launch of the schedule in use (profiles/, ncu --set full)
-        tr = json.load(open(os.path.join(ROOT, "profiles", "k1_traffic.json")))
-        key = f"{'gather' if gathered else 'split' if split else 'full'}_{K}"
-        traffic = tr[key]["bytes_per_pair"] * pairs_per_launch if key in tr else None
-    except Exception:
-        pass
     roof = {"bound": "tensor", "achieved": achieved, "peak": peak, "unit": "TOP/s", "frac": achieved / peak,
-            "traffic": traffic,
             "kernel": ("b2m_k1_filter_kernel x2 per batch: row direction of all pairs + column direction of the MATCHED columns "
                        "(gathered); " + ("overlapped order: K1 time = the two GEMM launches alone, CUDA events around each"
                                          if overlapped else
@@ -451,7 +478,6 @@ def main():
                        if split else "b2m_k1_filter_kernel"),
             "k1_dir1_mode": dir1_mode, "avg_launch_ms": k1_avg_ms,
             "pairs_per_launch": pairs_per_launch, "peak_source": peak_src,
-            "peak_burst": peak_burst, "frac_burst": achieved / peak_burst,
             "whole_step_frac": ops_per_pair * len(my_pairs) / (ms_per_step / 1e3) / 1e12 / peak,
             "algorithmic": "2*K1*K2*128 int8 ops per pair (one GEMM; the transposed GEMM of the cross-check "
                            "direction is not counted)"}
@@ -462,13 +488,13 @@ def main():
         res_e, res_f, res_h = st_end["verify_residuals"]
         flops = 33.0 * (res_e + res_f) + 19.0 * res_h
         ver_s = acc["ver_ms"] / 1e3
-        fp32_peak = 148 * 128 * 2 * 1.965e9 / 1e12
+        fp32_peak = 67.0
         roof_verify = {"bound": "alu", "residual_evaluations_per_s": (res_e + res_f + res_h) / max(ver_s, 1e-9),
                        "achieved": flops / max(ver_s, 1e-9) / 1e12, "unit": "TFLOP/s",
                        "peak": fp32_peak, "frac": flops / max(ver_s, 1e-9) / 1e12 / fp32_peak,
-                       "peak_fp64": 37.0,
-                       "peak_source": "nominal: fp32 148 SMs x 128 lanes x 2 x 1.965 GHz (the hypothesis-scoring loop is fp32 "
-                                      "with an exact fp64 recheck of borderline points); fp64 37 TFLOP/s (B200 datasheet)",
+                       "peak_fp64": 34.0,
+                       "peak_source": "H100 SXM data sheet at up to 700 W, not measured: fp32 67 TFLOP/s (the hypothesis-scoring "
+                                      "loop is fp32 with an exact fp64 recheck of borderline points); fp64 34 TFLOP/s",
                        "models_scored": list(st_end["verify_models_scored"]), "residuals": [res_e, res_f, res_h],
                        "ms_per_step": acc["ver_ms"] / args.steps,
                        "note": "time = resolve + cross-check compaction + E/F/H LO-RANSAC + decision kernels of this rank"}
@@ -527,6 +553,8 @@ def main():
         "gpu_launches": int(launches_total), "clocks": clk,
         "roofline": roof, "roofline_verify": roof_verify, "cpu_baseline": cb, "e2e": e2e,
     }
+    if dumped:
+        out["dump_outputs"] = dumped
     print(json.dumps(out))
     if world > 1:
         ctx.comm_destroy()

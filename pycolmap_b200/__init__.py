@@ -10,7 +10,7 @@ the reference:
     pycolmap.match_exhaustive(database_path, sift_options={"max_ratio": 0.8})
 
 No CPU fallback: the import fails loudly when the extension or the CUDA library is missing, and every entry
-point fails with B2M_ENODEV without an sm_100 device.
+point fails with B2M_ENODEV without an sm_90 device.
 """
 try:
     from ._core import *  # noqa: F401,F403

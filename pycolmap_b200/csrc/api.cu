@@ -104,7 +104,7 @@ int layout_images_impl(b2m_ctx* ctx, ImageSet& S, int n_images, const int32_t* n
                                 ctx->stream));
   }
   // One TMA tensor map over the whole set: dim0 = 128 descriptor bytes, dim1 = rows; box 128 x 128,
-  // SWIZZLE_128B so that the tile lands in the canonical K-major UMMA layout.
+  // SWIZZLE_128B so that the tile lands in the canonical K-major wgmma layout.
   PFN_encodeTiled enc = get_encode_tiled();
   if (!enc) return fail(ctx, B2M_ECUDA, "[api.cu] cuTensorMapEncodeTiled not available from the driver");
   cuuint64_t gdim[2] = {128, static_cast<cuuint64_t>(rows)};
@@ -269,7 +269,6 @@ int match_pairs_impl(b2m_ctx* ctx, ImageSet& S, const int32_t* pairs, int64_t n_
   const int64_t want = ctx->pair_batch_auto ? std::min<int64_t>(16384, std::max<int64_t>(1024, (int64_t{4096} * 8192) / rows_pad))
                                             : ctx->pair_batch;
   const int B = static_cast<int>(std::min<int64_t>(want, std::max<int64_t>(64, (int64_t{6} << 30) / (rows_pad * 128))));
-  // rows are handed out in 512-row cluster blocks: keep the per-pair stride a multiple of that
   // sized for the pairs of this call, not for a full batch: a context that only ever sees small jobs stays small
   if (int rc = ensure_workspace(ctx, static_cast<int>(std::min<int64_t>(B, std::max<int64_t>(n_pairs, 1))),
                                 round_up(S.max_feat_pad, 512)))
@@ -722,8 +721,10 @@ int b2m_device_count(void) {
   }
   int n = 0;
   for (int d = 0; d < ndev; ++d) {
-    int major = 0;
-    if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, d) == cudaSuccess && major == 10) n = d + 1;
+    int major = 0, minor = 0;
+    if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, d) == cudaSuccess &&
+        cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, d) == cudaSuccess && major == 9 && minor == 0)
+      n = d + 1;
   }
   return n;
 }
@@ -773,15 +774,15 @@ int b2m_create(const b2m_device_cfg* cfg, b2m_ctx** out) {
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
     cudaGetLastError();
     return fail(nullptr, B2M_ENODEV,
-                "[api.cu] no CUDA device visible: libb200match has no CPU fallback (B200 / sm_100 required)");
+                "[api.cu] no CUDA device visible: libb200match has no CPU fallback (H100 / sm_90 required)");
   }
   const int dev = cfg ? cfg->device : 0;
   if (dev < 0 || dev >= ndev) return fail(nullptr, B2M_EINVAL, "[api.cu] Check Failed: device ordinal in range");
   cudaDeviceProp prop;
   if (cudaGetDeviceProperties(&prop, dev) != cudaSuccess) return fail(nullptr, B2M_ECUDA, "cudaGetDeviceProperties");
-  if (prop.major != 10) {
+  if (prop.major != 9 || prop.minor != 0) {
     char b[256];
-    snprintf(b, sizeof(b), "[api.cu] device %d is sm_%d%d; this library is built for sm_100a only", dev, prop.major,
+    snprintf(b, sizeof(b), "[api.cu] device %d is sm_%d%d; this library is built for sm_90a only", dev, prop.major,
              prop.minor);
     return fail(nullptr, B2M_ENODEV, b);
   }

@@ -2,7 +2,7 @@
 // eigen-solver, real polynomial roots, 5-point essential (Nister elimination), 7-point and
 // normalised 8-point fundamental, normalised 4-point / N-point DLT homography, Sampson and
 // transfer residuals.  Header-only, fp64, `B2M_HD` = __host__ __device__ so that the same code is
-// unit-tested on the CPU (tests/helpers/geom_host.cpp) and runs one-hypothesis-per-thread on sm_100a.
+// unit-tested on the CPU (tests/helpers/geom_host.cpp) and runs one-hypothesis-per-thread on sm_90a.
 //
 // Semantics follow COLMAP 3.9.1 (SURVEY.md section 8 rows V4-V7):
 //   U:estimators/essential_matrix.cc   EssentialMatrixFivePointEstimator (>=5 points, <=10 models)

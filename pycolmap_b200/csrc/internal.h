@@ -89,11 +89,11 @@ int comm_allgather_regions(b2m_ctx* ctx, uint8_t* base, const std::vector<size_t
 
 struct b2m_ctx {
   int device = 0;
-  int num_sms = 148;
+  int num_sms = 132;
   uint64_t seed = 0;
   bool pair_batch_auto = true;  // no explicit b2m_device_cfg.pair_batch: the batch scales with the image size (api.cu)
   int pair_batch = 4096;  // pairs per kernel batch: ~380 verifiable pairs x 3 model kinds per launch keep the RANSAC
-                          // kernels at several CTAs per SM (A/B on 1000 x 8192: 1024 -> 4021, 4096 -> 3867, 8192 -> 3853 ms / step)
+                          // kernels at several CTAs per SM
   cudaStream_t stream = nullptr;
   cudaStream_t copy_stream = nullptr;
   cudaEvent_t ev_k[2] = {nullptr, nullptr};

@@ -1,37 +1,22 @@
-// match_filter_kernel.cu -- K1 (v14): persistent, clustered, pair-MMA tcgen05 int8 GEMM with a *filter*
-// epilogue, plus the exact resolve kernel.
+// match_filter_kernel.cu -- K1: persistent wgmma int8 GEMM with a *filter* epilogue, plus the exact
+// resolve kernel.
 //
-// Grid = one 2-CTA cluster per SM pair (74 clusters), persistent: every cluster walks a static list of
-// work items (image pair, direction, 256-row block of the "row" image A).
-//   * The two CTAs form a cta_group::2 pair: ONE elected thread of the leader CTA issues
-//     tcgen05.mma.cta_group::2.kind::i8 256x256x32 (four k-steps per 256-column tile of image B).  Each SM
-//     contributes its own 128-row A strip and stages only ITS 128-column half of every B tile, so each
-//     operand byte is written to and read from shared memory once per pair of SMs.
-//   * B streams through an 8-stage ring of 16 KiB half tiles (TMA, SWIZZLE_128B, both halves accounted on
-//     the leader's mbarrier); the A strips are double-buffered across work items, so the pipelines
-//     (TMA ring, TMEM accumulator stages, mbarrier phases) run straight across item boundaries and
-//     TMEM / barriers are set up once per launch.
-//   * Accumulators: TMEM, 2 stages x 256 columns = all 512 columns of each SM; every SM drains its own
-//     128 lanes.  Stage hand-back to the leader = one cluster-scope mbarrier arrival per epilogue warp
-//     (aggregating them on a shared-memory counter first was measured slower).
-//   * The TMA and MMA warps stay warp-converged and predicate only the tcgen05 / TMA instructions with
-//     elect.sync, so descriptors and addresses live in uniform registers.
+// Grid = one CTA per SM, persistent: every CTA walks a static list of work units (image pair, direction,
+// 256-row block of the "row" image A, 128-row half of that block).
+//   * Two consumer warpgroups each issue wgmma.mma_async m64n128k32 (u8 x u8 -> s32) for their 64 rows of
+//     the unit against each half of every 256-column tile of image B (four k-steps per half), accumulators in
+//     registers.  Halves rather than one m64n256 keep the 64 accumulators and the 32 slot maxima of a thread
+//     within the register budget of 288 threads per SM without spills.
+//   * One producer warp streams B through a 4-stage ring of 32 KiB tiles (TMA, SWIZZLE_128B) and the A
+//     strips through two buffers, so the pipeline runs straight across unit boundaries; barriers are set up
+//     once per launch.
+//   * While one warpgroup folds its accumulators the other one can use the tensor cores.
 //
-// Warp roles (19 warps, <= 96 registers per thread):
-//   warps 0..15  epilogue: warp w drains TMEM lane quarter w%4, column group w/4 (64 columns) of every tile
-//                with ONE round trip (four tcgen05.ld.x16 in flight, one wait::ld), hands the stage back, then
-//                folds the 64 accumulators of its row into 16 slot maxima.  What bounds K1 is the hand-shake
-//                chain MMA -> commit -> drain -> arrive -> MMA over only two accumulator stages, so the drain
-//                is kept to a single TMEM round trip and nothing else sits between wait::ld and the arrival.
-//   warp 16      TMA producer;  warp 17  MMA issuer (leader CTA only);
-//   warp 18      selector: turns the slot maxima of a finished item into reject / candidate decisions one item
-//                behind the epilogue warps, so the dependent global latencies (acos table, candidate counter)
-//                are off the chain.
-//
-// Filter: instead of an exact running top-2 (4 ALU ops per accumulator) each row keeps 64 "slot maxima"
-//     slot(g, r) = max over columns j = 256 t + 64 g + 16 c + r   (g = 0..3, r = 0..15; c = 0..3, all tiles t)
-// updated with two 3-input max (VIMNMX3) per four accumulators = 0.5 ALU op per accumulator.  At the end
-// of the row
+// Filter: instead of an exact running top-2 (4 ALU ops per accumulator) each row keeps 64 "slot maxima".
+// Thread lane l of a quad (q = l % 4) holds the columns 8 j + 2 q + e (j = 0..31, e = 0, 1) of its rows; its
+// slot r = 2 (j % 8) + e collects the four columns j = r / 2 + 8 c, c = 0..3, of every tile:
+//     slot(16 q + r) = max over columns 256 t + 64 c + 8 (r >> 1) + 2 q + (r & 1)     (c = 0..3, all tiles t)
+// At the end of the row
 //     best = max over slots (exact);   S1 = second largest slot maximum (multiset), which is a LOWER
 //     bound of the true second-best (= max(S1, second largest element inside the winning slot)).
 // acos is monotone, so a row failing `acos(best) <= max_distance`, or failing the ratio test already
@@ -40,8 +25,6 @@
 // with dp4a (all columns if several slots share the maximum), finds the lowest-index arg-max and the
 // hidden second-best, and applies the float32 test of FindBestMatchesOneWayBruteForce.  The match
 // indices are bit-identical to the exact kernel (match_kernel.cu) and to the CPU oracle.
-//
-// -DB2M_K1_PROF adds clock64 role counters (printed every 8th launch); see DESIGN.md for the readings.
 //
 // Semantics: U:feature/sift.cc (COLMAP 3.9.1), SURVEY.md section 8 rows M1-M3.
 #include <cstdio>
@@ -53,50 +36,34 @@ namespace b2m {
 namespace {
 
 constexpr int kDim = 128;
-constexpr int kTileM = 128;                        // rows per CTA and MMA (TMEM lanes)
-constexpr int kCluster = 2;                        // CTAs per cluster = one cta_group::2 pair
-constexpr int kRowsPerItem = kTileM * kCluster;    // 256 rows of A per work item == kRowPad
-constexpr int kTileN = 256;                        // columns per B tile: N = 256 hides the smem A read
-                                                   // (N <= 128 costs ~92 cycles per MMA regardless of N, profiles/r01_microbench2)
-constexpr int kUmmaK = 32;
-constexpr int kStages = 8;                         // B-tile ring depth (8 x 16 KiB: each CTA stages only ITS half)
-constexpr int kAccStages = 2;
-constexpr int kABufs = 2;                          // A strips double-buffered across work items
+constexpr int kTileM = 128;                        // rows per work unit: two consumer warpgroups of 64 rows
+constexpr int kRowsPerItem = 256;                  // rows of A per work item (two units) == kRowPad
+constexpr int kTileN = 256;                        // columns per B tile (the N of one wgmma)
+constexpr int kStages = 4;                         // B-tile ring depth
+constexpr int kABufs = 2;                          // A strips double-buffered across work units
 constexpr int kBytesA = kTileM * kDim;             // 16 KiB per strip
-constexpr int kBytesB = (kTileN / kCluster) * kDim;  // 16 KiB: this CTA's half (128 columns) of a B tile
-constexpr int kEpiWarps = 16;                      // warp w: TMEM lane quarter w%4, column group w/4 of every tile
-constexpr int kColGroups = kEpiWarps / 4;          // 4
-constexpr int kGroupCols = kTileN / kColGroups;    // 64 columns per warp and tile = four x16 loads
+constexpr int kBytesB = kTileN * kDim;             // 32 KiB per B tile
+constexpr int kConsumerWarps = 8;
 constexpr int kOwnSlots = 16;                      // slot maxima per row kept in one thread's registers
-constexpr int kSlots = kOwnSlots * kColGroups;     // 64 slot maxima per row
-constexpr int kSlotCols = kTileN / kSlots;         // 4 columns of every tile share a slot
-constexpr int kThreads = (kEpiWarps + 3) * 32;     // + TMA warp + MMA warp + selector warp
-constexpr int kAccCols = kTileN;                   // TMEM columns per accumulator stage
-constexpr uint32_t kIdesc = make_idesc_u8u8_s32(kTileM * kCluster, kTileN);  // one 256 x 256 x 32 MMA per CTA pair
-constexpr uint16_t kClusterMask = static_cast<uint16_t>((1u << kCluster) - 1u);
+constexpr int kSlots = kOwnSlots * 4;              // 64 slot maxima per row (four lanes of a quad)
+constexpr int kThreads = (kConsumerWarps + 1) * 32;  // + TMA producer warp
 static_assert(kRowsPerItem == kRowPad && kTileN == kRowPad, "images are padded to whole items / column tiles");
-static_assert(kGroupCols == 64 && kSlotCols == 4, "epilogue folds four x16 chunks into 16 slots");
 
 struct __align__(8) Barriers {
   uint64_t full_a[kABufs];
   uint64_t empty_a[kABufs];
   uint64_t full_b[kStages];
   uint64_t empty_b[kStages];
-  uint64_t tmem_full[kAccStages];
-  uint64_t tmem_empty[kAccStages];
-  uint64_t sel_full, sel_empty;  // slot maxima of an item handed to / consumed by the selector warp
-  uint32_t tmem_base;
 };
 
-constexpr int kMergeBytes = kTileM * kSlots * 4;   // slot maxima of one item, [slot][128 rows]
-constexpr size_t kSmemBytes = 1024 + kABufs * kBytesA + kStages * kBytesB + kMergeBytes + sizeof(Barriers);
+constexpr size_t kSmemBytes = 1024 + kABufs * kBytesA + kStages * kBytesB + sizeof(Barriers);
 
-// A work item and the data every warp role derives from its index (pure function of `w`).
+// A work unit and the data every warp role derives from its index (pure function of `w` and `half`).
 struct Item {
-  int pair, dir, nA, nB, rowA, rowB, n_tiles, row0;  // row0: first row (inside image A) of this CTA
+  int pair, dir, nA, nB, rowA, rowB, n_tiles, row0;  // row0: first row (inside image A) of this unit
   bool valid;
 };
-__device__ __forceinline__ Item decode_item(const MatchParams& p, int w, uint32_t cta_rank) {
+__device__ __forceinline__ Item decode_item(const MatchParams& p, int w, int half) {
   Item it;
   if (p.item_list) {
     // gathered column direction: rows = the gathered block of the pair (scratch tensor map), columns = image a
@@ -107,7 +74,7 @@ __device__ __forceinline__ Item decode_item(const MatchParams& p, int w, uint32_
     it.nA = p.gath_cnt[it.pair];
     it.nB = p.img_nfeat[ib];
     it.valid = cb * kRowsPerItem < it.nA;
-    it.row0 = cb * kRowsPerItem + static_cast<int>(cta_rank) * kTileM;
+    it.row0 = cb * kRowsPerItem + half * kTileM;
     it.rowA = it.pair * p.mstride + it.row0;
     it.rowB = p.img_row0[ib];
     it.n_tiles = (it.nB + kTileN - 1) / kTileN;
@@ -121,10 +88,10 @@ __device__ __forceinline__ Item decode_item(const MatchParams& p, int w, uint32_
   const int ib = p.pairs[2 * it.pair + (it.dir ^ 1)];
   it.nA = p.img_nfeat[ia];
   it.nB = p.img_nfeat[ib];
-  // same answer in both CTAs of the cluster; an empty image B still yields an item (n_tiles == 0)
+  // same answer for both halves of an item; an empty image B still yields a unit (n_tiles == 0)
   // so that its rows are written as "no match"
   it.valid = cb * kRowsPerItem < it.nA;
-  it.row0 = cb * kRowsPerItem + static_cast<int>(cta_rank) * kTileM;
+  it.row0 = cb * kRowsPerItem + half * kTileM;
   it.rowA = p.img_row0[ia] + it.row0;
   it.rowB = p.img_row0[ib];
   it.n_tiles = (it.nB + kTileN - 1) / kTileN;
@@ -133,32 +100,7 @@ __device__ __forceinline__ Item decode_item(const MatchParams& p, int w, uint32_
 
 }  // namespace
 
-#ifdef B2M_K1_PROF
-// role counters (SM cycles, summed over CTAs / warps): [0] MMA wait tmem_empty, [1] MMA wait full_b, [2] MMA issue,
-// [3] MMA tiles, [4] epi wait tmem_full, [5] epi drain (first ld .. wait::ld), [6] epi hand-back + fold,
-// [7] epi warp-tiles, [8] epi item tail (slot maxima -> shared memory), [9] epi items
-__device__ unsigned long long g_k1_prof[16];
-#define PROF_T(x) const long long x = clock64()
-#define PROF_ADD(acc, a, b) acc += (b) - (a)
-#else
-#define PROF_T(x)
-#define PROF_ADD(acc, a, b)
-#endif
-
-// elect.sync: true in exactly one (converged) lane.  The MMA / TMA roles keep their whole warp converged
-// and predicate only the tcgen05 / TMA instructions, so descriptors and addresses stay warp-uniform
-// (uniform registers) instead of being rebuilt in vector registers and moved over for every instruction.
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "elect.sync _|p, 0xffffffff;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(pred));
-  return pred != 0;
-}
-
-__global__ void __cluster_dims__(kCluster, 1, 1) __launch_bounds__(kThreads, 1)
+__global__ void __launch_bounds__(kThreads, 1)
 b2m_k1_filter_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ CUtensorMap tmap_a,
                      const MatchParams p) {
   // tmap: the resident descriptor set (column tiles; row strips too unless the rows are gathered), tmap_a: the row
@@ -166,295 +108,160 @@ b2m_k1_filter_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_cons
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* smA = smem;                                     // [kABufs][16 KiB]
-  uint8_t* smB = smem + kABufs * kBytesA;                  // [kStages][16 KiB]
-  uint32_t* merge = reinterpret_cast<uint32_t*>(smB + kStages * kBytesB);
-  Barriers* bars = reinterpret_cast<Barriers*>(smB + kStages * kBytesB + kMergeBytes);
+  uint8_t* smB = smem + kABufs * kBytesA;                  // [kStages][32 KiB]
+  Barriers* bars = reinterpret_cast<Barriers*>(smB + kStages * kBytesB);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const uint32_t cta_rank = cluster_ctarank();
-  const int cluster_id = blockIdx.x / kCluster;
-  const int n_clusters = gridDim.x / kCluster;
   // gathered column direction: the work list was built on the device, so was its length
-  const int n_items = p.item_list ? __ldg(p.n_items_ptr) : p.n_items;
+  const int n_units = 2 * (p.item_list ? __ldg(p.n_items_ptr) : p.n_items);
 
-  if (warp == kEpiWarps && lane == 0) {
+  if (warp == kConsumerWarps && lane == 0) {
     tma_prefetch_desc(&tmap);
     tma_prefetch_desc(&tmap_a);
     for (int s = 0; s < kABufs; ++s) {
       mbar_init(&bars->full_a[s], 1);
-      mbar_init(&bars->empty_a[s], 1);
+      mbar_init(&bars->empty_a[s], kConsumerWarps);
     }
     for (int s = 0; s < kStages; ++s) {
       mbar_init(&bars->full_b[s], 1);
-      mbar_init(&bars->empty_b[s], 1);  // the leader's pair-commit arrives here in both CTAs
+      mbar_init(&bars->empty_b[s], kConsumerWarps);
     }
-    for (int s = 0; s < kAccStages; ++s) {
-      mbar_init(&bars->tmem_full[s], 1);
-      mbar_init(&bars->tmem_empty[s], kCluster * kEpiWarps);  // leader only: one arrival per epilogue warp of the pair
-    }
-    mbar_init(&bars->sel_full, kEpiWarps);
-    mbar_init(&bars->sel_empty, 1);
     fence_mbar_init();
   }
-  if (warp == kEpiWarps + 1) {
-    tmem_alloc_pair(&bars->tmem_base, kAccStages * kAccCols);  // executed by the same warp of both CTAs
-    tmem_relinquish_pair();
-  }
-  tc_fence_before();
   __syncthreads();
-  cluster_sync_all();  // peer barriers are initialised before any remote arrival / multicast commit
-  tc_fence_after();
-  const uint32_t tmem_base = bars->tmem_base;
 
-  if (warp == kEpiWarps) {
-    // ===== TMA producer (whole warp converged, one elected lane issues) =====
-    uint32_t stage = 0, phase = 0, n_done = 0;
-    for (int w = cluster_id; w < n_items; w += n_clusters) {
-      const Item it = decode_item(p, w, cta_rank);
-      if (!it.valid) continue;
-      const uint32_t ab = n_done & 1, aph = (n_done >> 1) & 1;
-      ++n_done;
-      mbar_wait(&bars->empty_a[ab], aph ^ 1);  // the MMAs of the item that used this A buffer retired
-      if (elect_one()) {
-        // both CTAs' bytes are accounted on the LEADER's barriers (the leader issues the pair MMA)
-        if (cta_rank == 0) mbar_arrive_expect_tx(&bars->full_a[ab], kCluster * kBytesA);
-        tma_load_2d_pair(smA + ab * kBytesA, &tmap_a, &bars->full_a[ab], 0, it.rowA);
-      }
-      __syncwarp();
-      for (int t = 0; t < it.n_tiles; ++t) {
-        mbar_wait(&bars->empty_b[stage], phase ^ 1);
-        if (elect_one()) {
-          if (cta_rank == 0) mbar_arrive_expect_tx(&bars->full_b[stage], kCluster * kBytesB);
-          // this CTA stages only ITS 128-column half of the tile; the pair MMA reads the other half from
-          // the peer's shared memory, so each B byte is written to and read from shared memory once per pair
-          tma_load_2d_pair(smB + stage * kBytesB, &tmap, &bars->full_b[stage], 0,
-                           it.rowB + t * kTileN + static_cast<int>(cta_rank) * (kTileN / kCluster));
-        }
-        __syncwarp();
-        if (++stage == kStages) {
-          stage = 0;
-          phase ^= 1;
-        }
-      }
-    }
-  } else if (warp == kEpiWarps + 1) {
-    // ===== MMA issuer: the leader CTA's warp drives the 256-row MMAs of the pair (one elected lane issues) =====
-    if (cta_rank == 0) {
-      uint32_t stage = 0, phase = 0, as = 0, aphase = 0, n_done = 0;
-      const uint32_t smA_u32 = smem_u32(smA), smB_u32 = smem_u32(smB);
-#ifdef B2M_K1_PROF
-      long long pm_empty = 0, pm_fullb = 0, pm_issue = 0, pm_tiles = 0;
-#endif
-      for (int w = cluster_id; w < n_items; w += n_clusters) {
-        const Item it = decode_item(p, w, cta_rank);
-        if (!it.valid) continue;
+  if (warp == kConsumerWarps) {
+    // ===== TMA producer (one lane) =====
+    if (lane == 0) {
+      uint32_t stage = 0, phase = 0, n_done = 0;
+      for (int u = blockIdx.x; u < n_units; u += gridDim.x) {
+        const Item it = decode_item(p, u >> 1, u & 1);
+        if (!it.valid || it.n_tiles == 0) continue;
         const uint32_t ab = n_done & 1, aph = (n_done >> 1) & 1;
         ++n_done;
-        mbar_wait(&bars->full_a[ab], aph);
-        const uint64_t adesc = make_smem_desc_sw128(smA_u32 + ab * kBytesA);
-        if (it.n_tiles == 0) {  // nothing will read this A buffer: release it in both CTAs
-          if (elect_one()) {
-            mbar_arrive_cluster(&bars->empty_a[ab], 0);
-            mbar_arrive_cluster(&bars->empty_a[ab], 1);
-          }
-          __syncwarp();
-        }
+        mbar_wait(&bars->empty_a[ab], aph ^ 1);  // the MMAs of the unit that used this A buffer completed
+        mbar_arrive_expect_tx(&bars->full_a[ab], kBytesA);
+        tma_load_2d(smA + ab * kBytesA, &tmap_a, &bars->full_a[ab], 0, it.rowA);
         for (int t = 0; t < it.n_tiles; ++t) {
-          // B is normally resident long before the accumulator stage comes back: test it first so that
-          // nothing but the descriptor set-up sits between the stage hand-back and the first MMA
-          PROF_T(t1);
-          mbar_wait(&bars->full_b[stage], phase);
-          PROF_T(t2);
-          mbar_wait(&bars->tmem_empty[as], aphase ^ 1);
-          PROF_T(t0);
-          tc_fence_after();
-          const uint64_t bdesc = make_smem_desc_sw128(smB_u32 + stage * kBytesB);
-          const uint32_t tmem_d = tmem_base + as * kAccCols;
-          if (elect_one()) {
-#pragma unroll
-            for (int k = 0; k < kDim / kUmmaK; ++k)
-              mma_i8_ss_pair(tmem_d, adesc + 2 * k, bdesc + 2 * k, kIdesc, k > 0 ? 1u : 0u);
-            mma_commit_pair(&bars->tmem_full[as], kClusterMask);   // both CTAs' epilogues may drain (critical chain first)
-            mma_commit_pair(&bars->empty_b[stage], kClusterMask);  // both CTAs' producers may refill
-            if (t == it.n_tiles - 1) mma_commit_pair(&bars->empty_a[ab], kClusterMask);  // A buffers reusable
-          }
-          __syncwarp();
-#ifdef B2M_K1_PROF
-          {
-            PROF_T(t3);
-            PROF_ADD(pm_fullb, t1, t2);
-            PROF_ADD(pm_empty, t2, t0);
-            PROF_ADD(pm_issue, t0, t3);
-            ++pm_tiles;
-          }
-#endif
+          mbar_wait(&bars->empty_b[stage], phase ^ 1);
+          mbar_arrive_expect_tx(&bars->full_b[stage], kBytesB);
+          uint8_t* dst = smB + stage * kBytesB;
+          tma_load_2d(dst, &tmap, &bars->full_b[stage], 0, it.rowB + t * kTileN);
+          tma_load_2d(dst + kBytesA, &tmap, &bars->full_b[stage], 0, it.rowB + t * kTileN + 128);
           if (++stage == kStages) {
             stage = 0;
             phase ^= 1;
           }
-          if (++as == kAccStages) {
-            as = 0;
-            aphase ^= 1;
-          }
-        }
-      }
-#ifdef B2M_K1_PROF
-      if (lane == 0) {
-        atomicAdd(&g_k1_prof[0], (unsigned long long)pm_empty);
-        atomicAdd(&g_k1_prof[1], (unsigned long long)pm_fullb);
-        atomicAdd(&g_k1_prof[2], (unsigned long long)pm_issue);
-        atomicAdd(&g_k1_prof[3], (unsigned long long)pm_tiles);
-      }
-#endif
-    }
-  } else if (warp == kEpiWarps + 2) {
-    // ===== selector: slot maxima of one item (shared memory, [slot][row]) -> reject / candidate decisions =====
-    // Runs one item behind the epilogue warps, so the dependent global-memory latencies of the decision
-    // (acos table, candidate counter) are off the accumulator hand-shake chain.  Lane l owns rows l, l+32, ...
-    uint32_t sphase = 0;
-    for (int w = cluster_id; w < n_items; w += n_clusters) {
-      const Item it = decode_item(p, w, cta_rank);
-      if (!it.valid) continue;
-      mbar_wait(&bars->sel_full, sphase);
-      uint32_t best[4], s1[4];
-      int sstar[4];
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        best[q] = 0u;
-        s1[q] = 0u;
-        sstar[q] = 0;
-      }
-      // (largest, second largest) over the slot maxima, multiset semantics; lowest slot id on ties
-#pragma unroll 8
-      for (int r = 0; r < kSlots; ++r) {
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          const uint32_t v = merge[r * kTileM + q * 32 + lane];
-          if (v > best[q]) {
-            s1[q] = best[q];
-            best[q] = v;
-            sstar[q] = r;
-          } else {
-            s1[q] = max(s1[q], v);
-          }
-        }
-      }
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&bars->sel_empty);  // the epilogue warps may overwrite the buffer
-      sphase ^= 1;
-      float fa[4], fb[4];
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        fa[q] = __ldg(p.acos_lut + min(best[q], 262144u));
-        fb[q] = __ldg(p.acos_lut + min(s1[q], 262144u));
-      }
-      const int64_t base = (static_cast<int64_t>(it.pair) * 2 + it.dir) * p.mstride;
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        int32_t out = -1;
-        if (best[q] > 0u && !(fa[q] > p.max_distance) && !(fa[q] >= __fmul_rn(p.max_ratio, fb[q])))
-          out = -2 - sstar[q];  // candidate: resolve exactly
-        const int row = it.row0 + q * 32 + lane;
-        p.mbuf[base + row] = out;
-        if (out != -1 && row < it.nA) {
-          p.aux[base + row] = make_uint2(best[q], s1[q]);
-          const int k = atomicAdd(p.cand_cnt + it.pair * 2 + it.dir, 1);
-          p.cand_rows[base + k] = row | (sstar[q] << 24);  // winning slot travels with the row
         }
       }
     }
   } else {
-    // ===== filter epilogue =====
-    const int quarter = warp & 3;
-    const int group = warp >> 2;
-    const int row_in_cta = quarter * 32 + lane;
-    const uint32_t tcol = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + group * kGroupCols;
-    uint32_t as = 0, aphase = 0, sel_phase = 0;
-#ifdef B2M_K1_PROF
-    long long pe_full = 0, pe_drain = 0, pe_rest = 0, pe_tiles = 0, pe_tail = 0, pe_items = 0;
-#endif
-    for (int w = cluster_id; w < n_items; w += n_clusters) {
-      const Item it = decode_item(p, w, cta_rank);
+    // ===== consumers: MMA + filter epilogue =====
+    const int wg = warp >> 2;
+    const int q = lane & 3;
+    const int row_in_unit = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // rows row_in_unit and row_in_unit + 8
+    uint32_t acc[64];   // one 128-column half of a tile at a time: the slot maxima stay in registers beside it
+#pragma unroll
+    for (int i = 0; i < 64; ++i) acc[i] = 0u;
+    uint32_t stage = 0, phase = 0, n_done = 0;
+    for (int u = blockIdx.x; u < n_units; u += gridDim.x) {
+      const Item it = decode_item(p, u >> 1, u & 1);
       if (!it.valid) continue;
-      const int n_tiles = it.n_tiles;
-      uint32_t B[kOwnSlots];  // slot r: columns 64 g + 16 c + r, c = 0..3, of every tile
+      uint32_t S[2][kOwnSlots];   // slot maxima of the thread's two rows
 #pragma unroll
-      for (int r = 0; r < kOwnSlots; ++r) B[r] = 0u;
+      for (int i = 0; i < 2; ++i)
+#pragma unroll
+        for (int r = 0; r < kOwnSlots; ++r) S[i][r] = 0u;
+      if (it.n_tiles > 0) {
+        const uint32_t ab = n_done & 1, aph = (n_done >> 1) & 1;
+        ++n_done;
+        mbar_wait(&bars->full_a[ab], aph);
+        const uint32_t a_addr = smem_u32(smA + ab * kBytesA + wg * 64 * kDim);
 #pragma unroll 1
-      for (int t = 0; t < n_tiles; ++t) {
-        PROF_T(e0);
-        mbar_wait(&bars->tmem_full[as], aphase);
-        PROF_T(e1);
-        tc_fence_after();
-        const uint32_t taddr = tcol + as * kAccCols;
-        uint32_t v[4][16];
+        for (int t = 0; t < it.n_tiles; ++t) {
+          mbar_wait(&bars->full_b[stage], phase);
 #pragma unroll
-        for (int c = 0; c < 4; ++c) tmem_ld_32x16(taddr + c * 16, v[c]);
-        tmem_wait_ld();
-        PROF_T(e2);
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive_cluster(&bars->tmem_empty[as], 0);  // registers hold the tile: stage is free
+          for (int h = 0; h < 2; ++h) {
+            wgmma_tile_u8(acc, a_addr, smem_u32(smB + stage * kBytesB + h * (kBytesB / 2)));
+            if (h == 1) {
+              __syncwarp();
+              if (lane == 0) mbar_arrive(&bars->empty_b[stage]);   // the MMAs reading this stage have completed
+            }
+            // column 128 h + 8 j + 2 q + e (acc[4 j + 2 i + e], j < 16) = 64 c + 8 (r >> 1) + 2 q + (r & 1) with
+            // c = 2 h + j / 8, r = 2 (j % 8) + e
+#pragma unroll
+            for (int i = 0; i < 2; ++i)
+#pragma unroll
+              for (int r = 0; r < kOwnSlots; ++r) {
+                const int a0 = 4 * (r >> 1) + 2 * i + (r & 1);
+                S[i][r] = max(S[i][r], max(acc[a0], acc[a0 + 32]));
+              }
+          }
+          if (++stage == kStages) {
+            stage = 0;
+            phase ^= 1;
+          }
+        }
+        if (lane == 0) mbar_arrive(&bars->empty_a[ab]);
+      }
+      // (largest, second largest) over the 64 slot maxima of each row, multiset semantics, lowest slot id on ties:
+      // the thread's 16 slots first, then the four lanes of the quad (slot ids 16 q + r)
+      uint32_t best[2], s1[2];
+      int sstar[2];
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        best[i] = 0u;
+        s1[i] = 0u;
+        sstar[i] = 0;
 #pragma unroll
         for (int r = 0; r < kOwnSlots; ++r) {
-          const uint32_t m = max(B[r], max(v[0][r], v[1][r]));
-          B[r] = max(m, max(v[2][r], v[3][r]));
+          const uint32_t v = S[i][r];
+          if (v > best[i]) {
+            s1[i] = best[i];
+            best[i] = v;
+            sstar[i] = 16 * q + r;
+          } else {
+            s1[i] = max(s1[i], v);
+          }
         }
-#ifdef B2M_K1_PROF
-        {
-          PROF_T(e3);
-          PROF_ADD(pe_full, e0, e1);
-          PROF_ADD(pe_drain, e1, e2);
-          PROF_ADD(pe_rest, e2, e3);
-          ++pe_tiles;
-        }
-#endif
-        if (++as == kAccStages) {
-          as = 0;
-          aphase ^= 1;
-        }
-      }
-      // slot = 16 * group + r; all slot maxima of the item go to the selector warp through shared memory
-      // ([slot][row]: conflict-free for both sides); the buffer was consumed a whole item ago
-      PROF_T(x0);
-      mbar_wait(&bars->sel_empty, sel_phase ^ 1);
 #pragma unroll
-      for (int r = 0; r < kOwnSlots; ++r) merge[(group * kOwnSlots + r) * kTileM + row_in_cta] = B[r];
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&bars->sel_full);
-      sel_phase ^= 1;
-#ifdef B2M_K1_PROF
-      {
-        PROF_T(x1);
-        PROF_ADD(pe_tail, x0, x1);
-        ++pe_items;
+        for (int o = 1; o < 4; o <<= 1) {
+          const uint32_t ob = __shfl_xor_sync(0xffffffffu, best[i], o);
+          const uint32_t os = __shfl_xor_sync(0xffffffffu, s1[i], o);
+          const int oslot = __shfl_xor_sync(0xffffffffu, sstar[i], o);
+          const uint32_t ns = max(max(s1[i], os), min(best[i], ob));
+          if (ob > best[i] || (ob == best[i] && oslot < sstar[i])) {
+            best[i] = ob;
+            sstar[i] = oslot;
+          }
+          s1[i] = ns;
+        }
       }
-#endif
+      if (q < 2) {   // lane q of the quad decides row row_in_unit + 8 q
+        const uint32_t b = q ? best[1] : best[0], s = q ? s1[1] : s1[0];
+        const int slot = q ? sstar[1] : sstar[0];
+        const float fa = __ldg(p.acos_lut + min(b, 262144u));
+        const float fb = __ldg(p.acos_lut + min(s, 262144u));
+        int32_t out = -1;
+        if (b > 0u && !(fa > p.max_distance) && !(fa >= __fmul_rn(p.max_ratio, fb)))
+          out = -2 - slot;  // candidate: resolve exactly
+        const int64_t base = (static_cast<int64_t>(it.pair) * 2 + it.dir) * p.mstride;
+        const int row = it.row0 + row_in_unit + 8 * q;
+        p.mbuf[base + row] = out;
+        if (out != -1 && row < it.nA) {
+          p.aux[base + row] = make_uint2(b, s);
+          const int k = atomicAdd(p.cand_cnt + it.pair * 2 + it.dir, 1);
+          p.cand_rows[base + k] = row | (slot << 24);  // winning slot travels with the row
+        }
+      }
     }
-#ifdef B2M_K1_PROF
-    if (lane == 0) {
-      atomicAdd(&g_k1_prof[4], (unsigned long long)pe_full);
-      atomicAdd(&g_k1_prof[5], (unsigned long long)pe_drain);
-      atomicAdd(&g_k1_prof[6], (unsigned long long)pe_rest);
-      atomicAdd(&g_k1_prof[7], (unsigned long long)pe_tiles);
-      atomicAdd(&g_k1_prof[8], (unsigned long long)pe_tail);
-      atomicAdd(&g_k1_prof[9], (unsigned long long)pe_items);
-    }
-#endif
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();  // both CTAs are done with the pair's TMEM / barriers
-  if (warp == kEpiWarps + 1) {
-    tc_fence_after();
-    tmem_dealloc_pair(tmem_base, kAccStages * kAccCols);
   }
 }
 
 // Exact resolution of the candidate rows of one (pair, direction).
-// Slot s = 16 g + r holds the columns j = 256 t + 64 g + 16 c + r, c = 0..3, t = 0, 1, ... (slot_col below).
+// Slot s = 16 q + r holds the columns j = 256 t + 64 c + 8 (r >> 1) + 2 q + (r & 1), c = 0..3, t = 0, 1, ... (slot_col
+// below).
 // Candidates are bucketed by winning slot (counting sort in shared memory) so that the n2/64 columns
 // of a slot are staged in shared memory ONCE and reused by every candidate of the bucket (a warp per
 // candidate, dp4a, oracle scan order per lane, multiset-aware merge across lanes).  Rows whose
@@ -466,9 +273,9 @@ constexpr int kSlotColsMax = 256;      // columns of one slot staged in shared m
 constexpr int kResolveParts = 4;       // CTAs per (pair, direction); 1/2/4/8 measured within 1.5 % of each other
 constexpr int kSlotRowStride = 144;    // bytes; 128-byte descriptors padded so that LDS.128 is conflict-free
 
-// `it`-th column (ascending) of a slot: kSlotCols columns in every 256-column tile
+// `it`-th column (ascending) of a slot: four columns in every 256-column tile
 __device__ __forceinline__ int slot_col(int slot, int it) {
-  return 256 * (it >> 2) + 64 * (slot >> 4) + 16 * (it & 3) + (slot & 15);
+  return 256 * (it >> 2) + 64 * (it & 3) + 8 * ((slot & 15) >> 1) + 2 * (slot >> 4) + (slot & 1);
 }
 
 __device__ __forceinline__ uint32_t dot128(const uint32_t (&a)[32], const uint4* bp) {
@@ -670,27 +477,12 @@ cudaError_t launch_k1_filter(const CUtensorMap& tmap, const MatchParams& p_in,
   p.n_dirs = n_dirs;
   p.blocks_per_image = (max_strips * kTileM + kRowsPerItem - 1) / kRowsPerItem;
   p.n_items = n_pairs * n_dirs * p.blocks_per_image;
-  const int clusters = p.n_items < num_sms / kCluster ? p.n_items : num_sms / kCluster;
-  if (clusters > 0) {
-    b2m_k1_filter_kernel<<<clusters * kCluster, kThreads, kSmemBytes, stream>>>(tmap, tmap, p);
+  const int ctas = 2 * p.n_items < num_sms ? 2 * p.n_items : num_sms;
+  if (ctas > 0) {
+    b2m_k1_filter_kernel<<<ctas, kThreads, kSmemBytes, stream>>>(tmap, tmap, p);
     e = cudaGetLastError();
     if (e != cudaSuccess) return e;
   }
-#ifdef B2M_K1_PROF
-  {
-    static int n_launch = 0;
-    if (++n_launch % 8 == 0) {  // cumulative counters, printed every 8th launch
-      cudaStreamSynchronize(stream);
-      unsigned long long h[16];
-      cudaMemcpyFromSymbol(h, g_k1_prof, sizeof(h));
-      const double mt = h[3] ? double(h[3]) : 1.0, et = h[7] ? double(h[7]) : 1.0, ei = h[9] ? double(h[9]) : 1.0;
-      fprintf(stderr,
-              "[k1prof] per MMA tile: wait_empty %.0f wait_fullb %.0f issue %.0f | per epi warp-tile: wait_full %.0f "
-              "drain %.0f rest %.0f | per item tail %.0f (tiles/item %.1f)\n",
-              h[0] / mt, h[1] / mt, h[2] / mt, h[4] / et, h[5] / et, h[6] / et, h[8] / ei, et / ei);
-    }
-  }
-#endif
   if (after_filter) {
     e = cudaEventRecord(after_filter, stream);  // the roofline times the GEMM kernel alone
     if (e != cudaSuccess) return e;
@@ -747,10 +539,10 @@ cudaError_t launch_k1_filter_skip(const CUtensorMap& tmap, const MatchParams& p_
   p.n_dirs = 1;
   p.blocks_per_image = (max_strips * kTileM + kRowsPerItem - 1) / kRowsPerItem;
   p.n_items = n_pairs * p.blocks_per_image;
-  const int clusters = p.n_items < num_sms / kCluster ? p.n_items : num_sms / kCluster;
-  if (clusters > 0) {
+  const int ctas = 2 * p.n_items < num_sms ? 2 * p.n_items : num_sms;
+  if (ctas > 0) {
     // 1. row direction of every pair
-    b2m_k1_filter_kernel<<<clusters * kCluster, kThreads, kSmemBytes, stream>>>(tmap, tmap, p);
+    b2m_k1_filter_kernel<<<ctas, kThreads, kSmemBytes, stream>>>(tmap, tmap, p);
     e = cudaGetLastError();
     if (e != cudaSuccess) return e;
     // 2. live pairs swapped, dead pairs -> dummy image (0 features: every work item invalid)
@@ -767,7 +559,7 @@ cudaError_t launch_k1_filter_skip(const CUtensorMap& tmap, const MatchParams& p_
     q.cand_cnt = p.cand_cnt + 1;
     q.cand_rows = p.cand_rows + p.mstride;
     q.cand_sorted = p.cand_sorted + p.mstride;
-    b2m_k1_filter_kernel<<<clusters * kCluster, kThreads, kSmemBytes, stream>>>(tmap, tmap, q);
+    b2m_k1_filter_kernel<<<ctas, kThreads, kSmemBytes, stream>>>(tmap, tmap, q);
     e = cudaGetLastError();
     if (e != cudaSuccess) return e;
   }
@@ -899,9 +691,8 @@ cudaError_t launch_k1_gather_phase(int phase, const CUtensorMap& tmap, const CUt
   p.n_items = n_pairs * p.blocks_per_image;
   p.item_list = nullptr;
   p.gath_desc = nullptr;
-  const int max_clusters = num_sms / kCluster;
-  const int clusters = p.n_items < max_clusters ? p.n_items : max_clusters;
-  if (clusters <= 0) return cudaSuccess;
+  const int ctas = 2 * p.n_items < num_sms ? 2 * p.n_items : num_sms;
+  if (ctas <= 0) return cudaSuccess;
   cudaError_t e = cudaSuccess;
   switch (phase) {
     case 0:
@@ -909,7 +700,7 @@ cudaError_t launch_k1_gather_phase(int phase, const CUtensorMap& tmap, const CUt
       if (e != cudaSuccess) return e;
       e = cudaMemsetAsync(g.n_items, 0, sizeof(int32_t), stream);
       if (e != cudaSuccess) return e;
-      b2m_k1_filter_kernel<<<clusters * kCluster, kThreads, kSmemBytes, stream>>>(tmap, tmap, p);
+      b2m_k1_filter_kernel<<<ctas, kThreads, kSmemBytes, stream>>>(tmap, tmap, p);
       break;
     case 1:
       b2m_k1_resolve_kernel<<<n_pairs * kResolveParts, 256, 0, stream>>>(p, desc, 0);
@@ -927,7 +718,7 @@ cudaError_t launch_k1_gather_phase(int phase, const CUtensorMap& tmap, const CUt
       q.item_list = g.items;
       q.n_items_ptr = g.n_items;
       q.gath_cnt = g.cnt;
-      b2m_k1_filter_kernel<<<max_clusters * kCluster, kThreads, kSmemBytes, stream>>>(tmap, tmap_gath, q);
+      b2m_k1_filter_kernel<<<num_sms, kThreads, kSmemBytes, stream>>>(tmap, tmap_gath, q);
       break;
     }
     default:

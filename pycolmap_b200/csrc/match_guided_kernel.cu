@@ -1,4 +1,4 @@
-// match_guided_kernel.cu -- K1g: guided matching.  The tcgen05 int8 GEMM of K1 with an epilogue that
+// match_guided_kernel.cu -- K1g: guided matching.  The wgmma int8 GEMM of K1 with an epilogue that
 // first zeroes every dot product whose keypoint pair violates the two-view geometry of the image pair
 // (float32, as upstream) and then runs the exact running top-2 / ratio / distance logic.
 //
@@ -10,7 +10,8 @@
 // The float32 filter is written with non-fused single operations in the same order as the oracle
 // (oracle/oracle_match.c orc_match_guided, compiled with -ffp-contract=off) so that the match indices
 // are bit-identical.  Work unit = (pair, direction, 128-row strip); only pairs flagged by the decision
-// kernel do any work, so the simple non-persistent pipeline of match_kernel.cu is reused.
+// kernel do any work, so the simple non-persistent pipeline of match_kernel.cu is reused (in 128-column halves,
+// which leaves registers for the per-element test beside the accumulators).
 #include "match_kernel.cuh"
 #include "ptx.cuh"
 
@@ -19,25 +20,18 @@ namespace b2m {
 namespace {
 
 constexpr int kDim = 128;
-constexpr int kTileM = 128;
+constexpr int kTileM = 128;    // rows per CTA: two consumer warpgroups of 64 rows
 constexpr int kTileN = 256;
-constexpr int kUmmaK = 32;
-constexpr int kStages = 2;     // two CTAs per SM (85 KB shared memory, 256 of the 512 TMEM columns each): the epilogue -- ~50 ALU
-constexpr int kAccStages = 1;  // instructions per matrix element -- is the bound, so resident epilogue warps are what counts
+constexpr int kStages = 4;
 constexpr int kBytesA = kTileM * kDim;
 constexpr int kBytesB = kTileN * kDim;
-constexpr int kEpiWarps = 8;    // warp w: TMEM lane quarter w % 4 (32 rows), column half w / 4 (128 of the 256 columns of a tile)
-constexpr int kColGroups = kEpiWarps / 4;
-constexpr int kThreads = (kEpiWarps + 2) * 32;
-constexpr uint32_t kIdesc = make_idesc_u8u8_s32(kTileM, kTileN);
+constexpr int kConsumerWarps = 8;
+constexpr int kThreads = (kConsumerWarps + 1) * 32;   // + TMA producer warp
 
 struct __align__(8) Barriers {
   uint64_t full_a;
   uint64_t full_b[kStages];
   uint64_t empty_b[kStages];
-  uint64_t tmem_full[kAccStages];
-  uint64_t tmem_empty[kAccStages];
-  uint32_t tmem_base;
 };
 
 constexpr int kKpBytes = 2 * kTileN * 16;  // two buffers of 256 per-column float4 (the column's share of the residual)
@@ -95,128 +89,53 @@ __device__ __noinline__ bool sampson_sliver(float a, float den, float thr, doubl
   return lhs < rhs || (lhs == rhs && thr_even);
 }
 
-__device__ __forceinline__ float4 lds_f4(uint32_t addr) {   // shared-window load (the staging pointer is generic)
-  float4 r;
-  asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(r.x), "=f"(r.y), "=f"(r.z), "=f"(r.w) : "r"(addr));
-  return r;
-}
-
-// comparison -> 0xffffffff / 0 (ordered comparisons: false on NaN)
-__device__ __forceinline__ uint32_t set_lt(float a, float b) {
-  uint32_t m;
-  asm("set.lt.u32.f32 %0, %1, %2;" : "=r"(m) : "f"(a), "f"(b));
-  return m;
-}
-__device__ __forceinline__ uint32_t set_le(float a, float b) {
-  uint32_t m;
-  asm("set.le.u32.f32 %0, %1, %2;" : "=r"(m) : "f"(a), "f"(b));
-  return m;
-}
-__device__ __forceinline__ uint32_t set_gt(float a, float b) {
-  uint32_t m;
-  asm("set.gt.u32.f32 %0, %1, %2;" : "=r"(m) : "f"(a), "f"(b));
-  return m;
-}
-
-// One 32-column chunk of a row: mask the dot products by the geometric test, update the four running top-2 key pairs.
-// CB: first column of the chunk inside the warp's 128-column half of the tile -- a compile-time constant, so the
-// column byte of the key is an immediate.  Pipe balance (ncu r02: ALU pipe 70 % busy, FMA pipe 30 %): per element
-// 2 FSETP + SEL + PLOP3 + 3 VIMNMX on the ALU pipe, 5 FMUL + 4 FADD + 1 IMAD (key) on the FMA pipe.
-template <int MODE, int CB>
-__device__ __forceinline__ void scan_chunk(const uint32_t* v, uint32_t cols, const float4 r, float thr,
-                                           float thr_next, double thr_mid, bool thr_even, uint32_t* k1, uint32_t* k2) {
-  uint32_t undecided = 0;   // some element of the chunk needs the exact comparison: the chunk is revisited (rare)
-#pragma unroll
-  for (int j = 0; j < 32; ++j) {
-    const float4 c = lds_f4(cols + 16u * j);   // the same address for the whole warp: a broadcast
-    bool ok = false;
-    uint32_t d = 0;
-    float a = 0.f, den = 0.f;
-    if (MODE == 2) {
-      const float du = __fsub_rn(r.x, c.x), dv = __fsub_rn(r.y, c.y);
-      ok = __fadd_rn(__fmul_rn(du, du), __fmul_rn(dv, dv)) <= thr;
-    } else {
-      float num;
-      if (MODE == 0) {
-        num = __fadd_rn(__fadd_rn(__fmul_rn(c.x, r.x), __fmul_rn(c.y, r.y)), r.z);
-        den = __fadd_rn(__fadd_rn(r.w, c.z), c.w);
-      } else {
-        num = __fadd_rn(__fadd_rn(__fmul_rn(r.x, c.x), __fmul_rn(r.y, c.y)), c.z);
-        den = __fadd_rn(__fadd_rn(c.w, r.z), r.w);
-      }
-      a = __fmul_rn(num, num);
-      // ok = a < RD(den * thr); decided = ok | a > RU(den * thr_next) (ordered compares: a NaN stays undecided).
-      // One asm block so that each predicate is consumed where it is produced (left to itself the compiler parks the
-      // 32 `ok` flags of a chunk in a bit mask: two more ALU-pipe instructions per element).
-      asm("{\n\t.reg .pred p, q;\n\t"
-          "setp.lt.f32 p, %2, %3;\n\t"
-          "setp.gt.or.f32 q, %2, %4, p;\n\t"
-          "selp.u32 %0, %5, 0, p;\n\t"
-          "@!q or.b32 %1, %1, 1;\n\t}"
-          : "=r"(d), "+r"(undecided)
-          : "f"(a), "f"(__fmul_rd(den, thr)), "f"(__fmul_ru(den, thr_next)), "r"(v[j]));
-    }
-    if (MODE == 2) d = ok ? v[j] : 0u;
-    const uint32_t key = d * 256u + static_cast<uint32_t>(255 - (CB + j));
-    const uint32_t lo = min(k1[j & 3], key);
-    k1[j & 3] = max(k1[j & 3], key);
-    k2[j & 3] = max(k2[j & 3], lo);
-  }
-  if (MODE != 2 && undecided) {
-    // the masked key of an undecided element is already in (harmless: dot product 0); add the real one where the exact
-    // decision accepts.  The running top-2 is a multiset maximum: insertion order does not matter.
-#pragma unroll 1
-    for (int j = 0; j < 32; ++j) {
-      const float4 c = lds_f4(cols + 16u * j);
-      float num, den;
-      if (MODE == 0) {
-        num = __fadd_rn(__fadd_rn(__fmul_rn(c.x, r.x), __fmul_rn(c.y, r.y)), r.z);
-        den = __fadd_rn(__fadd_rn(r.w, c.z), c.w);
-      } else {
-        num = __fadd_rn(__fadd_rn(__fmul_rn(r.x, c.x), __fmul_rn(r.y, c.y)), c.z);
-        den = __fadd_rn(__fadd_rn(c.w, r.z), r.w);
-      }
-      const float a = __fmul_rn(num, num);
-      if (a < __fmul_rd(den, thr) || a > __fmul_ru(den, thr_next)) continue;   // decided in the sweep
-      if (!sampson_sliver(a, den, thr, thr_mid, thr_even)) continue;
-      uint32_t vj = 0;   // v[j] with a run-time j: a select chain instead of a local-memory array
-#pragma unroll
-      for (int q = 0; q < 32; ++q) vj = (q == j) ? v[q] : vj;
-      const uint32_t key = vj * 256u + static_cast<uint32_t>(255 - (CB + j));
-      const int a4 = j & 3;
-#pragma unroll
-      for (int q = 0; q < 4; ++q)
-        if (q == a4) {
-          const uint32_t lo = min(k1[q], key);
-          k1[q] = max(k1[q], key);
-          k2[q] = max(k2[q], lo);
-        }
-    }
-  }
-}
-
-// The warp's 128 columns of a tile: four 32-column TMEM loads, each swept against the staged column sides.
+// One 128-column half of a tile: mask the dot products of the thread's two rows by the geometric test and update
+// their tile-local top-2 keys.  Column 8 j + 2 q + e of the half is acc[4 j + 2 i + e] for row i; its side of the
+// residual is cols[8 j + 2 q + e].  An element whose Sampson test falls in the sliver between the two bounds takes the
+// exact decision at once (rare).
 template <int MODE>
-__device__ __forceinline__ void scan_half(uint32_t taddr, uint32_t cols, const float4 r, float thr, float thr_next,
-                                          double thr_mid, bool thr_even, uint32_t* k1, uint32_t* k2) {
-  uint32_t v[32];
-  tmem_ld_32x32(taddr, v);
-  tmem_wait_ld();
-  scan_chunk<MODE, 0>(v, cols, r, thr, thr_next, thr_mid, thr_even, k1, k2);
-  tmem_ld_32x32(taddr + 32, v);
-  tmem_wait_ld();
-  scan_chunk<MODE, 32>(v, cols + 32 * 16, r, thr, thr_next, thr_mid, thr_even, k1, k2);
-  tmem_ld_32x32(taddr + 64, v);
-  tmem_wait_ld();
-  scan_chunk<MODE, 64>(v, cols + 64 * 16, r, thr, thr_next, thr_mid, thr_even, k1, k2);
-  tmem_ld_32x32(taddr + 96, v);
-  tmem_wait_ld();
-  scan_chunk<MODE, 96>(v, cols + 96 * 16, r, thr, thr_next, thr_mid, thr_even, k1, k2);
+__device__ __forceinline__ void scan_half(const uint32_t (&acc)[64], const float4* cols, int q, int col0, const float4 (&r)[2],
+                                          float thr, float thr_next, double thr_mid, bool thr_even, uint32_t (&k1)[2],
+                                          uint32_t (&k2)[2]) {
+#pragma unroll
+  for (int j = 0; j < 16; ++j) {
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      const int col = 8 * j + 2 * q + e;
+      const float4 c = cols[col];
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        bool ok;
+        if (MODE == 2) {
+          const float du = __fsub_rn(r[i].x, c.x), dv = __fsub_rn(r[i].y, c.y);
+          ok = __fadd_rn(__fmul_rn(du, du), __fmul_rn(dv, dv)) <= thr;
+        } else {
+          float num, den;
+          if (MODE == 0) {
+            num = __fadd_rn(__fadd_rn(__fmul_rn(c.x, r[i].x), __fmul_rn(c.y, r[i].y)), r[i].z);
+            den = __fadd_rn(__fadd_rn(r[i].w, c.z), c.w);
+          } else {
+            num = __fadd_rn(__fadd_rn(__fmul_rn(r[i].x, c.x), __fmul_rn(r[i].y, c.y)), c.z);
+            den = __fadd_rn(__fadd_rn(c.w, r[i].z), r[i].w);
+          }
+          const float a = __fmul_rn(num, num);
+          // ok = a < RD(den * thr); decided = ok | a > RU(den * thr_next) (ordered compares: a NaN stays undecided)
+          ok = a < __fmul_rd(den, thr);
+          if (!ok && !(a > __fmul_ru(den, thr_next))) ok = sampson_sliver(a, den, thr, thr_mid, thr_even);
+        }
+        const uint32_t d = ok ? acc[4 * j + 2 * i + e] : 0u;
+        const uint32_t key = d * 256u + static_cast<uint32_t>(255 - (col0 + col));
+        const uint32_t lo = min(k1[i], key);
+        k1[i] = max(k1[i], key);
+        k2[i] = max(k2[i], lo);
+      }
+    }
+  }
 }
 
 }  // namespace
 
-__global__ void __launch_bounds__(kThreads, 2)  // 2 x 8 epilogue warps per SM
+__global__ void __launch_bounds__(kThreads, 1)
 b2m_k1_guided_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ CUtensorMap tmap_a, const MatchParams p,
                      const GuidedParams g) {
   const int pair = blockIdx.z;
@@ -246,30 +165,20 @@ b2m_k1_guided_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_cons
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
 
-  if (warp == kEpiWarps && lane == 0) {
+  if (warp == kConsumerWarps && lane == 0) {
     tma_prefetch_desc(&tmap);
     tma_prefetch_desc(&tmap_a);
     mbar_init(&bars->full_a, 1);
     for (int s = 0; s < kStages; ++s) {
       mbar_init(&bars->full_b[s], 1);
-      mbar_init(&bars->empty_b[s], 1);
-    }
-    for (int s = 0; s < kAccStages; ++s) {
-      mbar_init(&bars->tmem_full[s], 1);
-      mbar_init(&bars->tmem_empty[s], kEpiWarps * 32);
+      mbar_init(&bars->empty_b[s], kConsumerWarps);
     }
     fence_mbar_init();
   }
-  if (warp == kEpiWarps + 1) {
-    tmem_alloc(&bars->tmem_base, kAccStages * kTileN);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = bars->tmem_base;
 
-  if (warp == kEpiWarps) {
+  if (warp == kConsumerWarps) {
+    // ===== TMA producer =====
     if (lane == 0 && n_tiles > 0) {
       mbar_arrive_expect_tx(&bars->full_a, kBytesA);
       tma_load_2d(smA, &tmap_a, &bars->full_a, 0, rowA);
@@ -286,37 +195,11 @@ b2m_k1_guided_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_cons
         }
       }
     }
-  } else if (warp == kEpiWarps + 1) {
-    if (lane == 0 && n_tiles > 0) {
-      mbar_wait(&bars->full_a, 0);
-      const uint64_t adesc0 = make_smem_desc_sw128(smem_u32(smA));
-      uint32_t stage = 0, phase = 0, as = 0, aphase = 0;
-      for (int t = 0; t < n_tiles; ++t) {
-        mbar_wait(&bars->tmem_empty[as], aphase ^ 1);
-        mbar_wait(&bars->full_b[stage], phase);
-        tc_fence_after();
-        const uint64_t bdesc0 = make_smem_desc_sw128(smem_u32(smB + stage * kBytesB));
-        const uint32_t tmem_d = tmem_base + as * kTileN;
-#pragma unroll
-        for (int k = 0; k < kDim / kUmmaK; ++k)
-          mma_i8_ss(tmem_d, adesc0 + 2 * k, bdesc0 + 2 * k, kIdesc, k > 0 ? 1u : 0u);
-        mma_commit(&bars->empty_b[stage]);
-        mma_commit(&bars->tmem_full[as]);
-        if (++stage == kStages) {
-          stage = 0;
-          phase ^= 1;
-        }
-        if (++as == kAccStages) {
-          as = 0;
-          aphase ^= 1;
-        }
-      }
-    }
   } else {
-    // ===== epilogue: geometric mask, then exact running top-2 (thread <-> row) =====
-    const int quarter = warp & 3, group = warp >> 2;
-    const int row_in_strip = quarter * 32 + lane;
-    const int row = strip * kTileM + row_in_strip;
+    // ===== consumers: MMA, geometric mask, then exact running top-2 of the thread's two rows =====
+    const int wg = warp >> 2;
+    const int q = lane & 3;
+    const int row0 = strip * kTileM + wg * 64 + (warp & 3) * 16 + (lane >> 2);   // rows row0 and row0 + 8
     float M[9];
 #pragma unroll
     for (int k = 0; k < 9; ++k) M[k] = g.model[pair * 9 + k];
@@ -324,92 +207,80 @@ b2m_k1_guided_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_cons
     const float thr_next = __int_as_float(__float_as_int(thr) + 1);   // thr > 0: the next float above
     const double thr_mid = 0.5 * (static_cast<double>(thr) + static_cast<double>(thr_next));
     const bool thr_even = (__float_as_int(thr) & 1) == 0;
-    const float2 kr = (row < nA) ? g.kpts[p.img_row0[ia] + (gathered ? g.gath_cols[static_cast<int64_t>(pair) * p.mstride + row] : row)]
-                                 : make_float2(0.f, 0.f);
     const float2* kcol = g.kpts + p.img_row0[ib];
     // image 1 is pairs[2 * pair], image 2 is pairs[2 * pair + 1]: in direction 1 the rows are image 2
     const int mode = gkind == 0 ? dir : 2;
-    const float4 rc = (dir == 0) ? side_image1(gkind, M, kr.x, kr.y) : side_image2(gkind, M, kr.x, kr.y);
-    int32_t best_d = 0, best_c = -1, second_d = 0;
-    uint32_t as = 0, aphase = 0;
-    const uint32_t lane_base = (static_cast<uint32_t>(quarter * 32) << 16) + group * (kTileN / kColGroups);
+    float4 rc[2];
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const int row = row0 + 8 * i;
+      const float2 kr = (row < nA) ? g.kpts[p.img_row0[ia] + (gathered ? g.gath_cols[static_cast<int64_t>(pair) * p.mstride + row] : row)]
+                                   : make_float2(0.f, 0.f);
+      rc[i] = (dir == 0) ? side_image1(gkind, M, kr.x, kr.y) : side_image2(gkind, M, kr.x, kr.y);
+    }
+    int32_t best_d[2] = {0, 0}, best_c[2] = {-1, -1}, second_d[2] = {0, 0};
+    uint32_t acc[64];
+#pragma unroll
+    for (int i = 0; i < 64; ++i) acc[i] = 0u;
+    if (n_tiles > 0) mbar_wait(&bars->full_a, 0);
+    const uint32_t a_addr = smem_u32(smA + wg * 64 * kDim);
+    uint32_t stage = 0, phase = 0;
     for (int t = 0; t < n_tiles; ++t) {
       // stage the column side of this tile's 256 columns (one per thread), double-buffered by tile parity
       float4* kb = kp_s + (t & 1) * kTileN;
-      for (int c = threadIdx.x; c < kTileN; c += kEpiWarps * 32) {
+      for (int c = threadIdx.x; c < kTileN; c += kConsumerWarps * 32) {
         const int j = t * kTileN + c;
         const float2 kc = (j < nB) ? kcol[j] : make_float2(0.f, 0.f);
         kb[c] = (dir == 0) ? side_image2(gkind, M, kc.x, kc.y) : side_image1(gkind, M, kc.x, kc.y);
       }
-      asm volatile("bar.sync 1, %0;" ::"r"(kEpiWarps * 32) : "memory");
-      mbar_wait(&bars->tmem_full[as], aphase);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + lane_base + as * kTileN;
-      uint32_t k1[4] = {0, 0, 0, 0}, k2[4] = {0, 0, 0, 0};
-      const int col0 = group * (kTileN / kColGroups);   // this warp's columns of the tile
-      static_assert(kTileN / kColGroups == 128, "scan_half sweeps four chunks of 32 columns");
-      {
-        const uint32_t cols = smem_u32(kb + col0);
-        if (mode == 0) scan_half<0>(taddr, cols, rc, thr, thr_next, thr_mid, thr_even, k1, k2);
-        else if (mode == 1) scan_half<1>(taddr, cols, rc, thr, thr_next, thr_mid, thr_even, k1, k2);
-        else scan_half<2>(taddr, cols, rc, thr, thr_next, thr_mid, thr_even, k1, k2);
-      }
-      tc_fence_before();
-      mbar_arrive(&bars->tmem_empty[as]);
-      merge_top2(k1[0], k2[0], k1[1], k2[1]);
-      merge_top2(k1[2], k2[2], k1[3], k2[3]);
-      merge_top2(k1[0], k2[0], k1[2], k2[2]);
-      const int32_t d1 = static_cast<int32_t>(k1[0] >> 8);
-      const int32_t d2 = static_cast<int32_t>(k2[0] >> 8);
-      if (d1 > best_d) {
-        second_d = max(best_d, d2);
-        best_d = d1;
-        best_c = t * kTileN + col0 + (255 - static_cast<int32_t>(k1[0] & 255u));
-      } else {
-        second_d = max(second_d, d1);
-      }
-      if (++as == kAccStages) {
-        as = 0;
-        aphase ^= 1;
-      }
-    }
-    // merge the column halves of a row (group 1 -> shared memory -> group 0): the union's best is the larger dot
-    // product, the LOWER column on a tie; its second best = multiset second of the two (best, second) pairs
-    if (kColGroups > 1) {
-      int32_t* mg = reinterpret_cast<int32_t*>(kp_s);   // the keypoint staging buffer is free after the last tile
-      asm volatile("bar.sync 1, %0;" ::"r"(kEpiWarps * 32) : "memory");
-      if (group == 1) {
-        mg[row_in_strip * 3] = best_d;
-        mg[row_in_strip * 3 + 1] = second_d;
-        mg[row_in_strip * 3 + 2] = best_c;
-      }
-      asm volatile("bar.sync 1, %0;" ::"r"(kEpiWarps * 32) : "memory");
-      if (group == 0) {
-        const int32_t ob = mg[row_in_strip * 3], os = mg[row_in_strip * 3 + 1], oc = mg[row_in_strip * 3 + 2];
-        const int32_t ns = max(max(second_d, os), min(best_d, ob));
-        if (ob > best_d || (ob == best_d && oc >= 0 && (best_c < 0 || oc < best_c))) {
-          best_d = ob;
-          best_c = oc;
+      asm volatile("bar.sync 1, %0;" ::"r"(kConsumerWarps * 32) : "memory");
+      mbar_wait(&bars->full_b[stage], phase);
+      uint32_t k1[2] = {0, 0}, k2[2] = {0, 0};
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        wgmma_tile_u8(acc, a_addr, smem_u32(smB + stage * kBytesB + h * (kBytesB / 2)));
+        if (h == 1) {
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&bars->empty_b[stage]);   // the MMAs reading this stage have completed
         }
-        second_d = ns;
+        const float4* cols = kb + 128 * h;
+        if (mode == 0) scan_half<0>(acc, cols, q, 128 * h, rc, thr, thr_next, thr_mid, thr_even, k1, k2);
+        else if (mode == 1) scan_half<1>(acc, cols, q, 128 * h, rc, thr, thr_next, thr_mid, thr_even, k1, k2);
+        else scan_half<2>(acc, cols, q, 128 * h, rc, thr, thr_next, thr_mid, thr_even, k1, k2);
+      }
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        // the four lanes of a quad hold the four column residues of the same row (keys are unique inside a tile)
+#pragma unroll
+        for (int o = 1; o < 4; o <<= 1)
+          merge_top2(k1[i], k2[i], __shfl_xor_sync(0xffffffffu, k1[i], o), __shfl_xor_sync(0xffffffffu, k2[i], o));
+        const int32_t d1 = static_cast<int32_t>(k1[i] >> 8);
+        const int32_t d2 = static_cast<int32_t>(k2[i] >> 8);
+        if (d1 > best_d[i]) {
+          second_d[i] = max(best_d[i], d2);
+          best_d[i] = d1;
+          best_c[i] = t * kTileN + (255 - static_cast<int32_t>(k1[i] & 255u));
+        } else {
+          second_d[i] = max(second_d[i], d1);
+        }
+      }
+      if (++stage == kStages) {
+        stage = 0;
+        phase ^= 1;
       }
     }
-    int32_t out = -1;
-    if (best_d > 0) {
-      const float a = __ldg(p.acos_lut + min(best_d, 262144));
-      if (!(a > p.max_distance)) {
-        const float b = __ldg(p.acos_lut + min(second_d, 262144));
-        if (!(a >= __fmul_rn(p.max_ratio, b))) out = best_c;
+    if (q < 2) {  // lane q of the quad writes row row0 + 8 q
+      const int32_t bd = q ? best_d[1] : best_d[0], sd = q ? second_d[1] : second_d[0], bc = q ? best_c[1] : best_c[0];
+      int32_t out = -1;
+      if (bd > 0) {
+        const float a = __ldg(p.acos_lut + min(bd, 262144));
+        if (!(a > p.max_distance)) {
+          const float b = __ldg(p.acos_lut + min(sd, 262144));
+          if (!(a >= __fmul_rn(p.max_ratio, b))) out = bc;
+        }
       }
+      p.mbuf[(static_cast<int64_t>(pair) * 2 + dir) * p.mstride + row0 + 8 * q] = out;
     }
-    if (group == 0) p.mbuf[(static_cast<int64_t>(pair) * 2 + dir) * p.mstride + row] = out;
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == kEpiWarps + 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, kAccStages * kTileN);
   }
 }
 

@@ -1,5 +1,5 @@
-// match_kernel.cu -- K1: fused all-pairs uint8 descriptor GEMM (tcgen05.mma.kind::i8, TMA-staged
-// operands, accumulators in TMEM) + per-row top-2 / lowest-index arg-max / acos-LUT ratio &
+// match_kernel.cu -- K1: fused all-pairs uint8 descriptor GEMM (wgmma.mma_async u8, TMA-staged
+// operands, accumulators in registers) + per-row top-2 / lowest-index arg-max / acos-LUT ratio &
 // distance tests, and the cross-check + ordered compaction kernel.  The N x M distance matrix
 // never leaves the SM.
 //
@@ -14,24 +14,18 @@ namespace b2m {
 namespace {
 
 constexpr int kDim = 128;            // descriptor bytes == K of the GEMM
-constexpr int kTileM = 128;          // rows of A per CTA (TMEM lanes)
+constexpr int kTileM = 128;          // rows of A per CTA: two consumer warpgroups of 64 rows
 constexpr int kTileN = 256;          // columns of B per MMA tile
-constexpr int kUmmaK = 32;           // bytes of K per tcgen05.mma.kind::i8
 constexpr int kStages = 4;           // B-tile ring depth
-constexpr int kAccStages = 2;        // TMEM accumulator double buffer (2 x 256 columns = 512)
 constexpr int kBytesA = kTileM * kDim;        // 16 KiB
 constexpr int kBytesB = kTileN * kDim;        // 32 KiB
-constexpr int kEpiWarps = 4;
-constexpr int kThreads = (kEpiWarps + 2) * 32;  // 4 epilogue warps + TMA warp + MMA warp
-constexpr uint32_t kIdesc = make_idesc_u8u8_s32(kTileM, kTileN);
+constexpr int kConsumerWarps = 8;             // warpgroups 0 and 1: MMA + epilogue
+constexpr int kThreads = (kConsumerWarps + 1) * 32;  // + TMA producer warp
 
 struct __align__(8) Barriers {
   uint64_t full_a;
   uint64_t full_b[kStages];
   uint64_t empty_b[kStages];
-  uint64_t tmem_full[kAccStages];
-  uint64_t tmem_empty[kAccStages];
-  uint32_t tmem_base;
 };
 
 constexpr size_t kSmemBytes = 1024 /*align slack*/ + kBytesA + kStages * kBytesB + sizeof(Barriers);
@@ -54,7 +48,7 @@ b2m_k1_match_kernel(const __grid_constant__ CUtensorMap tmap, const MatchParams 
   const int ib = p.pairs[2 * pair + (dir ^ 1)];
   const int nA = p.img_nfeat[ia];
   const int nB = p.img_nfeat[ib];
-  if (strip * kTileM >= nA) return;  // uniform exit before any barrier / TMEM allocation
+  if (strip * kTileM >= nA) return;  // uniform exit before any barrier
   const int rowA = p.img_row0[ia] + strip * kTileM;
   const int rowB = p.img_row0[ib];
   const int n_tiles = (nB + kTileN - 1) / kTileN;
@@ -68,29 +62,18 @@ b2m_k1_match_kernel(const __grid_constant__ CUtensorMap tmap, const MatchParams 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
 
-  if (warp == kEpiWarps && lane == 0) {
+  if (warp == kConsumerWarps && lane == 0) {
     tma_prefetch_desc(&tmap);
     mbar_init(&bars->full_a, 1);
     for (int s = 0; s < kStages; ++s) {
       mbar_init(&bars->full_b[s], 1);
-      mbar_init(&bars->empty_b[s], 1);
-    }
-    for (int s = 0; s < kAccStages; ++s) {
-      mbar_init(&bars->tmem_full[s], 1);
-      mbar_init(&bars->tmem_empty[s], kEpiWarps * 32);
+      mbar_init(&bars->empty_b[s], kConsumerWarps);
     }
     fence_mbar_init();
   }
-  if (warp == kEpiWarps + 1) {
-    tmem_alloc(&bars->tmem_base, kAccStages * kTileN);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = bars->tmem_base;
 
-  if (warp == kEpiWarps) {
+  if (warp == kConsumerWarps) {
     // ===== TMA producer =====
     if (lane == 0 && n_tiles > 0) {
       mbar_arrive_expect_tx(&bars->full_a, kBytesA);
@@ -108,99 +91,76 @@ b2m_k1_match_kernel(const __grid_constant__ CUtensorMap tmap, const MatchParams 
         }
       }
     }
-  } else if (warp == kEpiWarps + 1) {
-    // ===== MMA issuer (one thread) =====
-    if (lane == 0 && n_tiles > 0) {
-      mbar_wait(&bars->full_a, 0);
-      const uint64_t adesc0 = make_smem_desc_sw128(smem_u32(smA));
-      uint32_t stage = 0, phase = 0, as = 0, aphase = 0;
-      for (int t = 0; t < n_tiles; ++t) {
-        mbar_wait(&bars->tmem_empty[as], aphase ^ 1);
-        mbar_wait(&bars->full_b[stage], phase);
-        tc_fence_after();
-        const uint64_t bdesc0 = make_smem_desc_sw128(smem_u32(smB + stage * kBytesB));
-        const uint32_t tmem_d = tmem_base + as * kTileN;
-#pragma unroll
-        for (int k = 0; k < kDim / kUmmaK; ++k) {
-          // +32 bytes of K inside the 128-B swizzle atom == +2 in the (addr >> 4) field
-          mma_i8_ss(tmem_d, adesc0 + 2 * k, bdesc0 + 2 * k, kIdesc, k > 0 ? 1u : 0u);
-        }
-        mma_commit(&bars->empty_b[stage]);  // smem stage reusable once these MMAs retire
-        mma_commit(&bars->tmem_full[as]);   // accumulator ready for the epilogue
-        if (++stage == kStages) {
-          stage = 0;
-          phase ^= 1;
-        }
-        if (++as == kAccStages) {
-          as = 0;
-          aphase ^= 1;
-        }
-      }
-    }
   } else {
-    // ===== epilogue: thread <-> row (TMEM lane); running top-2 over all column tiles =====
-    const int row_in_strip = warp * 32 + lane;
-    int32_t best_d = 0, best_c = -1, second_d = 0;
-    uint32_t as = 0, aphase = 0;
-    const uint32_t lane_base = static_cast<uint32_t>(warp * 32) << 16;
+    // ===== consumers: warpgroup wg multiplies rows 64 wg .. 64 wg + 63 with each 128-column half of every tile; each
+    // thread keeps the running top-2 of its two rows (16 w + l / 4 and + 8) over its 64 columns of the tile
+    const int wg = warp >> 2;
+    const int q = lane & 3;
+    const int row0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+    int32_t best_d[2] = {0, 0}, best_c[2] = {-1, -1}, second_d[2] = {0, 0};
+    uint32_t acc[64];   // one 128-column half of a tile at a time
+#pragma unroll
+    for (int i = 0; i < 64; ++i) acc[i] = 0u;
+    if (n_tiles > 0) mbar_wait(&bars->full_a, 0);
+    const uint32_t a_addr = smem_u32(smA + wg * 64 * kDim);
+    uint32_t stage = 0, phase = 0;
     for (int t = 0; t < n_tiles; ++t) {
-      mbar_wait(&bars->tmem_full[as], aphase);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + lane_base + as * kTileN;
-      uint32_t k1[4] = {0, 0, 0, 0}, k2[4] = {0, 0, 0, 0};
-      uint32_t va[32], vb[32];
-      tmem_ld_32x32(taddr, va);
+      mbar_wait(&bars->full_b[stage], phase);
+      uint32_t k1[2] = {0, 0}, k2[2] = {0, 0};
 #pragma unroll
-      for (int c = 0; c < kTileN / 32; ++c) {
-        tmem_wait_ld();
-        uint32_t(&cur)[32] = (c & 1) ? vb : va;
-        uint32_t(&nxt)[32] = (c & 1) ? va : vb;
-        if (c + 1 < kTileN / 32) tmem_ld_32x32(taddr + (c + 1) * 32, nxt);
+      for (int h = 0; h < 2; ++h) {
+        wgmma_tile_u8(acc, a_addr, smem_u32(smB + stage * kBytesB + h * (kBytesB / 2)));
+        if (h == 1) {
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&bars->empty_b[stage]);   // the MMAs reading this stage have completed
+        }
 #pragma unroll
-        for (int j = 0; j < 32; ++j) {
-          // key = dot * 256 + (255 - local column): max picks the largest dot, lowest column
-          const uint32_t key = (cur[j] << 8) | static_cast<uint32_t>(255 - (c * 32 + j));
-          const uint32_t lo = min(k1[j & 3], key);
-          k1[j & 3] = max(k1[j & 3], key);
-          k2[j & 3] = max(k2[j & 3], lo);
+        for (int i = 0; i < 2; ++i)
+#pragma unroll
+          for (int j = 0; j < 16; ++j)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              // key = dot * 256 + (255 - local column): max picks the largest dot, lowest column
+              const uint32_t key =
+                  (acc[4 * j + 2 * i + e] << 8) | static_cast<uint32_t>(255 - (128 * h + 8 * j + 2 * q + e));
+              const uint32_t lo = min(k1[i], key);
+              k1[i] = max(k1[i], key);
+              k2[i] = max(k2[i], lo);
+            }
+      }
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        // the four lanes of a quad hold the four column residues of the same row
+#pragma unroll
+        for (int o = 1; o < 4; o <<= 1)
+          merge_top2(k1[i], k2[i], __shfl_xor_sync(0xffffffffu, k1[i], o), __shfl_xor_sync(0xffffffffu, k2[i], o));
+        const int32_t d1 = static_cast<int32_t>(k1[i] >> 8);
+        const int32_t d2 = static_cast<int32_t>(k2[i] >> 8);
+        if (d1 > best_d[i]) {  // strict: an equal dot in a later tile never displaces an earlier column
+          second_d[i] = max(best_d[i], d2);
+          best_d[i] = d1;
+          best_c[i] = t * kTileN + (255 - static_cast<int32_t>(k1[i] & 255u));
+        } else {
+          second_d[i] = max(second_d[i], d1);
         }
       }
-      // all TMEM reads of this accumulator stage are complete -> hand it back to the MMA warp
-      tc_fence_before();
-      mbar_arrive(&bars->tmem_empty[as]);
-      merge_top2(k1[0], k2[0], k1[1], k2[1]);
-      merge_top2(k1[2], k2[2], k1[3], k2[3]);
-      merge_top2(k1[0], k2[0], k1[2], k2[2]);
-      const int32_t d1 = static_cast<int32_t>(k1[0] >> 8);
-      const int32_t d2 = static_cast<int32_t>(k2[0] >> 8);
-      if (d1 > best_d) {  // strict: an equal dot in a later tile never displaces an earlier column
-        second_d = max(best_d, d2);
-        best_d = d1;
-        best_c = t * kTileN + (255 - static_cast<int32_t>(k1[0] & 255u));
-      } else {
-        second_d = max(second_d, d1);
-      }
-      if (++as == kAccStages) {
-        as = 0;
-        aphase ^= 1;
+      if (++stage == kStages) {
+        stage = 0;
+        phase ^= 1;
       }
     }
-    int32_t out = -1;
-    if (best_d > 0) {
-      const float a = __ldg(p.acos_lut + min(best_d, 262144));
-      if (!(a > p.max_distance)) {
-        const float b = __ldg(p.acos_lut + min(second_d, 262144));
-        if (!(a >= __fmul_rn(p.max_ratio, b))) out = best_c;
+    if (q < 2) {  // lane q of the quad writes row q
+      const int32_t bd = q ? best_d[1] : best_d[0], sd = q ? second_d[1] : second_d[0], bc = q ? best_c[1] : best_c[0];
+      int32_t out = -1;
+      if (bd > 0) {
+        const float a = __ldg(p.acos_lut + min(bd, 262144));
+        if (!(a > p.max_distance)) {
+          const float b = __ldg(p.acos_lut + min(sd, 262144));
+          if (!(a >= __fmul_rn(p.max_ratio, b))) out = bc;
+        }
       }
+      p.mbuf[(static_cast<int64_t>(pair) * 2 + dir) * p.mstride + strip * kTileM + row0 + 8 * q] = out;
     }
-    p.mbuf[(static_cast<int64_t>(pair) * 2 + dir) * p.mstride + strip * kTileM + row_in_strip] = out;
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == kEpiWarps + 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, kAccStages * kTileN);
   }
 }
 

@@ -200,8 +200,6 @@ __device__ __forceinline__ void warp_score(const double* M, const double4* pts, 
   sum = warp_sum_d(s);
 }
 
-// (A variant of this sweep on packed fp32x2 registers -- FFMA2 / FMUL2, two matches per instruction -- measured no
-// faster on B200: H `score` 391 k vs 397 k Mcycles; the fp32 pipe, not instruction issue, is the limit.  Removed.)
 // Hypothesis scoring of one block of points: every thread keeps PPT matches (fp32) in registers and sweeps the
 // chunk's models: division-free fp32 test, fp64 only for the borderline points of a (thread, model).  Inlier counts
 // go to sh.chunk_cnt.
@@ -947,15 +945,15 @@ __global__ void __launch_bounds__(256) b2m_undistort_kernel(const VerifyParams P
   }
 }
 
-// B2M_E5_MINIMAL = thread | warp | hybrid: how the minimal 5-point solves of a RANSAC round are mapped (A/B switch; the
-// default is what measured fastest on B200, DESIGN.md section 4).
+// B2M_E5_MINIMAL = thread | warp | hybrid: how the minimal 5-point solves of a RANSAC round are mapped (A/B switch,
+// DESIGN.md section 4).
 int e5_minimal_mode() {
   static const int v = [] {
     const char* e = getenv("B2M_E5_MINIMAL");
     if (e && !strcmp(e, "warp")) return 1;
     if (e && !strcmp(e, "hybrid")) return 2;
     if (e && !strcmp(e, "thread")) return 0;
-    return 2;   // measured on B200 (1000 x 8192, B2M_PROF `solve` per two steps): thread 206-348 k, warp 651 k, hybrid 175 k Mcycles
+    return 2;
   }();
   return v;
 }
@@ -2018,7 +2016,7 @@ int b2m_estimate_two_view_geometry_batch(b2m_ctx* ctx, const b2m_tvg_problem* pr
   }
   cudaSetDevice(ctx->device);
   cudaStream_t st = ctx->stream;
-  constexpr int64_t kChunk = 4096;  // problems per launch: bounds the staging memory, plenty to fill 148 SMs
+  constexpr int64_t kChunk = 4096;  // problems per launch: bounds the staging memory, plenty to fill 132 SMs
   for (int64_t k0 = 0; k0 < n_problems; k0 += kChunk) {
     const int nb = static_cast<int>(std::min(kChunk, n_problems - k0));
     std::vector<double4> pts;

@@ -70,7 +70,7 @@ b2m_tvg_opts ToAbi(const TwoViewGeometryOptions& o) {
 b2m_camera ToAbi(const CameraRow& c) {
   if (b2m::cam::num_params(c.model) < 0)
     throw std::invalid_argument("[controllers.cc] camera model id " + std::to_string(c.model) +
-                                " is not supported by the B200 verifier (COLMAP 3.9.1 model ids 0-10)");
+                                " is not supported by the GPU verifier (COLMAP 3.9.1 model ids 0-10)");
   const size_t need = static_cast<size_t>(b2m::cam::num_params(c.model));
   if (c.params.size() != need)
     throw std::invalid_argument("[controllers.cc] Check Failed: camera has " + std::to_string(need) + " parameters");

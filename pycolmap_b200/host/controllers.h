@@ -89,7 +89,7 @@ b2m_tvg_opts ToAbi(const TwoViewGeometryOptions& o);
 b2m_camera ToAbi(const CameraRow& c);
 // SiftMatchingOptions.gpu_index: comma-separated CUDA ordinals, "0,1,2,3" = one matcher per listed GPU
 // (R:pipeline/match_features.h:76-81).  Duplicates are dropped, order kept.  "-1" (the default) expands to
-// every visible sm_100 device like upstream (b2m_device_count; device 0 when the count cannot be had).
+// every visible sm_90 device like upstream (b2m_device_count; device 0 when the count cannot be had).
 std::vector<int> ParseGpuIndices(const std::string& gpu_index);
 
 // ---- pair generators (rows P1, P2) -------------------------------------------------------------
