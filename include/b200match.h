@@ -26,7 +26,8 @@
 extern "C" {
 #endif
 
-#define B2M_ABI_VERSION 3   /* 2: b2m_camera carries 12 parameters, batch estimator; 3: multi-GPU entry points (NCCL) */
+#define B2M_ABI_VERSION 4   /* 2: b2m_camera carries 12 parameters, batch estimator; 3: multi-GPU entry points (NCCL);
+                             * 4: absolute pose estimation / refinement, b2m_stats.abs_pose_* */
 
 /* error codes */
 #define B2M_OK 0
@@ -315,6 +316,76 @@ int b2m_cam_from_img(b2m_ctx* ctx, const b2m_camera* camera, const double* point
 int b2m_squared_sampson_error(b2m_ctx* ctx, const double* points1, const double* points2, int64_t m,
                               const double* E, double* out_residuals);
 
+/* ---- absolute pose (callable without an image set) ----------------------------------- */
+
+/* AbsolutePoseEstimationOptions (R:pycolmap/estimators/absolute_pose.h:97-114; U:estimators/pose.h).  The defaults of
+ * b2m_abs_pose_opts_default are the C++ constructor's; pycolmap's Python-side defaults (estimate_focal_length = 0,
+ * ransac = RANSACOptions() with max_error 12) are set by the host module. */
+typedef struct b2m_abs_pose_opts {
+  uint32_t struct_size;
+  int32_t estimate_focal_length;    /* 0 */
+  int32_t num_focal_length_samples; /* 30 */
+  int32_t reserved;
+  double min_focal_length_ratio;    /* 0.2 */
+  double max_focal_length_ratio;    /* 5 */
+  b2m_ransac_opts ransac;           /* max_error in pixels */
+} b2m_abs_pose_opts;
+
+/* AbsolutePoseRefinementOptions (R:pycolmap/estimators/absolute_pose.h:116-131; U:estimators/pose.h). */
+typedef struct b2m_pose_refine_opts {
+  uint32_t struct_size;
+  int32_t max_num_iterations;       /* 100 */
+  double gradient_tolerance;        /* 1.0 */
+  double loss_function_scale;       /* 1.0 (CauchyLoss) */
+  int32_t refine_focal_length;      /* 1 */
+  int32_t refine_extra_params;      /* 1 */
+  int32_t print_summary;            /* 1; accepted and ignored (no solver log) */
+  int32_t reserved;
+} b2m_pose_refine_opts;
+
+void b2m_abs_pose_opts_default(b2m_abs_pose_opts* o);
+void b2m_pose_refine_opts_default(b2m_pose_refine_opts* o);
+
+/* One 2D-3D correspondence set: points2D[i] (pixels) observes points3D[i] (world). */
+typedef struct b2m_abs_pose_problem {
+  uint32_t struct_size;
+  int32_t reserved;
+  b2m_camera camera;
+  const double* points2D;  /* HOST [n x 2] float64 */
+  const double* points3D;  /* HOST [n x 3] float64 */
+  int64_t n;
+} b2m_abs_pose_problem;
+
+typedef struct b2m_abs_pose_result {
+  uint32_t struct_size;
+  int32_t success;          /* 0 mirrors the reference's `None` */
+  int64_t num_inliers;
+  double qvec[4];           /* cam_from_world rotation (w, x, y, z); identity on failure */
+  double tvec[3];           /* x_cam = R(qvec) x_world + tvec */
+  double params[B2M_CAMERA_MAX_PARAMS]; /* the camera's parameters after the call: focal scaled by the chosen factor when
+                                         * estimate_focal_length, refined ones after refinement; unchanged otherwise */
+  double covariance[36];    /* 6 x 6 row-major over (rotation tangent, translation) when requested */
+  int32_t focal_sample;     /* index of the chosen focal-length factor, -1 when no sample succeeded */
+  int32_t reserved;
+} b2m_abs_pose_result;
+
+/* Replaces EstimateAbsolutePose followed by RefineAbsolutePose (U:estimators/pose.cc), what
+ * pycolmap.absolute_pose_estimation runs per query (R:pycolmap/estimators/absolute_pose.h:18-63), over a batch of
+ * problems: one LO-RANSAC CTA per (problem, focal-length sample), then one warp per problem for the selection and the
+ * refinement.  refine == NULL: estimation only.  want_covariance: fill result.covariance (needs refine).
+ * inlier_masks: NULL, or [n_problems] HOST buffers of n_k bytes (NULL entries skip a problem).  Problem k is keyed by
+ * its position in the call, so problem 0 of any batch equals the single call bit for bit. */
+int b2m_estimate_absolute_pose_batch(b2m_ctx* ctx, const b2m_abs_pose_problem* problems, int64_t n_problems,
+                                     const b2m_abs_pose_opts* opts, const b2m_pose_refine_opts* refine,
+                                     int32_t want_covariance, b2m_abs_pose_result* out, uint8_t* const* inlier_masks);
+
+/* Replaces RefineAbsolutePose on caller-provided poses (pycolmap.pose_refinement,
+ * R:pycolmap/estimators/absolute_pose.h:65-94).  init_poses: [n_problems x 7] (qvec w, x, y, z, tvec);
+ * inlier_masks: [n_problems] HOST buffers of n_k bytes (nonzero = inlier). */
+int b2m_refine_absolute_pose_batch(b2m_ctx* ctx, const b2m_abs_pose_problem* problems, int64_t n_problems,
+                                   const double* init_poses, const uint8_t* const* inlier_masks,
+                                   const b2m_pose_refine_opts* refine, int32_t want_covariance, b2m_abs_pose_result* out);
+
 /* ---- instrumentation ---------------------------------------------------------------- */
 
 /* The cross-check consults m21 only at the columns some row matched (m21[m12[i]]): the column-direction GEMM is run
@@ -357,6 +428,8 @@ typedef struct b2m_stats {
   uint64_t verify_models_scored[3];   /* E / F / H: hypotheses + LO candidates scored against all matches since reset */
   uint64_t verify_residuals[3];       /* E / F / H: residual evaluations (models scored x matches of the pair) since reset */
   int32_t comm_size, comm_rank;       /* 1, 0 without a communicator */
+  uint64_t abs_pose_models_scored;    /* absolute pose: P3P / EPnP models scored against all correspondences since reset */
+  uint64_t abs_pose_residuals;        /* absolute pose: residual evaluations (models scored x correspondences) */
 } b2m_stats;
 int b2m_get_stats(b2m_ctx* ctx, b2m_stats* out);
 int b2m_reset_stats(b2m_ctx* ctx);

@@ -14,6 +14,8 @@ point fails with B2M_ENODEV without an sm_90 device.
 """
 try:
     from ._core import *  # noqa: F401,F403
+    from ._core import (AbsolutePoseEstimationOptions, AbsolutePoseRefinementOptions,  # noqa: F401
+                        absolute_pose_estimation, estimate_absolute_poses, pose_refinement)
     from ._core import (Context, Database, DatabaseTransaction, Device, ExhaustiveMatchingOptions,  # noqa: F401
                         RANSACOptions, Results, Rigid3d, Rotation3d, SequentialMatchingOptions,
                         SiftMatchingOptions, SpatialMatchingOptions, TwoViewGeometry,

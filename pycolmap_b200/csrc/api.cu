@@ -853,6 +853,7 @@ void b2m_destroy(b2m_ctx* ctx) {
   cudaDeviceSynchronize();
   comm_release(ctx);
   if (ctx->d_verify_counters) cudaFree(ctx->d_verify_counters);
+  if (ctx->d_abs_counters) cudaFree(ctx->d_abs_counters);
   ctx->images.release();
   ctx->ws.release();
   verify_release(ctx);
@@ -1155,6 +1156,14 @@ int b2m_get_stats(b2m_ctx* ctx, b2m_stats* out) {
         out->verify_residuals[k] = h[3 + k];
       }
   }
+  if (ctx->d_abs_counters) {  // same for the absolute pose estimator
+    unsigned long long h[2] = {0, 0};
+    cudaSetDevice(ctx->device);
+    if (cudaMemcpy(h, ctx->d_abs_counters, sizeof(h), cudaMemcpyDeviceToHost) == cudaSuccess) {
+      out->abs_pose_models_scored = h[0];
+      out->abs_pose_residuals = h[1];
+    }
+  }
   return B2M_OK;
 }
 int b2m_reset_stats(b2m_ctx* ctx) {
@@ -1164,6 +1173,10 @@ int b2m_reset_stats(b2m_ctx* ctx) {
   if (ctx->d_verify_counters) {
     cudaSetDevice(ctx->device);
     cudaMemset(ctx->d_verify_counters, 0, sizeof(unsigned long long) * 6);
+  }
+  if (ctx->d_abs_counters) {
+    cudaSetDevice(ctx->device);
+    cudaMemset(ctx->d_abs_counters, 0, sizeof(unsigned long long) * 2);
   }
   ctx->stats.k1_dir1_mode = static_cast<uint64_t>(ctx->k1_dir1_mode);  // a property of the context, not a counter
   return B2M_OK;

@@ -63,8 +63,11 @@ B2M_CAM_HD bool single_focal(int model) {
 }
 B2M_CAM_HD bool has_distortion(int model) { return model != kSimplePinhole && model != kPinhole; }
 
-// fx, fy, cx, cy and the index of the first distortion parameter
-B2M_CAM_HD void intrinsics(int model, const double* p, double* fx, double* fy, double* cx, double* cy, int* extra) {
+// fx, fy, cx, cy and the index of the first distortion parameter.  The functions that take a scalar type T are
+// templates so that the pose refinement can run them on forward-mode dual numbers (abs_pose.cu); with T = double
+// they are the plain functions.
+template <class T>
+B2M_CAM_HD void intrinsics(int model, const T* p, T* fx, T* fy, T* cx, T* cy, int* extra) {
   if (single_focal(model)) {
     *fx = *fy = p[0]; *cx = p[1]; *cy = p[2]; *extra = 3;
   } else {
@@ -76,28 +79,29 @@ B2M_CAM_HD void intrinsics(int model, const double* p, double* fx, double* fy, d
 B2M_CAM_HD double mean_focal_length(int model, const double* p) { return single_focal(model) ? p[0] : 0.5 * (p[0] + p[1]); }
 
 // d(u, v) of the model; k = pointer to the first distortion parameter
-B2M_CAM_HD void distortion(int model, const double* k, double u, double v, double* du, double* dv) {
-  const double u2 = u * u, v2 = v * v, r2 = u2 + v2;
+template <class T>
+B2M_CAM_HD void distortion(int model, const T* k, T u, T v, T* du, T* dv) {
+  const T u2 = u * u, v2 = v * v, r2 = u2 + v2;
   switch (model) {
     case kSimpleRadial: {
-      const double radial = k[0] * r2;
+      const T radial = k[0] * r2;
       *du = u * radial; *dv = v * radial;
       return;
     }
     case kRadial: {
-      const double radial = k[0] * r2 + k[1] * r2 * r2;
+      const T radial = k[0] * r2 + k[1] * r2 * r2;
       *du = u * radial; *dv = v * radial;
       return;
     }
     case kOpenCV: {
-      const double uv = u * v, radial = k[0] * r2 + k[1] * r2 * r2;
+      const T uv = u * v, radial = k[0] * r2 + k[1] * r2 * r2;
       *du = u * radial + 2.0 * k[2] * uv + k[3] * (r2 + 2.0 * u2);
       *dv = v * radial + 2.0 * k[3] * uv + k[2] * (r2 + 2.0 * v2);
       return;
     }
     case kFullOpenCV: {  // k1, k2, p1, p2, k3, k4, k5, k6
-      const double uv = u * v, r4 = r2 * r2, r6 = r4 * r2;
-      const double radial = (1.0 + k[0] * r2 + k[1] * r4 + k[4] * r6) / (1.0 + k[5] * r2 + k[6] * r4 + k[7] * r6);
+      const T uv = u * v, r4 = r2 * r2, r6 = r4 * r2;
+      const T radial = (1.0 + k[0] * r2 + k[1] * r4 + k[4] * r6) / (1.0 + k[5] * r2 + k[6] * r4 + k[7] * r6);
       *du = u * radial + 2.0 * k[2] * uv + k[3] * (r2 + 2.0 * u2) - u;
       *dv = v * radial + 2.0 * k[3] * uv + k[2] * (r2 + 2.0 * v2) - v;
       return;
@@ -105,39 +109,40 @@ B2M_CAM_HD void distortion(int model, const double* k, double u, double v, doubl
     case kOpenCVFisheye:
     case kSimpleRadialFisheye:
     case kRadialFisheye: {
-      const double r = sqrt(r2);
+      const T r = sqrt(r2);
       if (r > 2.220446049250313e-16) {  // std::numeric_limits<double>::epsilon()
-        const double theta = atan(r), t2 = theta * theta, t4 = t2 * t2;
-        double poly;
+        const T theta = atan(r), t2 = theta * theta, t4 = t2 * t2;
+        T poly;
         if (model == kOpenCVFisheye) poly = 1.0 + k[0] * t2 + k[1] * t4 + k[2] * t4 * t2 + k[3] * t4 * t4;
         else if (model == kRadialFisheye) poly = 1.0 + k[0] * t2 + k[1] * t4;
         else poly = 1.0 + k[0] * t2;
-        const double thetad = theta * poly;
+        const T thetad = theta * poly;
         *du = u * thetad / r - u;
         *dv = v * thetad / r - v;
       } else {
-        *du = 0.0; *dv = 0.0;
+        *du = T(0.0); *dv = T(0.0);
       }
       return;
     }
     case kThinPrismFisheye: {  // on the equidistant fisheye coordinates: k1, k2, p1, p2, k3, k4, sx1, sy1
-      const double uv = u * v, r4 = r2 * r2, r6 = r4 * r2, r8 = r6 * r2;
-      const double radial = k[0] * r2 + k[1] * r4 + k[4] * r6 + k[5] * r8;
+      const T uv = u * v, r4 = r2 * r2, r6 = r4 * r2, r8 = r6 * r2;
+      const T radial = k[0] * r2 + k[1] * r4 + k[4] * r6 + k[5] * r8;
       *du = u * radial + 2.0 * k[2] * uv + k[3] * (r2 + 2.0 * u2) + k[6] * r2;
       *dv = v * radial + 2.0 * k[3] * uv + k[2] * (r2 + 2.0 * v2) + k[7] * r2;
       return;
     }
     default:
-      *du = 0.0; *dv = 0.0;
+      *du = T(0.0); *dv = T(0.0);
   }
 }
 
 // FOV model: distorted = factor * undistorted with factor = atan(2 r tan(w/2)) / (r w) (-> 2 tan(w/2) / w as r -> 0,
 // -> 1 as w -> 0), and its closed-form inverse factor = tan(r_d w) / (2 r_d tan(w/2)).
-B2M_CAM_HD double fov_distort_factor(double omega, double r2) {
-  const double t = tan(0.5 * omega);
-  if (fabs(omega) < 1e-8) return 1.0;
-  const double x = 2.0 * sqrt(r2) * t;
+template <class T>
+B2M_CAM_HD T fov_distort_factor(T omega, T r2) {
+  const T t = tan(0.5 * omega);
+  if (fabs(omega) < 1e-8) return T(1.0);
+  const T x = 2.0 * sqrt(r2) * t;
   if (fabs(x) < 1e-6) return (2.0 * t / omega) * (1.0 - x * x / 3.0);
   return atan(x) / (sqrt(r2) * omega);
 }
@@ -200,18 +205,19 @@ B2M_CAM_HD void cam_from_img(int model, const double* p, double x, double y, dou
 }
 
 // Camera::ImgFromCam on normalised coordinates (used by the tests for round trips and to build scenes)
-B2M_CAM_HD void img_from_cam(int model, const double* p, double u, double v, double* x, double* y) {
-  double fx, fy, cx, cy, du = 0.0, dv = 0.0;
+template <class T>
+B2M_CAM_HD void img_from_cam(int model, const T* p, T u, T v, T* x, T* y) {
+  T fx, fy, cx, cy, du = T(0.0), dv = T(0.0);
   int extra;
   intrinsics(model, p, &fx, &fy, &cx, &cy, &extra);
   if (model == kFOV) {
-    const double f = fov_distort_factor(p[extra], u * u + v * v);
+    const T f = fov_distort_factor(p[extra], u * u + v * v);
     u *= f;
     v *= f;
   } else if (model == kThinPrismFisheye) {
-    const double r = sqrt(u * u + v * v);
+    const T r = sqrt(u * u + v * v);
     if (r > 2.220446049250313e-16) {
-      const double theta = atan(r);
+      const T theta = atan(r);
       u = theta * u / r;
       v = theta * v / r;
     }

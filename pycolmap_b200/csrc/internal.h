@@ -120,6 +120,7 @@ struct b2m_ctx {
   void* comm = nullptr;          // ncclComm_t
   int comm_size = 1, comm_rank = 0;
   unsigned long long* d_verify_counters = nullptr;  // [6]: models scored / residual evaluations per kind (verify.cu)
+  unsigned long long* d_abs_counters = nullptr;     // [2]: models scored / residual evaluations (abs_pose.cu)
 };
 
 namespace b2m {

@@ -24,6 +24,7 @@
 #include "eig_warp.cuh"
 #include "five_point_warp.cuh"
 #include "pose.h"
+#include "ransac_common.cuh"
 #include "verify.cuh"
 
 namespace b2m {
@@ -81,19 +82,6 @@ struct VerifyParams {
   int32_t guided_min_inliers; // < 0: guided matching off
 };
 
-__device__ __forceinline__ uint64_t splitmix64(uint64_t x) {
-  x += 0x9E3779B97F4A7C15ull;
-  x = (x ^ (x >> 30)) * 0xBF58476D1CE4E5B9ull;
-  x = (x ^ (x >> 27)) * 0x94D049BB133111EBull;
-  return x ^ (x >> 31);
-}
-
-__device__ __forceinline__ double shfl_d(double v, int src) { return __shfl_sync(0xffffffffu, v, src); }
-__device__ __forceinline__ double warp_sum_d(double v) {
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-
 // residual of point i under `model` for problem kind (0 = E on normalised coordinates)
 struct PointXform {
   double ax1, bx1, ay1, by1, ax2, bx2, ay2, by2;  // n = a * p + b  (identity for F / H)
@@ -135,11 +123,7 @@ __device__ __forceinline__ int inlier_f32(const float* M, float x1, float y1, fl
     lhs = num * num;
     rhs = thr * fmaf(a0, a0, fmaf(a1, a1, fmaf(b0, b0, b1 * b1)));
   }
-  // STRICT comparisons: lhs == rhs == 0 (both underflowed) or == inf (both overflowed) is neither clearly in nor
-  // clearly out, like any NaN -> borderline -> decided in fp64
-  const int in = lhs < 0.99f * rhs ? 1 : 0;
-  const int out = lhs > 1.01f * rhs ? 1 : 0;
-  return in | ((in | out) ^ 1) << 1;  // bit 0: inlier, bit 1: borderline (neither clearly in nor out)
+  return classify_f32(lhs, rhs);
 }
 
 template <int KIND>

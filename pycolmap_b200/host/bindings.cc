@@ -9,12 +9,15 @@
 //   essential / fundamental / homography_matrix_estimation    R:estimators/essential_matrix.h:19-103,
 //                                                             fundamental_matrix.h:17-50, homography_matrix.h:17-48
 //   RANSACOptions                                             R:optim/bindings.h:7-27
+//   absolute_pose_estimation, pose_refinement, AbsolutePose*Options  R:pycolmap/estimators/absolute_pose.h:18-166
 //   Device, has_cuda                                          R:utils.h:9-31, R:main.cc:98-106
 //   Database (open/close/counters/read_two_view_geometry/image_pair_to_pair_id)  R:scene/database.h:10-47
 // Everything below the option structs goes through the C ABI of include/b200match.h; there is no CPU path.
 #include <pybind11/numpy.h>
 #include <pybind11/pybind11.h>
 #include <pybind11/stl.h>
+
+#include <dlfcn.h>
 
 #include <array>
 #include <atomic>
@@ -301,6 +304,117 @@ std::vector<b2m_camera> CamerasFromPython(const py::object& cams) {
   std::vector<b2m_camera> out;
   for (const auto& c : cams) out.push_back(CameraFromPython(py::reinterpret_borrow<py::object>(c)));
   return out;
+}
+
+
+// ---- absolute pose (R:pycolmap/estimators/absolute_pose.h:18-166) ------------------------------------------
+void CheckAbsPoints(const ArrD& p2, const ArrD& p3) {
+  if (p2.ndim() != 2 || p2.shape(1) != 2)
+    throw std::invalid_argument("[bindings.cc] Check Failed: points2D is an N x 2 array");
+  if (p3.ndim() != 2 || p3.shape(1) != 3)
+    throw std::invalid_argument("[bindings.cc] Check Failed: points3D is an N x 3 array");
+  if (p2.shape(0) != p3.shape(0))  // THROW_CHECK_EQ(points2D.size(), points3D.size()), R:absolute_pose.h:26
+    throw std::invalid_argument("[absolute_pose.h:26] Check Failed: points2D.size() == points3D.size() (" +
+                                std::to_string(p2.shape(0)) + " vs. " + std::to_string(p3.shape(0)) + ")");
+}
+
+b2m_abs_pose_problem AbsProblem(const b2m_camera& cam, const ArrD& p2, const ArrD& p3) {
+  b2m_abs_pose_problem q;
+  memset(&q, 0, sizeof(q));
+  q.struct_size = sizeof(q);
+  q.camera = cam;
+  q.points2D = p2.data();
+  q.points3D = p3.data();
+  q.n = p2.shape(0);
+  return q;
+}
+
+// The reference takes Camera& and lets the estimator / the solver change its parameters: write them back into the
+// caller's object (the "params" key of a dict, else the `params` attribute).
+void WriteCameraParams(const py::object& camera, const b2m_abs_pose_result& r, int model) {
+  std::vector<double> p(r.params, r.params + b2m::cam::num_params(model));
+  if (py::isinstance<py::dict>(camera)) {
+    py::dict d = camera;
+    d["params"] = p;
+  } else {
+    py::setattr(camera, "params", py::array_t<double>(static_cast<py::ssize_t>(p.size()), p.data()));
+  }
+}
+
+py::object PoseToPython(const py::module_& m, const double* q, const double* t) {
+  const std::array<double, 4> xyzw{q[1], q[2], q[3], q[0]};
+  const std::array<double, 3> tr{t[0], t[1], t[2]};
+  return m.attr("Rigid3d")(m.attr("Rotation3d")(xyzw), tr);
+}
+
+// The absolute pose entry points (C ABI version 4) are bound at run time, like SQLite (sqlite_dyn.cc) and NCCL
+// (csrc/comm.cu): the host module references no version-4 symbol at link time, so it still loads against a
+// libb200match.so that predates them (the matching and verification surface keeps working) and reports their
+// absence when an absolute pose function is called.  There is no other path to these computations.
+struct AbsPoseApi {
+  decltype(&b2m_estimate_absolute_pose_batch) estimate = nullptr;
+  decltype(&b2m_refine_absolute_pose_batch) refine = nullptr;
+};
+const AbsPoseApi& AbsPose() {
+  static const AbsPoseApi api = [] {
+    AbsPoseApi a;
+    Dl_info info;   // the libb200match.so this module is linked against, found through one of its symbols
+    if (dladdr(reinterpret_cast<void*>(&b2m_abi_version), &info) && info.dli_fname)
+      if (void* h = dlopen(info.dli_fname, RTLD_NOW | RTLD_NOLOAD)) {
+        a.estimate = reinterpret_cast<decltype(a.estimate)>(dlsym(h, "b2m_estimate_absolute_pose_batch"));
+        a.refine = reinterpret_cast<decltype(a.refine)>(dlsym(h, "b2m_refine_absolute_pose_batch"));
+      }
+    return a;
+  }();
+  if (!api.estimate || !api.refine)
+    throw std::runtime_error("[bindings.cc] libb200match.so does not export the absolute pose entry points "
+                             "(C ABI version 4): rebuild it");
+  return api;
+}
+
+py::array_t<bool> MaskToNumpy(const std::vector<uint8_t>& mask, int64_t n) {
+  py::array_t<bool> a(static_cast<py::ssize_t>(n));
+  bool* p = a.mutable_data();
+  for (int64_t i = 0; i < n; ++i) p[i] = mask[i] != 0;
+  return a;
+}
+
+// Batched estimation + refinement; results in r, masks in masks.
+void EstimateAbsolutePoses(b2m_ctx* ctx, const std::vector<b2m_abs_pose_problem>& q, const AbsolutePoseEstimationOptions& eo,
+                           const AbsolutePoseRefinementOptions& ro, bool cov, std::vector<b2m_abs_pose_result>* r,
+                           std::vector<std::vector<uint8_t>>* masks) {
+  const b2m_abs_pose_opts e = ToAbi(eo);
+  const b2m_pose_refine_opts f = ToAbi(ro);
+  const AbsPoseApi& api = AbsPose();
+  const size_t n = q.size();
+  r->assign(n, b2m_abs_pose_result{});
+  masks->resize(n);
+  std::vector<uint8_t*> mp(n);
+  for (size_t k = 0; k < n; ++k) {
+    (*masks)[k].assign(static_cast<size_t>(std::max<int64_t>(q[k].n, 1)), 0);
+    mp[k] = (*masks)[k].data();
+  }
+  int rc;
+  {
+    py::gil_scoped_release release;
+    rc = api.estimate(ctx, q.data(), static_cast<int64_t>(n), &e, &f, cov ? 1 : 0, r->data(), mp.data());
+  }
+  ThrowOnError(ctx, rc);
+}
+
+py::object AbsResultToPython(const py::module_& m, const b2m_abs_pose_result& r, const std::vector<uint8_t>& mask, int64_t n,
+                             bool cov) {
+  if (!r.success) return py::none();
+  py::dict d;
+  d["cam_from_world"] = PoseToPython(m, r.qvec, r.tvec);
+  d["num_inliers"] = r.num_inliers;
+  d["inliers"] = MaskToNumpy(mask, n);
+  if (cov) {
+    py::array_t<double> c(std::vector<py::ssize_t>{6, 6});
+    memcpy(c.mutable_data(), r.covariance, sizeof(double) * 36);
+    d["covariance"] = c;
+  }
+  return d;
 }
 
 }  // namespace
@@ -651,6 +765,114 @@ PYBIND11_MODULE(_core, m) {
         },
         "camera1"_a, "points1"_a, "camera2"_a, "points2"_a, "geometry"_a,
         "Relative pose of an estimated geometry, in place (R:estimators/two_view_geometry.h:153-158).");
+  // ---- absolute pose ----
+  OptionsClass<AbsolutePoseEstimationOptions>(m, "AbsolutePoseEstimationOptions")
+      .field("estimate_focal_length", &AbsolutePoseEstimationOptions::estimate_focal_length)
+      .field("num_focal_length_samples", &AbsolutePoseEstimationOptions::num_focal_length_samples)
+      .field("min_focal_length_ratio", &AbsolutePoseEstimationOptions::min_focal_length_ratio)
+      .field("max_focal_length_ratio", &AbsolutePoseEstimationOptions::max_focal_length_ratio)
+      .field("ransac", &AbsolutePoseEstimationOptions::ransac)
+      .Finish();
+  OptionsClass<AbsolutePoseRefinementOptions>(m, "AbsolutePoseRefinementOptions")
+      .field("gradient_tolerance", &AbsolutePoseRefinementOptions::gradient_tolerance)
+      .field("max_num_iterations", &AbsolutePoseRefinementOptions::max_num_iterations)
+      .field("loss_function_scale", &AbsolutePoseRefinementOptions::loss_function_scale)
+      .field("refine_focal_length", &AbsolutePoseRefinementOptions::refine_focal_length)
+      .field("refine_extra_params", &AbsolutePoseRefinementOptions::refine_extra_params)
+      .field("print_summary", &AbsolutePoseRefinementOptions::print_summary)
+      .Finish();
+  m.def("absolute_pose_estimation",
+        [m](const ArrD& points2D, const ArrD& points3D, const py::object& camera,
+            const AbsolutePoseEstimationOptions& estimation_options, const AbsolutePoseRefinementOptions& refinement_options,
+            bool return_covariance) {
+          CheckAbsPoints(points2D, points3D);
+          const b2m_camera c = CameraFromPython(camera);
+          std::vector<b2m_abs_pose_problem> q{AbsProblem(c, points2D, points3D)};
+          std::vector<b2m_abs_pose_result> r;
+          std::vector<std::vector<uint8_t>> masks;
+          EstimateAbsolutePoses(Engine::Get(0), q, estimation_options, refinement_options, return_covariance, &r, &masks);
+          // the camera changes when the estimator scaled its focal length (EstimateAbsolutePose found inliers) or when
+          // RefineAbsolutePose, which runs after every such estimate, refined camera parameters
+          const bool estimated = r[0].focal_sample >= 0;
+          const bool refines = refinement_options.refine_focal_length || refinement_options.refine_extra_params;
+          if (estimated && (estimation_options.estimate_focal_length || refines))
+            WriteCameraParams(camera, r[0], c.model);
+          return AbsResultToPython(m, r[0], masks[0], q[0].n, return_covariance);
+        },
+        "points2D"_a, "points3D"_a, "camera"_a, "estimation_options"_a = AbsolutePoseEstimationOptions(),
+        "refinement_options"_a = AbsolutePoseRefinementOptions(), "return_covariance"_a = false,
+        "Absolute pose estimation with non-linear refinement.");
+  m.def("estimate_absolute_poses",
+        [m](const py::list& problems, const AbsolutePoseEstimationOptions& estimation_options,
+            const AbsolutePoseRefinementOptions& refinement_options, bool return_covariance) {
+          // Batched absolute_pose_estimation: problems = [(camera, points2D, points3D), ...], one GPU launch for all.
+          // Cameras are not modified; a successful result carries "camera_params" (the parameters after the call).
+          const size_t n = problems.size();
+          std::vector<ArrD> p2(n), p3(n);
+          std::vector<b2m_abs_pose_problem> q(n);
+          for (size_t k = 0; k < n; ++k) {
+            const py::tuple t = py::tuple(problems[k]);
+            if (t.size() != 3) throw std::invalid_argument("[bindings.cc] Check Failed: problem = (camera, points2D, points3D)");
+            p2[k] = ArrD::ensure(t[1]);
+            p3[k] = ArrD::ensure(t[2]);
+            if (!p2[k] || !p3[k]) throw std::invalid_argument("[bindings.cc] Check Failed: points are float64 arrays");
+            CheckAbsPoints(p2[k], p3[k]);
+            q[k] = AbsProblem(CameraFromPython(py::reinterpret_borrow<py::object>(t[0])), p2[k], p3[k]);
+          }
+          std::vector<b2m_abs_pose_result> r;
+          std::vector<std::vector<uint8_t>> masks;
+          EstimateAbsolutePoses(Engine::Get(0), q, estimation_options, refinement_options, return_covariance, &r, &masks);
+          py::list out;
+          for (size_t k = 0; k < n; ++k) {
+            py::object o = AbsResultToPython(m, r[k], masks[k], q[k].n, return_covariance);
+            if (!o.is_none()) {
+              const int np = b2m::cam::num_params(q[k].camera.model);
+              o.attr("__setitem__")("camera_params", py::array_t<double>(np, r[k].params));
+            }
+            out.append(o);
+          }
+          return out;
+        },
+        "problems"_a, "estimation_options"_a = AbsolutePoseEstimationOptions(),
+        "refinement_options"_a = AbsolutePoseRefinementOptions(), "return_covariance"_a = false,
+        "Batched absolute_pose_estimation: problems = [(camera, points2D, points3D), ...]");
+  m.def("pose_refinement",
+        [m](const py::object& cam_from_world, const ArrD& points2D, const ArrD& points3D, const py::object& inlier_mask,
+            const py::object& camera, const AbsolutePoseRefinementOptions& refinement_options) {
+          CheckAbsPoints(points2D, points3D);
+          const py::array_t<bool, py::array::c_style | py::array::forcecast> mask =
+              py::array_t<bool, py::array::c_style | py::array::forcecast>::ensure(inlier_mask);
+          if (!mask || mask.ndim() != 1 || mask.shape(0) != points2D.shape(0))  // R:absolute_pose.h:75
+            throw std::invalid_argument("[absolute_pose.h:75] Check Failed: inlier_mask.size() == points2D.size()");
+          const b2m_camera c = CameraFromPython(camera);
+          const py::array_t<double> quat = py::array_t<double>::ensure(cam_from_world.attr("rotation").attr("quat"));
+          const py::array_t<double> tr = py::array_t<double>::ensure(cam_from_world.attr("translation"));
+          if (!quat || quat.size() != 4 || !tr || tr.size() != 3)
+            throw std::invalid_argument("[bindings.cc] Check Failed: cam_from_world is a Rigid3d");
+          const double init[7] = {quat.data()[3], quat.data()[0], quat.data()[1], quat.data()[2], tr.data()[0], tr.data()[1],
+                                  tr.data()[2]};
+          std::vector<uint8_t> m8(static_cast<size_t>(std::max<py::ssize_t>(mask.shape(0), 1)), 0);
+          for (py::ssize_t i = 0; i < mask.shape(0); ++i) m8[i] = mask.data()[i] ? 1 : 0;
+          const uint8_t* mp = m8.data();
+          const b2m_abs_pose_problem q = AbsProblem(c, points2D, points3D);
+          const b2m_pose_refine_opts f = ToAbi(refinement_options);
+          b2m_abs_pose_result r;
+          const AbsPoseApi& api = AbsPose();
+          b2m_ctx* ctx = Engine::Get(0);
+          int rc;
+          {
+            py::gil_scoped_release release;
+            rc = api.refine(ctx, &q, 1, init, &mp, &f, 0, &r);
+          }
+          ThrowOnError(ctx, rc);
+          if (refinement_options.refine_focal_length || refinement_options.refine_extra_params) WriteCameraParams(camera, r, c.model);
+          if (!r.success) return py::object(py::none());
+          py::dict d;
+          d["cam_from_world"] = PoseToPython(m, r.qvec, r.tvec);
+          return py::object(d);
+        },
+        "cam_from_world"_a, "points2D"_a, "points3D"_a, "inlier_mask"_a, "camera"_a,
+        "refinement_options"_a = AbsolutePoseRefinementOptions(), "Non-linear refinement of absolute pose.");
   m.def("fundamental_matrix_estimation",
         [](const ArrD& points1, const ArrD& points2, const RANSACOptions& estimation_options) {
           CheckSameLength(points1, points2, "fundamental_matrix.h:22");

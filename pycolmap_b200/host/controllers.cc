@@ -50,6 +50,33 @@ b2m_ransac_opts ToAbi(const RANSACOptions& o) {
   return r;
 }
 
+// The absolute pose structs are filled field by field (no b2m_*_opts_default call): the host module binds the absolute
+// pose entry points at run time (bindings.cc) and references no symbol of C ABI version 4 at link time.
+b2m_abs_pose_opts ToAbi(const AbsolutePoseEstimationOptions& o) {
+  b2m_abs_pose_opts r;
+  memset(&r, 0, sizeof(r));
+  r.struct_size = sizeof(r);
+  r.estimate_focal_length = o.estimate_focal_length ? 1 : 0;
+  r.num_focal_length_samples = o.num_focal_length_samples;
+  r.min_focal_length_ratio = o.min_focal_length_ratio;
+  r.max_focal_length_ratio = o.max_focal_length_ratio;
+  r.ransac = ToAbi(o.ransac);
+  return r;
+}
+
+b2m_pose_refine_opts ToAbi(const AbsolutePoseRefinementOptions& o) {
+  b2m_pose_refine_opts r;
+  memset(&r, 0, sizeof(r));
+  r.struct_size = sizeof(r);
+  r.gradient_tolerance = o.gradient_tolerance;
+  r.max_num_iterations = o.max_num_iterations;
+  r.loss_function_scale = o.loss_function_scale;
+  r.refine_focal_length = o.refine_focal_length ? 1 : 0;
+  r.refine_extra_params = o.refine_extra_params ? 1 : 0;
+  r.print_summary = o.print_summary ? 1 : 0;
+  return r;
+}
+
 b2m_tvg_opts ToAbi(const TwoViewGeometryOptions& o) {
   b2m_tvg_opts t;
   b2m_tvg_opts_default(&t);

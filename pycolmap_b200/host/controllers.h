@@ -82,7 +82,29 @@ struct TwoViewGeometryOptions {
   RANSACOptions ransac{4.0, 0.25, 0.999, 3.0, 100, 10000};
 };
 
+// AbsolutePoseEstimationOptions / AbsolutePoseRefinementOptions as pycolmap constructs them
+// (R:pycolmap/estimators/absolute_pose.h:97-131): estimation with RANSACOptions() and max_error 12, refinement with
+// refine_focal_length = refine_extra_params = print_summary = false.
+struct AbsolutePoseEstimationOptions {
+  bool estimate_focal_length = false;
+  int num_focal_length_samples = 30;
+  double min_focal_length_ratio = 0.2;
+  double max_focal_length_ratio = 5.0;
+  RANSACOptions ransac{12.0, 0.01, 0.9999, 3.0, 1000, 100000};
+};
+
+struct AbsolutePoseRefinementOptions {
+  double gradient_tolerance = 1.0;
+  int max_num_iterations = 100;
+  double loss_function_scale = 1.0;
+  bool refine_focal_length = false;
+  bool refine_extra_params = false;
+  bool print_summary = false;
+};
+
 b2m_sift_opts ToAbi(const SiftMatchingOptions& o);
+b2m_abs_pose_opts ToAbi(const AbsolutePoseEstimationOptions& o);
+b2m_pose_refine_opts ToAbi(const AbsolutePoseRefinementOptions& o);
 b2m_ransac_opts ToAbi(const RANSACOptions& o);
 b2m_tvg_opts ToAbi(const TwoViewGeometryOptions& o);
 // Database camera -> ABI camera; throws std::invalid_argument for models the verifier does not take.

@@ -23,4 +23,14 @@ $T $S --tool synccheck --error-exitcode 1 python -m pytest -q -x -m gpu -p no:ca
 echo "synccheck exit $?" | tee -a gpurun_out/sanitize_synccheck.log
 DIAG_N=120 DIAG_REPS=1 $T $S --tool racecheck --error-exitcode 1 python tools/diag_determinism.py > gpurun_out/sanitize_racecheck_verifier.log 2>&1
 echo "racecheck (verifier) exit $?" | tee -a gpurun_out/sanitize_racecheck_verifier.log
+# absolute pose: the RANSAC, selection and refinement kernels on small shapes (logs under $ABS_LOGS, default out/)
+ABS_LOGS=${ABS_LOGS:-out}
+mkdir -p "$ABS_LOGS"
+$T $S --tool memcheck --error-exitcode 1 python -m pytest -q -x -m gpu -p no:cacheprovider tests/test_zz_abs_pose_gpu.py \
+    -k "not 4097" > $ABS_LOGS/sanitize_memcheck_abs_pose.log 2>&1
+echo "memcheck (absolute pose) exit $?" | tee -a $ABS_LOGS/sanitize_memcheck_abs_pose.log
+$T $S --tool racecheck --error-exitcode 1 python -m pytest -q -x -m gpu -p no:cacheprovider tests/test_zz_abs_pose_gpu.py \
+    -k "covariance or pose_refinement" > $ABS_LOGS/sanitize_racecheck_abs_pose.log 2>&1
+echo "racecheck (absolute pose) exit $?" | tee -a $ABS_LOGS/sanitize_racecheck_abs_pose.log
 tail -n 4 gpurun_out/sanitize_*.log
+tail -n 4 "$ABS_LOGS"/sanitize_*_abs_pose.log
