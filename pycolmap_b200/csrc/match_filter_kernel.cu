@@ -2,14 +2,17 @@
 // resolve kernel.
 //
 // Grid = one CTA per SM, persistent: every CTA walks a static list of work units (image pair, direction,
-// 256-row block of the "row" image A, 128-row half of that block).
-//   * Two consumer warpgroups each issue wgmma.mma_async m64n128k32 (u8 x u8 -> s32) for their 64 rows of
-//     the unit against each half of every 256-column tile of image B (four k-steps per half), accumulators in
-//     registers.  Halves rather than one m64n256 keep the 64 accumulators and the 32 slot maxima of a thread
-//     within the register budget of 288 threads per SM without spills.
-//   * One producer warp streams B through a 4-stage ring of 32 KiB tiles (TMA, SWIZZLE_128B) and the A
+// 256-row block of the "row" image A).
+//   * Two consumer warpgroups own 128 rows of the unit each, as two 64-row blocks.  At the start of a unit every
+//     consumer thread loads its A fragments (2 blocks x 4 k-steps x 4 registers) from the swizzled strip into
+//     registers and releases the strip at once; from then on only B is read from shared memory.  For each
+//     128-column half of every 256-column tile of image B and each block, a warpgroup issues four
+//     wgmma.mma_async m64n128k32 (u8 x u8 -> s32, A from registers) into one 64-register accumulator bank, waits
+//     and folds it into the slot maxima of that block.  Halves rather than one m64n256 keep the 64 accumulators,
+//     32 A registers and 64 slot maxima of a thread within the 232 registers a consumer thread gets (setmaxnreg).
+//   * One lane of a producer warpgroup streams B through a 4-stage ring of 32 KiB tiles (TMA, SWIZZLE_128B) and the 32 KiB A
 //     strips through two buffers, so the pipeline runs straight across unit boundaries; barriers are set up
-//     once per launch.
+//     once per launch.  Each B tile serves 256 rows, and A costs shared-memory bandwidth once per unit.
 //   * While one warpgroup folds its accumulators the other one can use the tensor cores.
 //
 // Filter: instead of an exact running top-2 (4 ALU ops per accumulator) each row keeps 64 "slot maxima".
@@ -36,17 +39,25 @@ namespace b2m {
 namespace {
 
 constexpr int kDim = 128;
-constexpr int kTileM = 128;                        // rows per work unit: two consumer warpgroups of 64 rows
-constexpr int kRowsPerItem = 256;                  // rows of A per work item (two units) == kRowPad
+constexpr int kRowsPerItem = 256;                  // rows of A per work unit == kRowPad: two warpgroups x 2 x 64
+constexpr int kBoxRows = 128;                      // rows of one TMA box (tensor maps are 128 x 128 bytes)
+constexpr int kStripRows = 128;                    // the launchers' max_strips counts 128-row strips
 constexpr int kTileN = 256;                        // columns per B tile (the N of one wgmma)
 constexpr int kStages = 4;                         // B-tile ring depth
 constexpr int kABufs = 2;                          // A strips double-buffered across work units
-constexpr int kBytesA = kTileM * kDim;             // 16 KiB per strip
+constexpr int kBytesA = kRowsPerItem * kDim;       // 32 KiB per strip
 constexpr int kBytesB = kTileN * kDim;             // 32 KiB per B tile
+constexpr int kBytesBox = kBoxRows * kDim;         // 16 KiB per TMA box
 constexpr int kConsumerWarps = 8;
 constexpr int kOwnSlots = 16;                      // slot maxima per row kept in one thread's registers
 constexpr int kSlots = kOwnSlots * 4;              // 64 slot maxima per row (four lanes of a quad)
-constexpr int kThreads = (kConsumerWarps + 1) * 32;  // + TMA producer warp
+// + a producer warpgroup (one lane issues the TMA loads).  Warps are spread over the SM's four sub-partitions of 16 384
+// registers each: with 288 threads one of them holds three warps, so a thread could use no more than 168 registers, as
+// with 384.  A whole producer warpgroup can hand its registers to the consumers (setmaxnreg): 128 x 40 + 256 x 232 =
+// 64 512 of the SM's 65 536.
+constexpr int kThreads = (kConsumerWarps + 4) * 32;
+constexpr int kProducerRegs = 40;
+constexpr int kConsumerRegs = 232;
 static_assert(kRowsPerItem == kRowPad && kTileN == kRowPad, "images are padded to whole items / column tiles");
 
 struct __align__(8) Barriers {
@@ -58,12 +69,12 @@ struct __align__(8) Barriers {
 
 constexpr size_t kSmemBytes = 1024 + kABufs * kBytesA + kStages * kBytesB + sizeof(Barriers);
 
-// A work unit and the data every warp role derives from its index (pure function of `w` and `half`).
+// A work unit and the data every warp role derives from its index (pure function of `w`).
 struct Item {
   int pair, dir, nA, nB, rowA, rowB, n_tiles, row0;  // row0: first row (inside image A) of this unit
   bool valid;
 };
-__device__ __forceinline__ Item decode_item(const MatchParams& p, int w, int half) {
+__device__ __forceinline__ Item decode_item(const MatchParams& p, int w) {
   Item it;
   if (p.item_list) {
     // gathered column direction: rows = the gathered block of the pair (scratch tensor map), columns = image a
@@ -74,7 +85,7 @@ __device__ __forceinline__ Item decode_item(const MatchParams& p, int w, int hal
     it.nA = p.gath_cnt[it.pair];
     it.nB = p.img_nfeat[ib];
     it.valid = cb * kRowsPerItem < it.nA;
-    it.row0 = cb * kRowsPerItem + half * kTileM;
+    it.row0 = cb * kRowsPerItem;
     it.rowA = it.pair * p.mstride + it.row0;
     it.rowB = p.img_row0[ib];
     it.n_tiles = (it.nB + kTileN - 1) / kTileN;
@@ -88,10 +99,9 @@ __device__ __forceinline__ Item decode_item(const MatchParams& p, int w, int hal
   const int ib = p.pairs[2 * it.pair + (it.dir ^ 1)];
   it.nA = p.img_nfeat[ia];
   it.nB = p.img_nfeat[ib];
-  // same answer for both halves of an item; an empty image B still yields a unit (n_tiles == 0)
-  // so that its rows are written as "no match"
+  // an empty image B still yields a unit (n_tiles == 0) so that its rows are written as "no match"
   it.valid = cb * kRowsPerItem < it.nA;
-  it.row0 = cb * kRowsPerItem + half * kTileM;
+  it.row0 = cb * kRowsPerItem;
   it.rowA = p.img_row0[ia] + it.row0;
   it.rowB = p.img_row0[ib];
   it.n_tiles = (it.nB + kTileN - 1) / kTileN;
@@ -107,14 +117,14 @@ b2m_k1_filter_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_cons
   // strips (== tmap except for the gathered column direction, where it covers the gather scratch)
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* smA = smem;                                     // [kABufs][16 KiB]
+  uint8_t* smA = smem;                                     // [kABufs][32 KiB]
   uint8_t* smB = smem + kABufs * kBytesA;                  // [kStages][32 KiB]
   Barriers* bars = reinterpret_cast<Barriers*>(smB + kStages * kBytesB);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   // gathered column direction: the work list was built on the device, so was its length
-  const int n_units = 2 * (p.item_list ? __ldg(p.n_items_ptr) : p.n_items);
+  const int n_units = p.item_list ? __ldg(p.n_items_ptr) : p.n_items;
 
   if (warp == kConsumerWarps && lane == 0) {
     tma_prefetch_desc(&tmap);
@@ -131,24 +141,26 @@ b2m_k1_filter_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_cons
   }
   __syncthreads();
 
-  if (warp == kConsumerWarps) {
+  if (warp >= kConsumerWarps) {
     // ===== TMA producer (one lane) =====
-    if (lane == 0) {
+    setmaxnreg_dec<kProducerRegs>();
+    if (warp == kConsumerWarps && lane == 0) {
       uint32_t stage = 0, phase = 0, n_done = 0;
       for (int u = blockIdx.x; u < n_units; u += gridDim.x) {
-        const Item it = decode_item(p, u >> 1, u & 1);
+        const Item it = decode_item(p, u);
         if (!it.valid || it.n_tiles == 0) continue;
         const uint32_t ab = n_done & 1, aph = (n_done >> 1) & 1;
         ++n_done;
-        mbar_wait(&bars->empty_a[ab], aph ^ 1);  // the MMAs of the unit that used this A buffer completed
+        mbar_wait(&bars->empty_a[ab], aph ^ 1);  // the consumers of the unit that used this A buffer hold it in registers
         mbar_arrive_expect_tx(&bars->full_a[ab], kBytesA);
         tma_load_2d(smA + ab * kBytesA, &tmap_a, &bars->full_a[ab], 0, it.rowA);
+        tma_load_2d(smA + ab * kBytesA + kBytesBox, &tmap_a, &bars->full_a[ab], 0, it.rowA + kBoxRows);
         for (int t = 0; t < it.n_tiles; ++t) {
           mbar_wait(&bars->empty_b[stage], phase ^ 1);
           mbar_arrive_expect_tx(&bars->full_b[stage], kBytesB);
           uint8_t* dst = smB + stage * kBytesB;
           tma_load_2d(dst, &tmap, &bars->full_b[stage], 0, it.rowB + t * kTileN);
-          tma_load_2d(dst + kBytesA, &tmap, &bars->full_b[stage], 0, it.rowB + t * kTileN + 128);
+          tma_load_2d(dst + kBytesBox, &tmap, &bars->full_b[stage], 0, it.rowB + t * kTileN + kBoxRows);
           if (++stage == kStages) {
             stage = 0;
             phase ^= 1;
@@ -158,59 +170,68 @@ b2m_k1_filter_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_cons
     }
   } else {
     // ===== consumers: MMA + filter epilogue =====
+    setmaxnreg_inc<kConsumerRegs>();
     const int wg = warp >> 2;
     const int q = lane & 3;
-    const int row_in_unit = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // rows row_in_unit and row_in_unit + 8
-    uint32_t acc[64];   // one 128-column half of a tile at a time: the slot maxima stay in registers beside it
+    // the thread's rows: row_in_unit + 64 blk + 8 i (blk, i = 0, 1)
+    const int row_in_unit = wg * 128 + (warp & 3) * 16 + (lane >> 2);
+    uint32_t acc[64];   // one 64-row block x 128-column half of a tile at a time
 #pragma unroll
     for (int i = 0; i < 64; ++i) acc[i] = 0u;
     uint32_t stage = 0, phase = 0, n_done = 0;
     for (int u = blockIdx.x; u < n_units; u += gridDim.x) {
-      const Item it = decode_item(p, u >> 1, u & 1);
+      const Item it = decode_item(p, u);
       if (!it.valid) continue;
-      uint32_t S[2][kOwnSlots];   // slot maxima of the thread's two rows
+      const int n_tiles = it.n_tiles;
+      uint32_t S[4][kOwnSlots];   // slot maxima of the thread's four rows, [2 blk + i]
 #pragma unroll
-      for (int i = 0; i < 2; ++i)
+      for (int i = 0; i < 4; ++i)
 #pragma unroll
         for (int r = 0; r < kOwnSlots; ++r) S[i][r] = 0u;
-      if (it.n_tiles > 0) {
+      if (n_tiles > 0) {
         const uint32_t ab = n_done & 1, aph = (n_done >> 1) & 1;
         ++n_done;
         mbar_wait(&bars->full_a[ab], aph);
-        const uint32_t a_addr = smem_u32(smA + ab * kBytesA + wg * 64 * kDim);
+        uint32_t afrag[2][16];
+#pragma unroll
+        for (int blk = 0; blk < 2; ++blk)
+          load_a_frag_sw128(afrag[blk], smA + ab * kBytesA + (wg * 128 + blk * 64) * kDim, warp & 3, lane);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&bars->empty_a[ab]);   // the strip lives in registers from here on
 #pragma unroll 1
-        for (int t = 0; t < it.n_tiles; ++t) {
+        for (int t = 0; t < n_tiles; ++t) {
           mbar_wait(&bars->full_b[stage], phase);
 #pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            wgmma_tile_u8(acc, a_addr, smem_u32(smB + stage * kBytesB + h * (kBytesB / 2)));
-            if (h == 1) {
-              __syncwarp();
-              if (lane == 0) mbar_arrive(&bars->empty_b[stage]);   // the MMAs reading this stage have completed
-            }
-            // column 128 h + 8 j + 2 q + e (acc[4 j + 2 i + e], j < 16) = 64 c + 8 (r >> 1) + 2 q + (r & 1) with
-            // c = 2 h + j / 8, r = 2 (j % 8) + e
+          for (int h = 0; h < 2; ++h)
 #pragma unroll
-            for (int i = 0; i < 2; ++i)
-#pragma unroll
-              for (int r = 0; r < kOwnSlots; ++r) {
-                const int a0 = 4 * (r >> 1) + 2 * i + (r & 1);
-                S[i][r] = max(S[i][r], max(acc[a0], acc[a0 + 32]));
+            for (int blk = 0; blk < 2; ++blk) {
+              wgmma_tile_u8_rs(acc, afrag[blk], smem_u32(smB + stage * kBytesB + h * (kBytesB / 2)));
+              if (h == 1 && blk == 1) {
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&bars->empty_b[stage]);   // the MMAs reading this stage have completed
               }
-          }
+              // column 128 h + 8 j + 2 q + e (acc[4 j + 2 i + e], j < 16) = 64 c + 8 (r >> 1) + 2 q + (r & 1) with
+              // c = 2 h + j / 8, r = 2 (j % 8) + e
+#pragma unroll
+              for (int i = 0; i < 2; ++i)
+#pragma unroll
+                for (int r = 0; r < kOwnSlots; ++r) {
+                  const int a0 = 4 * (r >> 1) + 2 * i + (r & 1);
+                  S[2 * blk + i][r] = max(S[2 * blk + i][r], max(acc[a0], acc[a0 + 32]));
+                }
+            }
           if (++stage == kStages) {
             stage = 0;
             phase ^= 1;
           }
         }
-        if (lane == 0) mbar_arrive(&bars->empty_a[ab]);
       }
       // (largest, second largest) over the 64 slot maxima of each row, multiset semantics, lowest slot id on ties:
       // the thread's 16 slots first, then the four lanes of the quad (slot ids 16 q + r)
-      uint32_t best[2], s1[2];
-      int sstar[2];
+      uint32_t best[4], s1[4];
+      int sstar[4];
 #pragma unroll
-      for (int i = 0; i < 2; ++i) {
+      for (int i = 0; i < 4; ++i) {
         best[i] = 0u;
         s1[i] = 0u;
         sstar[i] = 0;
@@ -238,22 +259,28 @@ b2m_k1_filter_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_cons
           s1[i] = ns;
         }
       }
-      if (q < 2) {   // lane q of the quad decides row row_in_unit + 8 q
-        const uint32_t b = q ? best[1] : best[0], s = q ? s1[1] : s1[0];
-        const int slot = q ? sstar[1] : sstar[0];
-        const float fa = __ldg(p.acos_lut + min(b, 262144u));
-        const float fb = __ldg(p.acos_lut + min(s, 262144u));
-        int32_t out = -1;
-        if (b > 0u && !(fa > p.max_distance) && !(fa >= __fmul_rn(p.max_ratio, fb)))
-          out = -2 - slot;  // candidate: resolve exactly
-        const int64_t base = (static_cast<int64_t>(it.pair) * 2 + it.dir) * p.mstride;
-        const int row = it.row0 + row_in_unit + 8 * q;
-        p.mbuf[base + row] = out;
-        if (out != -1 && row < it.nA) {
-          p.aux[base + row] = make_uint2(b, s);
-          const int k = atomicAdd(p.cand_cnt + it.pair * 2 + it.dir, 1);
-          p.cand_rows[base + k] = row | (slot << 24);  // winning slot travels with the row
+      // lane q of the quad decides row row_in_unit + 64 (q >> 1) + 8 (q & 1)
+      uint32_t b = best[0], s = s1[0];
+      int slot = sstar[0];
+#pragma unroll
+      for (int i = 1; i < 4; ++i)
+        if (q == i) {
+          b = best[i];
+          s = s1[i];
+          slot = sstar[i];
         }
+      const float fa = __ldg(p.acos_lut + min(b, 262144u));
+      const float fb = __ldg(p.acos_lut + min(s, 262144u));
+      int32_t out = -1;
+      if (b > 0u && !(fa > p.max_distance) && !(fa >= __fmul_rn(p.max_ratio, fb)))
+        out = -2 - slot;  // candidate: resolve exactly
+      const int64_t base = (static_cast<int64_t>(it.pair) * 2 + it.dir) * p.mstride;
+      const int row = it.row0 + row_in_unit + 64 * (q >> 1) + 8 * (q & 1);
+      p.mbuf[base + row] = out;
+      if (out != -1 && row < it.nA) {
+        p.aux[base + row] = make_uint2(b, s);
+        const int k = atomicAdd(p.cand_cnt + it.pair * 2 + it.dir, 1);
+        p.cand_rows[base + k] = row | (slot << 24);  // winning slot travels with the row
       }
     }
   }
@@ -475,9 +502,9 @@ cudaError_t launch_k1_filter(const CUtensorMap& tmap, const MatchParams& p_in,
   if (e != cudaSuccess) return e;
   // rows never visited by a work item (dir 1 without cross-check is simply not produced)
   p.n_dirs = n_dirs;
-  p.blocks_per_image = (max_strips * kTileM + kRowsPerItem - 1) / kRowsPerItem;
+  p.blocks_per_image = (max_strips * kStripRows + kRowsPerItem - 1) / kRowsPerItem;
   p.n_items = n_pairs * n_dirs * p.blocks_per_image;
-  const int ctas = 2 * p.n_items < num_sms ? 2 * p.n_items : num_sms;
+  const int ctas = p.n_items < num_sms ? p.n_items : num_sms;
   if (ctas > 0) {
     b2m_k1_filter_kernel<<<ctas, kThreads, kSmemBytes, stream>>>(tmap, tmap, p);
     e = cudaGetLastError();
@@ -537,9 +564,9 @@ cudaError_t launch_k1_filter_skip(const CUtensorMap& tmap, const MatchParams& p_
   cudaError_t e = cudaMemsetAsync(p.cand_cnt, 0, sizeof(int32_t) * 2 * n_pairs, stream);
   if (e != cudaSuccess) return e;
   p.n_dirs = 1;
-  p.blocks_per_image = (max_strips * kTileM + kRowsPerItem - 1) / kRowsPerItem;
+  p.blocks_per_image = (max_strips * kStripRows + kRowsPerItem - 1) / kRowsPerItem;
   p.n_items = n_pairs * p.blocks_per_image;
-  const int ctas = 2 * p.n_items < num_sms ? 2 * p.n_items : num_sms;
+  const int ctas = p.n_items < num_sms ? p.n_items : num_sms;
   if (ctas > 0) {
     // 1. row direction of every pair
     b2m_k1_filter_kernel<<<ctas, kThreads, kSmemBytes, stream>>>(tmap, tmap, p);
@@ -687,11 +714,11 @@ cudaError_t launch_k1_gather_phase(int phase, const CUtensorMap& tmap, const CUt
   if (n_pairs <= 0) return cudaSuccess;
   MatchParams p = p_in;
   p.n_dirs = 1;
-  p.blocks_per_image = (max_strips * kTileM + kRowsPerItem - 1) / kRowsPerItem;
+  p.blocks_per_image = (max_strips * kStripRows + kRowsPerItem - 1) / kRowsPerItem;
   p.n_items = n_pairs * p.blocks_per_image;
   p.item_list = nullptr;
   p.gath_desc = nullptr;
-  const int ctas = 2 * p.n_items < num_sms ? 2 * p.n_items : num_sms;
+  const int ctas = p.n_items < num_sms ? p.n_items : num_sms;
   if (ctas <= 0) return cudaSuccess;
   cudaError_t e = cudaSuccess;
   switch (phase) {

@@ -54,6 +54,16 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m
       : "memory");
 }
 
+// ---- register reallocation between warpgroups (all warps of a warpgroup execute it) -----
+template <uint32_t N>
+__device__ __forceinline__ void setmaxnreg_dec() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N));
+}
+template <uint32_t N>
+__device__ __forceinline__ void setmaxnreg_inc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N));
+}
+
 // ---- wgmma (Hopper warpgroup MMA) -------------------------------------------------------
 // Shared-memory matrix descriptor for a K-major tile whose rows are exactly 128 bytes (= one SWIZZLE_128B
 // atom, the layout TMA writes with CU_TENSOR_MAP_SWIZZLE_128B): 8-row groups are 1024 B apart (SBO), LBO
@@ -94,6 +104,31 @@ __device__ __forceinline__ void wgmma_m64n128k32_u8(uint32_t (&d)[64], uint64_t 
         "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63])
       : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
+// Same MMA with A[64 x 32] in registers (four 32-bit registers a[0..3] per thread, the mma.m16n8k32 int8 A fragment
+// of the thread's warp: warp w covers rows 16 w .. 16 w + 15; with g = l / 4, t = l % 4, a[0] = row g, bytes 4 t .. 4 t + 3,
+// a[1] = row g + 8, same bytes, a[2] / a[3] = rows g / g + 8, bytes 16 + 4 t .. 16 + 4 t + 3).  Only B is read from
+// shared memory.  The registers of a must not change until the MMA has completed.
+__device__ __forceinline__ void wgmma_m64n128k32_u8_rs(uint32_t (&d)[64], const uint32_t* a, uint64_t bdesc,
+                                                       uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %69, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k32.s32.u8.u8 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "{%64, %65, %66, %67}, %68, p;\n\t}"
+      : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]),
+        "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]),
+        "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]),
+        "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]),
+        "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]),
+        "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]),
+        "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]),
+        "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate));
+}
 // Keeps the compiler from moving accesses of the accumulators across the asynchronous MMA.
 __device__ __forceinline__ void wgmma_fence_regs(uint32_t (&d)[64]) {
 #pragma unroll
@@ -111,6 +146,34 @@ __device__ __forceinline__ void wgmma_tile_u8(uint32_t (&d)[64], uint32_t a_smem
   wgmma_commit();
   wgmma_wait_all();
   wgmma_fence_regs(d);
+}
+
+// The same tile with A in registers: a[4 k .. 4 k + 3] is the fragment of k-step k (wgmma_m64n128k32_u8_rs).
+__device__ __forceinline__ void wgmma_tile_u8_rs(uint32_t (&d)[64], const uint32_t (&a)[16], uint32_t b_smem) {
+  const uint64_t bdesc = make_wgmma_desc_sw128(b_smem);
+  wgmma_fence_regs(d);
+  wgmma_fence();
+#pragma unroll
+  for (int k = 0; k < 4; ++k) wgmma_m64n128k32_u8_rs(d, a + 4 * k, bdesc + 2 * k, k > 0 ? 1u : 0u);
+  wgmma_commit();
+  wgmma_wait_all();
+  wgmma_fence_regs(d);
+}
+
+// A fragments of a 64-row block for wgmma_tile_u8_rs, read from a SWIZZLE_128B tile (rows of 128 bytes, 16-byte chunk c
+// of row r stored at chunk c ^ (r % 8); 1024-B aligned).  `warp` is the warp's index inside its warpgroup.  Per warp
+// the 32 lanes hit 32 distinct banks.
+__device__ __forceinline__ void load_a_frag_sw128(uint32_t (&a)[16], const uint8_t* block, int warp, int lane) {
+  const int g = lane >> 2, t = lane & 3;
+  const uint8_t* r0 = block + (16 * warp + g) * 128;   // rows g and g + 8 share the swizzle phase g
+#pragma unroll
+  for (int k = 0; k < 4; ++k)
+#pragma unroll
+    for (int hi = 0; hi < 2; ++hi) {
+      const int off = (((2 * k + hi) ^ g) << 4) + 4 * t;
+      a[4 * k + 2 * hi] = *reinterpret_cast<const uint32_t*>(r0 + off);
+      a[4 * k + 2 * hi + 1] = *reinterpret_cast<const uint32_t*>(r0 + 8 * 128 + off);
+    }
 }
 
 }  // namespace b2m
