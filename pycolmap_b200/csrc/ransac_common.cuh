@@ -21,8 +21,9 @@ __device__ __forceinline__ double warp_sum_d(double v) {
 }
 
 // Outcome of `residual <= thr` evaluated as lhs <= rhs = thr * denominator in fp32: bit 0 = clearly an inlier,
-// bit 1 = borderline (within 1 % of the threshold, or not finite) -- the caller re-evaluates those in fp64, so every
-// decision equals the fp64 one.  STRICT comparisons: lhs == rhs == 0 (both underflowed) or == inf (both overflowed) is
+// bit 1 = borderline (within 1 % of the threshold, or not finite) -- the caller re-evaluates those in fp64, so a
+// decision equals the fp64 one as long as the fp32 rounding of lhs and rhs stays inside the 1 % band (see the
+// limits at verify.cu inlier_f32).  STRICT comparisons: lhs == rhs == 0 (both underflowed) or == inf (both overflowed) is
 // neither clearly in nor clearly out, like any NaN.
 __device__ __forceinline__ int classify_f32(float lhs, float rhs) {
   const int in = lhs < 0.99f * rhs ? 1 : 0;

@@ -102,7 +102,12 @@ __device__ __forceinline__ double residual(const double* M, double x1, double y1
 
 // Division-free fp32 inlier test used by the hypothesis-scoring loop: r <= thr  <=>  lhs <= thr * rhs
 // with r = lhs / rhs.  Returns +1 inlier, 0 outlier, -1 borderline (within 1 % of the threshold, or
-// not finite): the caller re-evaluates those in fp64, so decisions equal the fp64 evaluation.
+// not finite): the caller re-evaluates those in fp64.  The 1 % band covers the fp32 rounding only while the
+// operands are small enough: the H arm scores raw pixel coordinates, and ex = x2 w - u cancels, so on images
+// 20 000 px wide at max_error 0.25 px (40 000 px at <= 0.5 px) a point a few % off the threshold can get a
+// confident decision that differs from fp64 (tests/test_fp32_inlier_emulation.py emulates this arm).  The final
+// inlier mask is recomputed in fp64 from the best model either way; such a decision only changes which
+// hypothesis wins.
 template <int KIND>
 __device__ __forceinline__ int inlier_f32(const float* M, float x1, float y1, float x2, float y2, float thr) {
   float lhs, rhs;
