@@ -26,8 +26,9 @@
 extern "C" {
 #endif
 
-#define B2M_ABI_VERSION 4   /* 2: b2m_camera carries 12 parameters, batch estimator; 3: multi-GPU entry points (NCCL);
-                             * 4: absolute pose estimation / refinement, b2m_stats.abs_pose_* */
+#define B2M_ABI_VERSION 5   /* 2: b2m_camera carries 12 parameters, batch estimator; 3: multi-GPU entry points (NCCL);
+                             * 4: absolute pose estimation / refinement, b2m_stats.abs_pose_*;
+                             * 5: triangulation, b2m_stats.tri_* */
 
 /* error codes */
 #define B2M_OK 0
@@ -386,6 +387,35 @@ int b2m_refine_absolute_pose_batch(b2m_ctx* ctx, const b2m_abs_pose_problem* pro
                                    const double* init_poses, const uint8_t* const* inlier_masks,
                                    const b2m_pose_refine_opts* refine, int32_t want_covariance, b2m_abs_pose_result* out);
 
+/* ---- triangulation (callable without an image set) ----------------------------------- */
+
+/* EstimateTriangulationOptions (R:pycolmap/estimators/triangulation.h:46-77; U:estimators/triangulation.h).  The
+ * residual is upstream's default and pycolmap's only one, ANGULAR_ERROR: ransac.max_error is an angle in radians.
+ * b2m_tri_opts_default gives the C++ RANSACOptions defaults; the host module sets pycolmap's Python-side ones. */
+typedef struct b2m_tri_opts {
+  uint32_t struct_size;
+  int32_t reserved;
+  double min_tri_angle;          /* 0, radians */
+  b2m_ransac_opts ransac;        /* max_error in radians (angular residual) */
+} b2m_tri_opts;
+
+void b2m_tri_opts_default(b2m_tri_opts* o);
+
+/* Replaces EstimateTriangulation (U:estimators/triangulation.cc; R:pycolmap/estimators/triangulation.h:17-44) over a
+ * batch of tracks: LO-RANSAC with the two-view DLT as minimal estimator and TriangulateMultiViewPoint as local one,
+ * sample pairs enumerated in lexicographic order (CombinationSampler), so the result is deterministic.
+ * Track k owns observations [track_offsets[k], track_offsets[k + 1]) of points_normalized (camera-normalised (u, v))
+ * and image_idx (index into cams_from_world, [n_images x 12], each a 3 x 4 row-major cam_from_world); every track needs
+ * at least 2 observations (B2M_EINVAL otherwise, as for an out-of-range image index).  The projection centres are
+ * -R^T t of the given matrices.  Out: xyz [n_tracks x 3] (NaN on failure), num_inliers [n_tracks] (the best support,
+ * also on failure), success [n_tracks], inlier_mask [M] or NULL.  Internally in chunks of up to 32768 tracks; results
+ * do not depend on the chunking or the order of the tracks. */
+int b2m_estimate_triangulation_batch(b2m_ctx* ctx, int64_t n_tracks, const int64_t* track_offsets /* n_tracks + 1 */,
+                                     const double* points_normalized /* [M x 2] */, const int32_t* image_idx /* [M] */,
+                                     int32_t n_images, const double* cams_from_world /* [n_images x 12] */,
+                                     const b2m_tri_opts* opts, double* xyz /* [n_tracks x 3] */, int32_t* num_inliers,
+                                     uint8_t* success, uint8_t* inlier_mask /* [M] or NULL */);
+
 /* ---- instrumentation ---------------------------------------------------------------- */
 
 /* The cross-check consults m21 only at the columns some row matched (m21[m12[i]]): the column-direction GEMM is run
@@ -430,6 +460,8 @@ typedef struct b2m_stats {
   int32_t comm_size, comm_rank;       /* 1, 0 without a communicator */
   uint64_t abs_pose_models_scored;    /* absolute pose: P3P / EPnP models scored against all correspondences since reset */
   uint64_t abs_pose_residuals;        /* absolute pose: residual evaluations (models scored x correspondences) */
+  uint64_t tri_models_scored;         /* triangulation: two-view and LO models scored against all observations */
+  uint64_t tri_residuals;             /* triangulation: residual evaluations (models scored x observations of the track) */
 } b2m_stats;
 int b2m_get_stats(b2m_ctx* ctx, b2m_stats* out);
 int b2m_reset_stats(b2m_ctx* ctx);

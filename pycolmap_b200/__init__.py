@@ -16,6 +16,8 @@ try:
     from ._core import *  # noqa: F401,F403
     from ._core import (AbsolutePoseEstimationOptions, AbsolutePoseRefinementOptions,  # noqa: F401
                         absolute_pose_estimation, estimate_absolute_poses, pose_refinement)
+    from ._core import (EstimateTriangulationOptions, PointData, estimate_triangulation,  # noqa: F401
+                        estimate_triangulations)
     from ._core import (Context, Database, DatabaseTransaction, Device, ExhaustiveMatchingOptions,  # noqa: F401
                         RANSACOptions, Results, Rigid3d, Rotation3d, SequentialMatchingOptions,
                         SiftMatchingOptions, SpatialMatchingOptions, TwoViewGeometry,

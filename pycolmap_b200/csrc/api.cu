@@ -854,6 +854,7 @@ void b2m_destroy(b2m_ctx* ctx) {
   comm_release(ctx);
   if (ctx->d_verify_counters) cudaFree(ctx->d_verify_counters);
   if (ctx->d_abs_counters) cudaFree(ctx->d_abs_counters);
+  tri_release(ctx);
   ctx->images.release();
   ctx->ws.release();
   verify_release(ctx);
@@ -1164,6 +1165,14 @@ int b2m_get_stats(b2m_ctx* ctx, b2m_stats* out) {
       out->abs_pose_residuals = h[1];
     }
   }
+  {
+    unsigned long long h[2] = {0, 0};
+    cudaSetDevice(ctx->device);
+    if (tri_counters(ctx, h)) {  // and for triangulation
+      out->tri_models_scored = h[0];
+      out->tri_residuals = h[1];
+    }
+  }
   return B2M_OK;
 }
 int b2m_reset_stats(b2m_ctx* ctx) {
@@ -1178,6 +1187,8 @@ int b2m_reset_stats(b2m_ctx* ctx) {
     cudaSetDevice(ctx->device);
     cudaMemset(ctx->d_abs_counters, 0, sizeof(unsigned long long) * 2);
   }
+  cudaSetDevice(ctx->device);
+  tri_reset_counters(ctx);
   ctx->stats.k1_dir1_mode = static_cast<uint64_t>(ctx->k1_dir1_mode);  // a property of the context, not a counter
   return B2M_OK;
 }

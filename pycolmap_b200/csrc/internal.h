@@ -121,7 +121,15 @@ struct b2m_ctx {
   int comm_size = 1, comm_rank = 0;
   unsigned long long* d_verify_counters = nullptr;  // [6]: models scored / residual evaluations per kind (verify.cu)
   unsigned long long* d_abs_counters = nullptr;     // [2]: models scored / residual evaluations (abs_pose.cu)
+  void* tri_state = nullptr;     // b2m::TriState (triangulation.cu): pinned staging, device buffers, counters
 };
+
+namespace b2m {
+// triangulation.cu
+void tri_release(b2m_ctx* ctx);
+bool tri_counters(b2m_ctx* ctx, unsigned long long* out);  // [2]: models scored, residual evaluations
+void tri_reset_counters(b2m_ctx* ctx);
+}  // namespace b2m
 
 namespace b2m {
 // Allocator of the two big result arrays (hundreds of MB per exhaustive call): resize() leaves new elements

@@ -10,6 +10,7 @@
 //                                                             fundamental_matrix.h:17-50, homography_matrix.h:17-48
 //   RANSACOptions                                             R:optim/bindings.h:7-27
 //   absolute_pose_estimation, pose_refinement, AbsolutePose*Options  R:pycolmap/estimators/absolute_pose.h:18-166
+//   estimate_triangulation, PointData, EstimateTriangulationOptions  R:pycolmap/estimators/triangulation.h:17-77
 //   Device, has_cuda                                          R:utils.h:9-31, R:main.cc:98-106
 //   Database (open/close/counters/read_two_view_geometry/image_pair_to_pair_id)  R:scene/database.h:10-47
 // Everything below the option structs goes through the C ABI of include/b200match.h; there is no CPU path.
@@ -114,6 +115,17 @@ struct Rigid3d {
   Rotation3d rotation;
   std::array<double, 3> translation{0.0, 0.0, 0.0};
 };
+
+// Rigid3d::ToMatrix(): [R | t], 3 x 4 row-major
+std::array<double, 12> RigidToMatrix(const Rigid3d& g) {
+  const Mat3 R = QuatToRotation(g.rotation.wxyz);
+  std::array<double, 12> p;
+  for (int i = 0; i < 3; ++i) {
+    for (int j = 0; j < 3; ++j) p[i * 4 + j] = R[i * 3 + j];
+    p[i * 4 + 3] = g.translation[i];
+  }
+  return p;
+}
 
 struct TwoViewGeometry {
   TwoViewGeometryConfiguration config = TwoViewGeometryConfiguration::UNDEFINED;
@@ -417,6 +429,133 @@ py::object AbsResultToPython(const py::module_& m, const b2m_abs_pose_result& r,
   return d;
 }
 
+// ---- triangulation (R:pycolmap/estimators/triangulation.h:17-77) -------------------------------------------
+// PointData (R:pycolmap/estimators/triangulation.h): the pixel and the camera-normalised observation; only
+// point_normalized enters the angular residual.
+struct PointData {
+  std::array<double, 2> point{0.0, 0.0}, point_normalized{0.0, 0.0};
+};
+
+// Bound at run time like the absolute pose entry points: the host references no C ABI version 5 symbol at link time.
+using TriEstimateFn = decltype(&b2m_estimate_triangulation_batch);
+TriEstimateFn TriEstimate() {
+  static const TriEstimateFn fn = []() -> TriEstimateFn {
+    Dl_info info;
+    if (dladdr(reinterpret_cast<void*>(&b2m_abi_version), &info) && info.dli_fname)
+      if (void* h = dlopen(info.dli_fname, RTLD_NOW | RTLD_NOLOAD))
+        return reinterpret_cast<TriEstimateFn>(dlsym(h, "b2m_estimate_triangulation_batch"));
+    return nullptr;
+  }();
+  if (!fn)
+    throw std::runtime_error("[bindings.cc] libb200match.so does not export the triangulation entry point "
+                             "(C ABI version 5): rebuild it");
+  return fn;
+}
+
+// EstimateTriangulationOptions::Check and RANSACOptions::Check (U:estimators/triangulation.h, U:optim/ransac.h); upstream
+// CHECKs abort the process, here they raise ValueError before any GPU work.
+void CheckTriOptions(const EstimateTriangulationOptions& o) {
+  auto fail = [](const char* what) { throw std::invalid_argument(std::string("[triangulation.h] Check Failed: ") + what); };
+  if (!(o.min_tri_angle >= 0.0)) fail("min_tri_angle >= 0");
+  if (!(o.ransac.max_error > 0.0)) fail("ransac.max_error > 0");
+  if (!(o.ransac.min_inlier_ratio >= 0.0 && o.ransac.min_inlier_ratio <= 1.0)) fail("0 <= ransac.min_inlier_ratio <= 1");
+  if (!(o.ransac.confidence >= 0.0 && o.ransac.confidence <= 1.0)) fail("0 <= ransac.confidence <= 1");
+  if (!(o.ransac.min_num_trials <= o.ransac.max_num_trials)) fail("ransac.min_num_trials <= ransac.max_num_trials");
+}
+
+// cam_from_world of an entry of `images`: an object with a `cam_from_world` attribute (pycolmap's Image; a method
+// returning it is called) or a Rigid3d itself.
+std::array<double, 12> ImagePoseMatrix(const py::handle& image) {
+  py::object g = py::reinterpret_borrow<py::object>(image);
+  if (!py::isinstance<Rigid3d>(g) && py::hasattr(g, "cam_from_world")) {
+    g = g.attr("cam_from_world");
+    if (!py::isinstance<Rigid3d>(g) && PyCallable_Check(g.ptr())) g = g();
+  }
+  if (!py::isinstance<Rigid3d>(g))
+    throw std::invalid_argument("[bindings.cc] Check Failed: each image is a Rigid3d or has a cam_from_world Rigid3d");
+  return RigidToMatrix(g.cast<Rigid3d>());
+}
+
+struct TriBatchOut {
+  std::vector<double> xyz;
+  std::vector<int32_t> num_inliers;
+  std::vector<uint8_t> success, mask;
+};
+
+// One call of the batch entry point; offsets [T + 1], points [M x 2], image indices [M], cams [I x 12].
+TriBatchOut EstimateTriangulationsAbi(b2m_ctx* ctx, const std::vector<int64_t>& off, const double* pts, const int32_t* img,
+                                      int32_t n_images, const double* cams, const EstimateTriangulationOptions& options) {
+  const b2m_tri_opts o = ToAbi(options);
+  const TriEstimateFn fn = TriEstimate();
+  const int64_t T = static_cast<int64_t>(off.size()) - 1, M = off.back();
+  TriBatchOut r;
+  r.xyz.assign(3 * static_cast<size_t>(std::max<int64_t>(T, 1)), 0.0);
+  r.num_inliers.assign(static_cast<size_t>(std::max<int64_t>(T, 1)), 0);
+  r.success.assign(static_cast<size_t>(std::max<int64_t>(T, 1)), 0);
+  r.mask.assign(static_cast<size_t>(std::max<int64_t>(M, 1)), 0);
+  int rc;
+  {
+    py::gil_scoped_release release;
+    rc = fn(ctx, T, off.data(), pts, img, n_images, cams, &o, r.xyz.data(), r.num_inliers.data(), r.success.data(),
+            r.mask.data());
+  }
+  ThrowOnError(ctx, rc);
+  return r;
+}
+
+// estimate_triangulations: (M, 2) points, (T,) lengths, (M,) image indices, (I, 3, 4) cams_from_world.
+py::dict EstimateTriangulationsPy(const std::function<b2m_ctx*()>& get_ctx, const py::object& points_normalized,
+                                  const py::object& track_lengths, const py::object& image_idxs,
+                                  const py::object& cams_from_world, const EstimateTriangulationOptions& options) {
+  CheckTriOptions(options);
+  const ArrD pts = ArrD::ensure(points_normalized);
+  if (!pts || pts.ndim() != 2 || pts.shape(1) != 2)
+    throw std::invalid_argument("[bindings.cc] Check Failed: points_normalized is an M x 2 float64 array");
+  using ArrI64 = py::array_t<int64_t, py::array::c_style | py::array::forcecast>;
+  const ArrI64 len = ArrI64::ensure(track_lengths), idx = ArrI64::ensure(image_idxs);
+  if (!len || len.ndim() != 1) throw std::invalid_argument("[bindings.cc] Check Failed: track_lengths is a 1-D integer array");
+  if (!idx || idx.ndim() != 1) throw std::invalid_argument("[bindings.cc] Check Failed: image_idxs is a 1-D integer array");
+  const ArrD cams = ArrD::ensure(cams_from_world);
+  if (!cams || cams.ndim() != 3 || cams.shape(1) != 3 || cams.shape(2) != 4)
+    throw std::invalid_argument("[bindings.cc] Check Failed: cams_from_world is an I x 3 x 4 float64 array");
+  const int64_t T = len.shape(0), M = pts.shape(0), I = cams.shape(0);
+  if (I > INT32_MAX) throw std::invalid_argument("[bindings.cc] Check Failed: fewer than 2^31 images");
+  std::vector<int64_t> off(static_cast<size_t>(T) + 1, 0);
+  for (int64_t k = 0; k < T; ++k) {
+    if (len.data()[k] < 2)  // THROW_CHECK_GE(point_data.size(), 2)
+      throw std::invalid_argument("[triangulation.cc] Check Failed: track_lengths[" + std::to_string(k) + "] >= 2");
+    off[k + 1] = off[k] + len.data()[k];
+  }
+  if (off[T] != M)
+    throw std::invalid_argument("[bindings.cc] Check Failed: sum(track_lengths) == len(points_normalized) (" +
+                                std::to_string(off[T]) + " vs. " + std::to_string(M) + ")");
+  if (idx.shape(0) != M)
+    throw std::invalid_argument("[bindings.cc] Check Failed: len(image_idxs) == len(points_normalized)");
+  std::vector<int32_t> img(static_cast<size_t>(std::max<int64_t>(M, 1)));
+  for (int64_t i = 0; i < M; ++i) {
+    const int64_t v = idx.data()[i];
+    if (v < 0 || v >= I)
+      throw std::invalid_argument("[bindings.cc] Check Failed: 0 <= image_idxs[" + std::to_string(i) + "] < " + std::to_string(I));
+    img[i] = static_cast<int32_t>(v);
+  }
+  const TriBatchOut r = EstimateTriangulationsAbi(get_ctx(), off, pts.data(), img.data(), static_cast<int32_t>(I), cams.data(),
+                                                  options);
+  py::array_t<double> xyz(std::vector<py::ssize_t>{static_cast<py::ssize_t>(T), 3});
+  py::array_t<bool> success(static_cast<py::ssize_t>(T));
+  py::array_t<int64_t> num_inliers(static_cast<py::ssize_t>(T));
+  for (int64_t k = 0; k < T; ++k) {
+    for (int a = 0; a < 3; ++a) xyz.mutable_data()[3 * k + a] = r.xyz[3 * k + a];
+    success.mutable_data()[k] = r.success[k] != 0;
+    num_inliers.mutable_data()[k] = r.num_inliers[k];
+  }
+  py::dict d;
+  d["xyz"] = xyz;
+  d["success"] = success;
+  d["num_inliers"] = num_inliers;
+  d["inliers"] = MaskToNumpy(r.mask, M);
+  return d;
+}
+
 }  // namespace
 
 PYBIND11_MODULE(_core, m) {
@@ -537,13 +676,9 @@ PYBIND11_MODULE(_core, m) {
         return a;
       })
       .def("matrix", [](const Rigid3d& g) {
-        const Mat3 R = QuatToRotation(g.rotation.wxyz);
+        const std::array<double, 12> m = RigidToMatrix(g);
         py::array_t<double> a(std::vector<py::ssize_t>{3, 4});
-        double* p = a.mutable_data();
-        for (int i = 0; i < 3; ++i) {
-          for (int j = 0; j < 3; ++j) p[i * 4 + j] = R[i * 3 + j];
-          p[i * 4 + 3] = g.translation[i];
-        }
+        std::copy(m.begin(), m.end(), a.mutable_data());
         return a;
       })
       .def("inverse", [](const Rigid3d& g) {
@@ -873,6 +1008,68 @@ PYBIND11_MODULE(_core, m) {
         },
         "cam_from_world"_a, "points2D"_a, "points3D"_a, "inlier_mask"_a, "camera"_a,
         "refinement_options"_a = AbsolutePoseRefinementOptions(), "Non-linear refinement of absolute pose.");
+  // ---- triangulation ----
+  py::class_<PointData>(m, "PointData")
+      .def(py::init([](const std::array<double, 2>& point, const std::array<double, 2>& point_normalized) {
+             return PointData{point, point_normalized};
+           }),
+           "point"_a, "point_normalized"_a)
+      .def_property_readonly("point", [](const PointData& d) { return py::array_t<double>(2, d.point.data()); })
+      .def_property_readonly("point_normalized",
+                             [](const PointData& d) { return py::array_t<double>(2, d.point_normalized.data()); })
+      .def("__repr__", [](const PointData& d) {
+        return "PointData(point=[" + std::to_string(d.point[0]) + ", " + std::to_string(d.point[1]) +
+               "], point_normalized=[" + std::to_string(d.point_normalized[0]) + ", " +
+               std::to_string(d.point_normalized[1]) + "])";
+      });
+  OptionsClass<EstimateTriangulationOptions>(m, "EstimateTriangulationOptions")
+      .field("min_tri_angle", &EstimateTriangulationOptions::min_tri_angle, "Minimum triangulation angle in radians.")
+      .field("ransac", &EstimateTriangulationOptions::ransac, "RANSAC options; max_error is an angle in radians.")
+      .Finish();
+  m.def("estimate_triangulation",
+        [](const py::list& point_data, const py::list& images, const py::list& cameras,
+           const EstimateTriangulationOptions& opions) {
+          const size_t n = images.size();
+          if (cameras.size() != n)  // THROW_CHECK_EQ(images.size(), cameras.size()), R:triangulation.h
+            throw std::invalid_argument("[triangulation.h] Check Failed: images.size() == cameras.size() (" +
+                                        std::to_string(n) + " vs. " + std::to_string(cameras.size()) + ")");
+          if (point_data.size() != n)
+            throw std::invalid_argument("[triangulation.h] Check Failed: images.size() == point_data.size() (" +
+                                        std::to_string(n) + " vs. " + std::to_string(point_data.size()) + ")");
+          CheckTriOptions(opions);
+          if (n < 2) throw std::invalid_argument("[triangulation.cc] Check Failed: point_data.size() >= 2");
+          std::vector<double> pts(2 * n), cams(12 * n);
+          std::vector<int32_t> img(n);
+          for (size_t i = 0; i < n; ++i) {
+            CameraFromPython(py::reinterpret_borrow<py::object>(cameras[i]));  // validates; the angular residual does not use it
+            const PointData d = point_data[i].cast<PointData>();
+            pts[2 * i] = d.point_normalized[0];
+            pts[2 * i + 1] = d.point_normalized[1];
+            const std::array<double, 12> P = ImagePoseMatrix(images[i]);
+            std::copy(P.begin(), P.end(), cams.begin() + 12 * i);
+            img[i] = static_cast<int32_t>(i);
+          }
+          const std::vector<int64_t> off{0, static_cast<int64_t>(n)};
+          const TriBatchOut r =
+              EstimateTriangulationsAbi(Engine::Get(0), off, pts.data(), img.data(), static_cast<int32_t>(n), cams.data(), opions);
+          if (!r.success[0]) return py::object(py::none());
+          py::dict d;
+          d["xyz"] = py::array_t<double>(3, r.xyz.data());
+          d["inliers"] = MaskToNumpy(r.mask, static_cast<int64_t>(n));
+          return py::object(d);
+        },
+        "point_data"_a, "images"_a, "cameras"_a, "opions"_a = EstimateTriangulationOptions(),
+        "Robustly triangulate one track from its observations (the options keyword is spelled `opions`, as in pycolmap).");
+  m.def("estimate_triangulations",
+        [](const py::object& points_normalized, const py::object& track_lengths, const py::object& image_idxs,
+           const py::object& cams_from_world, const EstimateTriangulationOptions& options) {
+          return EstimateTriangulationsPy([] { return Engine::Get(0); }, points_normalized, track_lengths, image_idxs,
+                                          cams_from_world, options);
+        },
+        "points_normalized"_a, "track_lengths"_a, "image_idxs"_a, "cams_from_world"_a,
+        "options"_a = EstimateTriangulationOptions(),
+        "Batched estimate_triangulation over T tracks stored back to back: returns dict(xyz (T, 3), NaN rows on failure; "
+        "success (T,); num_inliers (T,); inliers (M,))");
   m.def("fundamental_matrix_estimation",
         [](const ArrD& points1, const ArrD& points2, const RANSACOptions& estimation_options) {
           CheckSameLength(points1, points2, "fundamental_matrix.h:22");
@@ -1369,6 +1566,14 @@ PYBIND11_MODULE(_core, m) {
            },
            "camera1"_a, "points1"_a, "camera2"_a, "points2"_a, "matches"_a = py::none(),
            "options"_a = TwoViewGeometryOptions())
+      .def("estimate_triangulations",
+           [](CoreContext& c, const py::object& points_normalized, const py::object& track_lengths,
+              const py::object& image_idxs, const py::object& cams_from_world, const EstimateTriangulationOptions& options) {
+             return EstimateTriangulationsPy([&c] { return c.Handle(); }, points_normalized, track_lengths, image_idxs,
+                                             cams_from_world, options);
+           },
+           "points_normalized"_a, "track_lengths"_a, "image_idxs"_a, "cams_from_world"_a,
+           "options"_a = EstimateTriangulationOptions())
       .def("debug_five_point",
            [](CoreContext& c, const ArrD& nullspaces) {
              if (nullspaces.size() % 36) throw std::invalid_argument("[bindings.cc] Check Failed: null spaces are n x 4 x 9");
@@ -1395,7 +1600,8 @@ PYBIND11_MODULE(_core, m) {
                                                                   s.verify_models_scored[2]),
                         "verify_residuals"_a = py::make_tuple(s.verify_residuals[0], s.verify_residuals[1],
                                                               s.verify_residuals[2]),
-                        "comm_size"_a = s.comm_size, "comm_rank"_a = s.comm_rank);
+                        "comm_size"_a = s.comm_size, "comm_rank"_a = s.comm_rank,
+                        "tri_models_scored"_a = s.tri_models_scored, "tri_residuals"_a = s.tri_residuals);
       })
       .def("reset_stats", [](CoreContext& c) { ThrowOnError(c.Handle(), b2m_reset_stats(c.Handle()));
       });

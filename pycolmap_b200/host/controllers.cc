@@ -64,6 +64,16 @@ b2m_abs_pose_opts ToAbi(const AbsolutePoseEstimationOptions& o) {
   return r;
 }
 
+// Filled field by field for the same reason (C ABI version 5).
+b2m_tri_opts ToAbi(const EstimateTriangulationOptions& o) {
+  b2m_tri_opts r;
+  memset(&r, 0, sizeof(r));
+  r.struct_size = sizeof(r);
+  r.min_tri_angle = o.min_tri_angle;
+  r.ransac = ToAbi(o.ransac);
+  return r;
+}
+
 b2m_pose_refine_opts ToAbi(const AbsolutePoseRefinementOptions& o) {
   b2m_pose_refine_opts r;
   memset(&r, 0, sizeof(r));

@@ -102,7 +102,15 @@ struct AbsolutePoseRefinementOptions {
   bool print_summary = false;
 };
 
+// EstimateTriangulationOptions as pycolmap constructs it (R:pycolmap/estimators/triangulation.h:46-77): min_tri_angle 0
+// and RANSACOptions(); ransac.max_error is an angle in radians (the ANGULAR_ERROR residual).
+struct EstimateTriangulationOptions {
+  double min_tri_angle = 0.0;
+  RANSACOptions ransac{4.0, 0.01, 0.9999, 3.0, 1000, 100000};
+};
+
 b2m_sift_opts ToAbi(const SiftMatchingOptions& o);
+b2m_tri_opts ToAbi(const EstimateTriangulationOptions& o);
 b2m_abs_pose_opts ToAbi(const AbsolutePoseEstimationOptions& o);
 b2m_pose_refine_opts ToAbi(const AbsolutePoseRefinementOptions& o);
 b2m_ransac_opts ToAbi(const RANSACOptions& o);
