@@ -26,9 +26,9 @@
 extern "C" {
 #endif
 
-#define B2M_ABI_VERSION 5   /* 2: b2m_camera carries 12 parameters, batch estimator; 3: multi-GPU entry points (NCCL);
+#define B2M_ABI_VERSION 6   /* 2: b2m_camera carries 12 parameters, batch estimator; 3: multi-GPU entry points (NCCL);
                              * 4: absolute pose estimation / refinement, b2m_stats.abs_pose_*;
-                             * 5: triangulation, b2m_stats.tri_* */
+                             * 5: triangulation, b2m_stats.tri_*; 6: SIFT feature extraction, b2m_stats.sift_* */
 
 /* error codes */
 #define B2M_OK 0
@@ -416,6 +416,61 @@ int b2m_estimate_triangulation_batch(b2m_ctx* ctx, int64_t n_tracks, const int64
                                      const b2m_tri_opts* opts, double* xyz /* [n_tracks x 3] */, int32_t* num_inliers,
                                      uint8_t* success, uint8_t* inlier_mask /* [M] or NULL */);
 
+/* ---- SIFT feature extraction (callable without an image set) -------------------------- */
+
+/* SiftExtractionOptions (R:pipeline/extract_features.h:78-139; defaults U:feature/sift.h, the C++ constructor's).
+ * pycolmap.Sift() overrides peak_threshold = 0.01, first_octave = 0, max_image_size = 7000 (R:pycolmap/feature/sift.h:
+ * 99-102); the host module sets those.  The covariant path (estimate_affine_shape, domain_size_pooling) and SiftGPU's
+ * darkness_adaptivity have no implementation here: a nonzero value is B2M_EINVAL. */
+#define B2M_NORMALIZATION_L1_ROOT 0
+#define B2M_NORMALIZATION_L2 1
+typedef struct b2m_extract_opts {
+  uint32_t struct_size;
+  int32_t max_image_size;        /* 3200: larger images are B2M_EINVAL (pycolmap's Sift.extract does not resize) */
+  int32_t max_num_features;      /* 8192 */
+  int32_t first_octave;          /* -1 */
+  int32_t num_octaves;           /* 4 */
+  int32_t octave_resolution;     /* 3 */
+  double peak_threshold;         /* 0.02 / 3 */
+  double edge_threshold;         /* 10 */
+  int32_t max_num_orientations;  /* 2 */
+  int32_t upright;               /* 0 */
+  int32_t normalization;         /* B2M_NORMALIZATION_L1_ROOT */
+  int32_t estimate_affine_shape; /* 0 */
+  int32_t domain_size_pooling;   /* 0 */
+  int32_t darkness_adaptivity;   /* 0 */
+} b2m_extract_opts;
+
+void b2m_extract_opts_default(b2m_extract_opts* o);
+
+/* One grey image: row-major uint8, `stride` bytes between rows (>= width). */
+typedef struct b2m_image {
+  int32_t width, height;
+  int64_t stride;
+  const uint8_t* data;
+} b2m_image;
+
+typedef struct b2m_features b2m_features;
+
+typedef struct b2m_feature_view {
+  uint32_t struct_size;
+  int32_t reserved;
+  int64_t n;                     /* features of the image */
+  const float* keypoints;        /* [n x 4] (x, y, scale, orientation): x, y with pixel centres at +0.5, orientation in
+                                  * (-pi, pi] (FeatureKeypoint::ComputeScale / ComputeOrientation) */
+  const uint8_t* descriptors;    /* [n x 128] uint8, UBC layout */
+} b2m_feature_view;
+
+/* Replaces SiftCPUFeatureExtractor::Extract (U:feature/sift.cc; VLFeat's vl_sift) as pycolmap.Sift.extract calls it
+ * (R:pycolmap/feature/sift.h:41-80), over `n` images.  Output order per image: octave ascending, then VLFeat's
+ * detection scan order (level, y, x), the orientations of one keypoint consecutive; the max_num_features cut keeps
+ * whole (octave, level) runs from the coarsest down, the run that passes the limit included.  Deterministic, and
+ * independent of the other images of the call.  *out is owned by the caller until b2m_features_free. */
+int b2m_extract_features_batch(b2m_ctx* ctx, const b2m_image* images, int32_t n, const b2m_extract_opts* opts,
+                               b2m_features** out);
+int b2m_features_get(const b2m_features* f, int32_t image, b2m_feature_view* out);
+void b2m_features_free(b2m_features* f);
+
 /* ---- instrumentation ---------------------------------------------------------------- */
 
 /* The cross-check consults m21 only at the columns some row matched (m21[m12[i]]): the column-direction GEMM is run
@@ -462,6 +517,9 @@ typedef struct b2m_stats {
   uint64_t abs_pose_residuals;        /* absolute pose: residual evaluations (models scored x correspondences) */
   uint64_t tri_models_scored;         /* triangulation: two-view and LO models scored against all observations */
   uint64_t tri_residuals;             /* triangulation: residual evaluations (models scored x observations of the track) */
+  uint64_t sift_images;               /* SIFT extraction: images processed since reset */
+  uint64_t sift_keypoints;            /* SIFT extraction: keypoints kept after the max_num_features cut */
+  uint64_t sift_descriptors;          /* SIFT extraction: descriptors computed (keypoints x orientations) */
 } b2m_stats;
 int b2m_get_stats(b2m_ctx* ctx, b2m_stats* out);
 int b2m_reset_stats(b2m_ctx* ctx);

@@ -18,6 +18,7 @@ try:
                         absolute_pose_estimation, estimate_absolute_poses, pose_refinement)
     from ._core import (EstimateTriangulationOptions, PointData, estimate_triangulation,  # noqa: F401
                         estimate_triangulations)
+    from ._core import Normalization, Sift, SiftExtractionOptions  # noqa: F401
     from ._core import (Context, Database, DatabaseTransaction, Device, ExhaustiveMatchingOptions,  # noqa: F401
                         RANSACOptions, Results, Rigid3d, Rotation3d, SequentialMatchingOptions,
                         SiftMatchingOptions, SpatialMatchingOptions, TwoViewGeometry,

@@ -855,6 +855,7 @@ void b2m_destroy(b2m_ctx* ctx) {
   if (ctx->d_verify_counters) cudaFree(ctx->d_verify_counters);
   if (ctx->d_abs_counters) cudaFree(ctx->d_abs_counters);
   tri_release(ctx);
+  sift_release(ctx);
   ctx->images.release();
   ctx->ws.release();
   verify_release(ctx);

@@ -122,6 +122,7 @@ struct b2m_ctx {
   unsigned long long* d_verify_counters = nullptr;  // [6]: models scored / residual evaluations per kind (verify.cu)
   unsigned long long* d_abs_counters = nullptr;     // [2]: models scored / residual evaluations (abs_pose.cu)
   void* tri_state = nullptr;     // b2m::TriState (triangulation.cu): pinned staging, device buffers, counters
+  void* sift_state = nullptr;    // b2m::SiftState (sift.cu): pyramid, gradient and keypoint buffers
 };
 
 namespace b2m {
@@ -129,6 +130,8 @@ namespace b2m {
 void tri_release(b2m_ctx* ctx);
 bool tri_counters(b2m_ctx* ctx, unsigned long long* out);  // [2]: models scored, residual evaluations
 void tri_reset_counters(b2m_ctx* ctx);
+// sift.cu
+void sift_release(b2m_ctx* ctx);
 }  // namespace b2m
 
 namespace b2m {

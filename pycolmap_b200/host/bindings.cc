@@ -556,6 +556,145 @@ py::dict EstimateTriangulationsPy(const std::function<b2m_ctx*()>& get_ctx, cons
   return d;
 }
 
+// ---- SIFT extraction (R:pycolmap/feature/sift.h, R:pipeline/extract_features.h:63-139) ------------------------------
+// Bound at run time like the triangulation entry point: the host references no C ABI version 6 symbol at link time.
+template <typename F>
+F SiftSymbol(const char* name) {
+  static void* handle = []() -> void* {
+    Dl_info info;
+    if (dladdr(reinterpret_cast<void*>(&b2m_abi_version), &info) && info.dli_fname)
+      return dlopen(info.dli_fname, RTLD_NOW | RTLD_NOLOAD);
+    return nullptr;
+  }();
+  void* p = handle ? dlsym(handle, name) : nullptr;
+  if (!p)
+    throw std::runtime_error(std::string("[bindings.cc] libb200match.so does not export ") + name +
+                             " (C ABI version 6): rebuild it");
+  return reinterpret_cast<F>(p);
+}
+
+// SiftExtractionOptions::Check (U:feature/sift.cc); the options without a path here are refused, not ignored.
+void CheckSiftOptions(const SiftExtractionOptions& o) {
+  auto fail = [](const std::string& what) { throw std::invalid_argument("[sift.cc] Check Failed: " + what); };
+  if (!(o.max_image_size > 0)) fail("max_image_size > 0");
+  if (!(o.max_num_features > 0)) fail("max_num_features > 0");
+  if (!(o.octave_resolution > 0)) fail("octave_resolution > 0");
+  if (!(o.peak_threshold > 0.0)) fail("peak_threshold > 0");
+  if (!(o.edge_threshold > 0.0)) fail("edge_threshold > 0");
+  if (!(o.max_num_orientations > 0)) fail("max_num_orientations > 0");
+  if (o.domain_size_pooling) {
+    if (!(o.dsp_min_scale > 0)) fail("dsp_min_scale > 0");
+    if (!(o.dsp_max_scale >= o.dsp_min_scale)) fail("dsp_max_scale >= dsp_min_scale");
+    if (!(o.dsp_num_scales > 0)) fail("dsp_num_scales > 0");
+  }
+  auto unsupported = [](const std::string& what) {
+    throw std::invalid_argument("[bindings.cc] Check Failed: " + what + " is not supported (no GPU path)");
+  };
+  if (!(o.num_octaves > 0)) unsupported("num_octaves <= 0");
+  if (!(o.first_octave >= -3 && o.first_octave <= 16)) unsupported("first_octave outside [-3, 16]");
+  if (o.estimate_affine_shape) unsupported("estimate_affine_shape");
+  if (o.domain_size_pooling) unsupported("domain_size_pooling");
+  if (o.darkness_adaptivity) unsupported("darkness_adaptivity");
+}
+
+// IsGPU / VerifyGPUParams (R:utils.h:11-31) for one extractor: Device.cpu is refused, gpu_index names one device.
+int SiftDevice(Device device, const SiftExtractionOptions& o) {
+  if (device == Device::CPU)
+    throw std::invalid_argument("[bindings.cc] pycolmap_b200 has no CPU path: use Device.auto or Device.cuda");
+  if (o.gpu_index.find(',') != std::string::npos)
+    throw std::invalid_argument("[bindings.cc] Check Failed: Sift runs on one GPU: gpu_index is a single index, got \"" +
+                                o.gpu_index + "\"");
+  int v;
+  try {
+    v = std::stoi(o.gpu_index);
+  } catch (const std::exception&) {
+    throw std::invalid_argument("[bindings.cc] Check Failed: gpu_index is an integer, got \"" + o.gpu_index + "\"");
+  }
+  if (v < -1) throw std::invalid_argument("[bindings.cc] Check Failed: gpu_index >= -1");
+  return v < 0 ? 0 : v;
+}
+
+struct Sift {
+  SiftExtractionOptions options;
+  Device device = Device::AUTO;
+};
+
+// A 2-D uint8 or float32 array -> a packed uint8 copy; float32 goes through (x * 255) cast to uint8 like
+// R:pycolmap/feature/sift.h:82-85, after a range check (upstream's cast is undefined outside [0, 1]).
+std::vector<uint8_t> ImageToU8(const py::handle& obj, int max_image_size, int* w, int* h) {
+  if (!py::isinstance<py::array>(obj)) throw py::type_error("Sift.extract: image is a 2-D numpy array of uint8 or float32");
+  const py::array a = py::reinterpret_borrow<py::array>(obj);
+  const bool u8 = a.dtype().is(py::dtype::of<uint8_t>()), f32 = a.dtype().is(py::dtype::of<float>());
+  if (!u8 && !f32)
+    throw py::type_error("Sift.extract: image dtype must be uint8 or float32, got " + py::str(a.dtype()).cast<std::string>());
+  if (a.ndim() != 2) throw std::invalid_argument("[bindings.cc] Check Failed: image.ndim() == 2");
+  const int64_t rows = a.shape(0), cols = a.shape(1);
+  if (rows == 0 || cols == 0) throw std::invalid_argument("[bindings.cc] Check Failed: image is not empty");
+  if (rows > max_image_size)
+    throw std::invalid_argument("[sift.h:42] Check Failed: image.rows() <= options_.max_image_size (" + std::to_string(rows) +
+                                " vs. " + std::to_string(max_image_size) + ")");
+  if (cols > max_image_size)
+    throw std::invalid_argument("[sift.h:43] Check Failed: image.cols() <= options_.max_image_size (" + std::to_string(cols) +
+                                " vs. " + std::to_string(max_image_size) + ")");
+  *w = static_cast<int>(cols);
+  *h = static_cast<int>(rows);
+  std::vector<uint8_t> out(static_cast<size_t>(rows * cols));
+  if (u8) {
+    const auto v = py::array_t<uint8_t, py::array::c_style | py::array::forcecast>::ensure(a);
+    std::memcpy(out.data(), v.data(), out.size());
+  } else {
+    const auto v = py::array_t<float, py::array::c_style | py::array::forcecast>::ensure(a);
+    const float* p = v.data();
+    for (size_t i = 0; i < out.size(); ++i) {
+      if (!(p[i] >= 0.0f && p[i] <= 1.0f))
+        throw std::invalid_argument("[bindings.cc] Check Failed: float32 image values are finite and in [0, 1]");
+      out[i] = static_cast<uint8_t>(p[i] * 255.0f);
+    }
+  }
+  return out;
+}
+
+// One ABI call over all images; each result is (keypoints (N, 4) float32, descriptors (N, 128) float32 = u8 / 512).
+py::list ExtractBatch(const Sift& s, const py::sequence& images) {
+  CheckSiftOptions(s.options);
+  const int dev = SiftDevice(s.device, s.options);
+  const size_t n = images.size();
+  std::vector<std::vector<uint8_t>> px(n);
+  std::vector<b2m_image> im(n);
+  for (size_t i = 0; i < n; ++i) {
+    int w = 0, h = 0;
+    px[i] = ImageToU8(images[i], s.options.max_image_size, &w, &h);
+    im[i] = b2m_image{w, h, w, px[i].data()};
+  }
+  const auto extract = SiftSymbol<decltype(&b2m_extract_features_batch)>("b2m_extract_features_batch");
+  const auto get = SiftSymbol<decltype(&b2m_features_get)>("b2m_features_get");
+  const auto release = SiftSymbol<decltype(&b2m_features_free)>("b2m_features_free");
+  b2m_ctx* ctx = Engine::Get(dev);
+  const b2m_extract_opts o = ToAbi(s.options);
+  b2m_features* f = nullptr;
+  int rc;
+  {
+    py::gil_scoped_release release_gil;
+    rc = extract(ctx, im.data(), static_cast<int32_t>(n), &o, &f);
+  }
+  ThrowOnError(ctx, rc);
+  std::unique_ptr<b2m_features, decltype(release)> guard(f, release);
+  py::list out;
+  for (size_t i = 0; i < n; ++i) {
+    b2m_feature_view v;
+    std::memset(&v, 0, sizeof(v));
+    v.struct_size = sizeof(v);
+    ThrowOnError(ctx, get(f, static_cast<int32_t>(i), &v));
+    py::array_t<float> kp(std::vector<py::ssize_t>{static_cast<py::ssize_t>(v.n), 4});
+    py::array_t<float> desc(std::vector<py::ssize_t>{static_cast<py::ssize_t>(v.n), 128});
+    if (v.n) std::memcpy(kp.mutable_data(), v.keypoints, sizeof(float) * 4 * v.n);
+    float* d = desc.mutable_data();
+    for (int64_t k = 0; k < 128 * v.n; ++k) d[k] = static_cast<float>(v.descriptors[k]) / 512.0f;
+    out.append(py::make_tuple(kp, desc));
+  }
+  return out;
+}
+
 }  // namespace
 
 PYBIND11_MODULE(_core, m) {
@@ -1070,6 +1209,69 @@ PYBIND11_MODULE(_core, m) {
         "options"_a = EstimateTriangulationOptions(),
         "Batched estimate_triangulation over T tracks stored back to back: returns dict(xyz (T, 3), NaN rows on failure; "
         "success (T,); num_inliers (T,); inliers (M,))");
+  // ---- SIFT extraction ----
+  auto normalization = py::enum_<Normalization>(m, "Normalization")
+                           .value("L1_ROOT", Normalization::L1_ROOT,
+                                  "L1-normalizes each descriptor followed by element-wise square rooting.")
+                           .value("L2", Normalization::L2, "Each vector is L2-normalized.");
+  AddStringConstructor(normalization);
+  OptionsClass<SiftExtractionOptions>(m, "SiftExtractionOptions")
+      .field("num_threads", &SiftExtractionOptions::num_threads, "Number of threads (accepted; extraction runs on the GPU).")
+      .field("gpu_index", &SiftExtractionOptions::gpu_index, "Index of the GPU used for feature extraction (one index).")
+      .field("max_image_size", &SiftExtractionOptions::max_image_size,
+             "Maximum image size; Sift.extract refuses larger images (it does not resize).")
+      .field("max_num_features", &SiftExtractionOptions::max_num_features,
+             "Maximum number of features to detect, keeping larger-scale features.")
+      .field("first_octave", &SiftExtractionOptions::first_octave,
+             "First octave in the pyramid, i.e. -1 upsamples the image by one level.")
+      .field("num_octaves", &SiftExtractionOptions::num_octaves)
+      .field("octave_resolution", &SiftExtractionOptions::octave_resolution, "Number of levels per octave.")
+      .field("peak_threshold", &SiftExtractionOptions::peak_threshold, "Peak threshold for detection.")
+      .field("edge_threshold", &SiftExtractionOptions::edge_threshold, "Edge threshold for detection.")
+      .field("estimate_affine_shape", &SiftExtractionOptions::estimate_affine_shape,
+             "Estimate affine shape of SIFT features (not supported: True is refused).")
+      .field("max_num_orientations", &SiftExtractionOptions::max_num_orientations,
+             "Maximum number of orientations per keypoint.")
+      .field("upright", &SiftExtractionOptions::upright, "Fix the orientation to 0 for upright features")
+      .field("darkness_adaptivity", &SiftExtractionOptions::darkness_adaptivity,
+             "SiftGPU-only upstream (not supported: True is refused).")
+      .field("domain_size_pooling", &SiftExtractionOptions::domain_size_pooling,
+             "Domain-size pooling (not supported: True is refused).")
+      .field("dsp_min_scale", &SiftExtractionOptions::dsp_min_scale)
+      .field("dsp_max_scale", &SiftExtractionOptions::dsp_max_scale)
+      .field("dsp_num_scales", &SiftExtractionOptions::dsp_num_scales)
+      .field("normalization", &SiftExtractionOptions::normalization, "L1_ROOT or L2 descriptor normalization")
+      .Finish();
+  {
+    SiftExtractionOptions pycolmap_defaults;  // R:pycolmap/feature/sift.h:99-102
+    pycolmap_defaults.peak_threshold = 0.01;
+    pycolmap_defaults.first_octave = 0;
+    pycolmap_defaults.max_image_size = 7000;
+    py::class_<Sift>(m, "Sift")
+        .def(py::init([](const SiftExtractionOptions& options, Device device) {
+               CheckSiftOptions(options);
+               SiftDevice(device, options);
+               return Sift{options, device};
+             }),
+             "options"_a = pycolmap_defaults, "device"_a = Device::AUTO)
+        .def("extract",
+             [](const Sift& s, const py::object& image) {
+               py::list one;
+               one.append(image);
+               const py::list r = ExtractBatch(s, one);
+               return py::object(r[0]);
+             },
+             "image"_a,
+             "SIFT features of a 2-D uint8 or float32 image: (keypoints (N, 4) [x, y, scale, orientation], "
+             "descriptors (N, 128) float32 = uint8 / 512)")
+        .def("extract_batch", &ExtractBatch, "images"_a,
+             "Sift.extract over a list of images in one GPU call; a list of (keypoints, descriptors)")
+        .def_property_readonly("options", [](const Sift& s) { return s.options; })
+        .def_property_readonly(
+            "device", [](const Sift&) { return Device::CUDA; },
+            "The device the extractor runs on, resolved like upstream's Sift::GetDevice (use_gpu ? CUDA : CPU): always "
+            "Device.cuda, since Device.auto resolves to the GPU and Device.cpu is refused.");
+  }
   m.def("fundamental_matrix_estimation",
         [](const ArrD& points1, const ArrD& points2, const RANSACOptions& estimation_options) {
           CheckSameLength(points1, points2, "fundamental_matrix.h:22");
@@ -1601,7 +1803,9 @@ PYBIND11_MODULE(_core, m) {
                         "verify_residuals"_a = py::make_tuple(s.verify_residuals[0], s.verify_residuals[1],
                                                               s.verify_residuals[2]),
                         "comm_size"_a = s.comm_size, "comm_rank"_a = s.comm_rank,
-                        "tri_models_scored"_a = s.tri_models_scored, "tri_residuals"_a = s.tri_residuals);
+                        "tri_models_scored"_a = s.tri_models_scored, "tri_residuals"_a = s.tri_residuals,
+                        "sift_images"_a = s.sift_images, "sift_keypoints"_a = s.sift_keypoints,
+                        "sift_descriptors"_a = s.sift_descriptors);
       })
       .def("reset_stats", [](CoreContext& c) { ThrowOnError(c.Handle(), b2m_reset_stats(c.Handle()));
       });

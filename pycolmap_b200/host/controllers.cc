@@ -64,6 +64,27 @@ b2m_abs_pose_opts ToAbi(const AbsolutePoseEstimationOptions& o) {
   return r;
 }
 
+// Filled field by field for the same reason (C ABI version 6).
+b2m_extract_opts ToAbi(const SiftExtractionOptions& o) {
+  b2m_extract_opts r;
+  memset(&r, 0, sizeof(r));
+  r.struct_size = sizeof(r);
+  r.max_image_size = o.max_image_size;
+  r.max_num_features = o.max_num_features;
+  r.first_octave = o.first_octave;
+  r.num_octaves = o.num_octaves;
+  r.octave_resolution = o.octave_resolution;
+  r.peak_threshold = o.peak_threshold;
+  r.edge_threshold = o.edge_threshold;
+  r.max_num_orientations = o.max_num_orientations;
+  r.upright = o.upright;
+  r.normalization = o.normalization == Normalization::L2 ? B2M_NORMALIZATION_L2 : B2M_NORMALIZATION_L1_ROOT;
+  r.estimate_affine_shape = o.estimate_affine_shape;
+  r.domain_size_pooling = o.domain_size_pooling;
+  r.darkness_adaptivity = o.darkness_adaptivity;
+  return r;
+}
+
 // Filled field by field for the same reason (C ABI version 5).
 b2m_tri_opts ToAbi(const EstimateTriangulationOptions& o) {
   b2m_tri_opts r;

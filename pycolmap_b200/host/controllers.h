@@ -109,7 +109,31 @@ struct EstimateTriangulationOptions {
   RANSACOptions ransac{4.0, 0.01, 0.9999, 3.0, 1000, 100000};
 };
 
+// SiftExtractionOptions with the C++ constructor's defaults (R:pipeline/extract_features.h:78-139; U:feature/sift.h).
+enum class Normalization { L1_ROOT = 0, L2 = 1 };
+struct SiftExtractionOptions {
+  int num_threads = -1;
+  std::string gpu_index = "-1";
+  int max_image_size = 3200;
+  int max_num_features = 8192;
+  int first_octave = -1;
+  int num_octaves = 4;
+  int octave_resolution = 3;
+  double peak_threshold = 0.02 / 3;
+  double edge_threshold = 10.0;
+  bool estimate_affine_shape = false;
+  int max_num_orientations = 2;
+  bool upright = false;
+  bool darkness_adaptivity = false;
+  bool domain_size_pooling = false;
+  double dsp_min_scale = 1.0 / 6;
+  double dsp_max_scale = 3.0;
+  int dsp_num_scales = 10;
+  Normalization normalization = Normalization::L1_ROOT;
+};
+
 b2m_sift_opts ToAbi(const SiftMatchingOptions& o);
+b2m_extract_opts ToAbi(const SiftExtractionOptions& o);
 b2m_tri_opts ToAbi(const EstimateTriangulationOptions& o);
 b2m_abs_pose_opts ToAbi(const AbsolutePoseEstimationOptions& o);
 b2m_pose_refine_opts ToAbi(const AbsolutePoseRefinementOptions& o);

@@ -135,3 +135,50 @@ def make_scene(n_images, n_feat, seed=0, device="cpu", window_images=24.0, vis_f
     cams = [dict(model=0, width=width, height=height, params=[focal, cx, cy], has_prior_focal_length=1)
             for _ in range(n_out)]
     return dict(desc=desc, kpts=kpts, point_id=pid, cameras=cams)
+
+
+def textured_plane(rng, size=1024, octaves=(4, 8, 16, 32, 64)):
+    """Seeded band-limited random texture in [0, 1]: a sum of bilinearly upsampled white-noise grids (one per
+    period in pixels), so it has blob-like structure at every scale SIFT looks at."""
+    tex = np.zeros((size, size))
+    for period in octaves:
+        n = size // period + 2
+        g = rng.random((n, n))
+        t = (np.arange(size) + 0.5) / period
+        i = np.floor(t).astype(np.int64)
+        f = t - i
+        rows = g[i] * (1 - f)[:, None] + g[i + 1] * f[:, None]
+        tex += rows[:, i] * (1 - f)[None, :] + rows[:, i + 1] * f[None, :]
+    tex -= tex.min()
+    return tex / tex.max()
+
+
+def render_view(texture, H, width, height):
+    """uint8 view of the texture plane through the homography H (texture pixel coordinates -> view pixel
+    coordinates, both with pixel centres at +0.5, COLMAP's keypoint convention): bilinear sampling, clamped at the
+    texture border, quantised to uint8."""
+    ys, xs = np.mgrid[0:height, 0:width]
+    p = np.stack([xs.ravel() + 0.5, ys.ravel() + 0.5, np.ones(xs.size)])
+    q = np.linalg.solve(H, p)
+    u = np.clip(q[0] / q[2] - 0.5, 0, texture.shape[1] - 1.000001)
+    v = np.clip(q[1] / q[2] - 0.5, 0, texture.shape[0] - 1.000001)
+    i, j = np.floor(v).astype(np.int64), np.floor(u).astype(np.int64)
+    fv, fu = v - i, u - j
+    val = (texture[i, j] * (1 - fu) * (1 - fv) + texture[i, j + 1] * fu * (1 - fv)
+           + texture[i + 1, j] * (1 - fu) * fv + texture[i + 1, j + 1] * fu * fv)
+    return np.clip(np.round(255.0 * val), 0, 255).astype(np.uint8).reshape(height, width)
+
+
+def homography_pair(rng, width, height, size=1024):
+    """Two rendered views of one textured plane and the planted homography from view 1 to view 2 (pixel
+    coordinates with centres at +0.5)."""
+    tex = textured_plane(rng, size)
+    s = 0.8 * min(width, height) / size
+    H1 = np.array([[s, 0.0, 0.1 * width], [0.0, s, 0.1 * height], [0.0, 0.0, 1.0]])
+    a = 0.15
+    R = np.array([[np.cos(a), -np.sin(a), 0.0], [np.sin(a), np.cos(a), 0.0], [0.0, 0.0, 1.0]])
+    P = np.array([[1.0, 0.0, 0.0], [0.0, 1.0, 0.0], [1e-4 / max(width, height) * 100, 0.0, 1.0]])
+    c = np.array([[1.0, 0.0, width / 2], [0.0, 1.0, height / 2], [0.0, 0.0, 1.0]])
+    H12 = c @ P @ R @ np.linalg.inv(c)
+    H2 = H12 @ H1
+    return render_view(tex, H1, width, height), render_view(tex, H2, width, height), H12
