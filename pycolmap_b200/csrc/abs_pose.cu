@@ -1268,45 +1268,6 @@ __global__ void __launch_bounds__(32) b2m_abs_refine_kernel(const RefineParams P
   }
 }
 
-#define A_TRY(ctx, expr)                                                                    \
-  do {                                                                                      \
-    cudaError_t _e = (expr);                                                                \
-    if (_e != cudaSuccess) {                                                                \
-      char _b[512];                                                                         \
-      snprintf(_b, sizeof(_b), "[%s:%d] CUDA error: %s (%s)", __FILE__, __LINE__,          \
-               cudaGetErrorString(_e), #expr);                                              \
-      (ctx)->err = _b;                                                                      \
-      return _e == cudaErrorMemoryAllocation ? B2M_ENOMEM : B2M_ECUDA;                      \
-    }                                                                                       \
-  } while (0)
-
-// Device buffers of one chunk of problems; freed on scope exit.
-struct Bufs {
-  std::vector<void*> ptrs;
-  ~Bufs() {
-    for (void* p : ptrs) cudaFree(p);
-  }
-  template <class T>
-  cudaError_t alloc(T** p, size_t count) {
-    *p = nullptr;
-    const cudaError_t e = cudaMalloc(reinterpret_cast<void**>(p), sizeof(T) * std::max<size_t>(count, 1));
-    if (e == cudaSuccess) ptrs.push_back(*p);
-    return e;
-  }
-};
-
-unsigned long long* abs_counters(b2m_ctx* ctx) {
-  if (!ctx->d_abs_counters) {
-    if (cudaMalloc(&ctx->d_abs_counters, sizeof(unsigned long long) * 2) != cudaSuccess) {
-      cudaGetLastError();
-      ctx->d_abs_counters = nullptr;
-      return nullptr;
-    }
-    cudaMemset(ctx->d_abs_counters, 0, sizeof(unsigned long long) * 2);
-  }
-  return ctx->d_abs_counters;
-}
-
 // Packed host copies of a chunk [k0, k0 + nb) of the problems.
 struct Packed {
   std::vector<double> px, p3, centroid;
@@ -1370,25 +1331,24 @@ const char* check_refine_opts(const b2m_pose_refine_opts* r) {
   return nullptr;
 }
 
-int launch_refine(b2m_ctx* ctx, Bufs& B, const Packed& H, int nb, const double* d_px, const double* d_p3, const int64_t* d_off,
+// d_model and d_cov (left empty unless want_cov) belong to the caller's chunk: the kernel reads them after the return.
+int launch_refine(b2m_ctx* ctx, const Packed& H, int nb, const double* d_px, const double* d_p3, const int64_t* d_off,
                   const int32_t* d_cnt, const uint8_t* d_mask, double* d_pose, double* d_params, int32_t* d_success,
-                  const b2m_pose_refine_opts* r, int want_cov, double** d_cov) {
-  int32_t* d_model = nullptr;
-  *d_cov = nullptr;
-  A_TRY(ctx, B.alloc(&d_model, nb));
-  A_TRY(ctx, cudaMemcpyAsync(d_model, H.model.data(), sizeof(int32_t) * nb, cudaMemcpyHostToDevice, ctx->stream));
-  if (want_cov) A_TRY(ctx, B.alloc(d_cov, 36 * static_cast<size_t>(nb)));
-  if (want_cov) A_TRY(ctx, cudaMemsetAsync(*d_cov, 0, sizeof(double) * 36 * nb, ctx->stream));
+                  const b2m_pose_refine_opts* r, int want_cov, DeviceArray<int32_t>& d_model, DeviceArray<double>& d_cov) {
+  B2M_CUDA_TRY(ctx, d_model.ensure(nb));
+  B2M_CUDA_TRY(ctx, cudaMemcpyAsync(d_model, H.model.data(), sizeof(int32_t) * nb, cudaMemcpyHostToDevice, ctx->stream));
+  if (want_cov) B2M_CUDA_TRY(ctx, d_cov.ensure(36 * static_cast<size_t>(nb)));
+  if (want_cov) B2M_CUDA_TRY(ctx, cudaMemsetAsync(d_cov, 0, sizeof(double) * 36 * nb, ctx->stream));
   RefineParams Q{};
   Q.px = d_px; Q.p3 = d_p3; Q.off = d_off; Q.cnt = d_cnt; Q.model = d_model; Q.mask = d_mask;
-  Q.pose = d_pose; Q.params = d_params; Q.success = d_success; Q.cov = *d_cov;
+  Q.pose = d_pose; Q.params = d_params; Q.success = d_success; Q.cov = d_cov;
   Q.gradient_tolerance = r->gradient_tolerance;
   Q.loss_scale = r->loss_function_scale;
   Q.max_num_iterations = r->max_num_iterations;
   Q.refine_focal = r->refine_focal_length;
   Q.refine_extra = r->refine_extra_params;
   b2m_abs_refine_kernel<<<nb, 32, 0, ctx->stream>>>(Q);
-  A_TRY(ctx, cudaGetLastError());
+  B2M_CUDA_TRY(ctx, cudaGetLastError());
   ctx->stats.kernel_launches += 1;
   return B2M_OK;
 }
@@ -1444,24 +1404,20 @@ int b2m_estimate_absolute_pose_batch(b2m_ctx* ctx, const b2m_abs_pose_problem* p
                                      const b2m_abs_pose_opts* opts, const b2m_pose_refine_opts* refine,
                                      int32_t want_covariance, b2m_abs_pose_result* out, uint8_t* const* inlier_masks) {
   if (!ctx) return B2M_EINVAL;
-  auto bad = [&](const char* msg) {
-    ctx->err = msg;
-    return B2M_EINVAL;
-  };
   if (n_problems < 0 || (n_problems > 0 && (!problems || !out)) || !opts)
-    return bad("[abs_pose.cu] Check Failed: problems, options and out != NULL");
+    return fail(ctx, B2M_EINVAL, "[abs_pose.cu] Check Failed: problems, options and out != NULL");
   if (opts->struct_size != sizeof(b2m_abs_pose_opts))
-    return bad("[abs_pose.cu] Check Failed: b2m_abs_pose_opts.struct_size == sizeof(b2m_abs_pose_opts)");
+    return fail(ctx, B2M_EINVAL, "[abs_pose.cu] Check Failed: b2m_abs_pose_opts.struct_size == sizeof(b2m_abs_pose_opts)");
   // AbsolutePoseEstimationOptions::Check (U:estimators/pose.h)
-  if (opts->num_focal_length_samples <= 0) return bad("[pose.h] Check Failed: num_focal_length_samples > 0");
-  if (!(opts->min_focal_length_ratio > 0)) return bad("[pose.h] Check Failed: min_focal_length_ratio > 0");
-  if (!(opts->max_focal_length_ratio > 0)) return bad("[pose.h] Check Failed: max_focal_length_ratio > 0");
+  if (opts->num_focal_length_samples <= 0) return fail(ctx, B2M_EINVAL, "[pose.h] Check Failed: num_focal_length_samples > 0");
+  if (!(opts->min_focal_length_ratio > 0)) return fail(ctx, B2M_EINVAL, "[pose.h] Check Failed: min_focal_length_ratio > 0");
+  if (!(opts->max_focal_length_ratio > 0)) return fail(ctx, B2M_EINVAL, "[pose.h] Check Failed: max_focal_length_ratio > 0");
   if (!(opts->min_focal_length_ratio < opts->max_focal_length_ratio))
-    return bad("[pose.h] Check Failed: min_focal_length_ratio < max_focal_length_ratio");
-  if (!(opts->ransac.max_error > 0)) return bad("[ransac.h] Check Failed: max_error > 0");
+    return fail(ctx, B2M_EINVAL, "[pose.h] Check Failed: min_focal_length_ratio < max_focal_length_ratio");
+  if (!(opts->ransac.max_error > 0)) return fail(ctx, B2M_EINVAL, "[ransac.h] Check Failed: max_error > 0");
   if (refine)
-    if (const char* why = check_refine_opts(refine)) return bad(why);
-  if (const char* why = check_problems(problems, n_problems)) return bad(why);
+    if (const char* why = check_refine_opts(refine)) return fail(ctx, B2M_EINVAL, why);
+  if (const char* why = check_problems(problems, n_problems)) return fail(ctx, B2M_EINVAL, why);
   cudaSetDevice(ctx->device);
   cudaStream_t st = ctx->stream;
   std::vector<double> factors;
@@ -1496,76 +1452,74 @@ int b2m_estimate_absolute_pose_batch(b2m_ctx* ctx, const b2m_abs_pose_problem* p
         xoff[static_cast<size_t>(k) * nf + f] = pos;
         pos += H.cnt[k];
       }
-    Bufs B;
-    double *d_px, *d_p3, *d_cent, *d_models, *d_fac, *d_pose, *d_params;
-    int64_t *d_off, *d_xoff;
-    int32_t *d_cnt, *d_sup, *d_succ, *d_osucc, *d_oinl, *d_ofac;
-    DevCam* d_cams;
-    double2* d_xn;
-    uint8_t *d_cmask, *d_mask;
+    DeviceArray<double> d_px, d_p3, d_cent, d_models, d_fac, d_pose, d_params, d_cov;
+    DeviceArray<int64_t> d_off, d_xoff;
+    DeviceArray<int32_t> d_cnt, d_sup, d_succ, d_osucc, d_oinl, d_ofac, d_model;
+    DeviceArray<DevCam> d_cams;
+    DeviceArray<double2> d_xn;
+    DeviceArray<uint8_t> d_cmask, d_mask;
     const size_t nc = static_cast<size_t>(nb) * nf;
-    A_TRY(ctx, B.alloc(&d_px, 2 * H.total));
-    A_TRY(ctx, B.alloc(&d_p3, 3 * H.total));
-    A_TRY(ctx, B.alloc(&d_cent, 3 * static_cast<size_t>(nb)));
-    A_TRY(ctx, B.alloc(&d_models, 12 * nc));
-    A_TRY(ctx, B.alloc(&d_fac, nf));
-    A_TRY(ctx, B.alloc(&d_pose, 7 * static_cast<size_t>(nb)));
-    A_TRY(ctx, B.alloc(&d_params, 12 * static_cast<size_t>(nb)));
-    A_TRY(ctx, B.alloc(&d_off, nb));
-    A_TRY(ctx, B.alloc(&d_xoff, nc));
-    A_TRY(ctx, B.alloc(&d_cnt, nb));
-    A_TRY(ctx, B.alloc(&d_sup, nc));
-    A_TRY(ctx, B.alloc(&d_succ, nc));
-    A_TRY(ctx, B.alloc(&d_osucc, nb));
-    A_TRY(ctx, B.alloc(&d_oinl, nb));
-    A_TRY(ctx, B.alloc(&d_ofac, nb));
-    A_TRY(ctx, B.alloc(&d_cams, nb));
-    A_TRY(ctx, B.alloc(&d_xn, pos));
-    A_TRY(ctx, B.alloc(&d_cmask, pos));
-    A_TRY(ctx, B.alloc(&d_mask, H.total));
+    B2M_CUDA_TRY(ctx, d_px.ensure(2 * H.total));
+    B2M_CUDA_TRY(ctx, d_p3.ensure(3 * H.total));
+    B2M_CUDA_TRY(ctx, d_cent.ensure(3 * static_cast<size_t>(nb)));
+    B2M_CUDA_TRY(ctx, d_models.ensure(12 * nc));
+    B2M_CUDA_TRY(ctx, d_fac.ensure(nf));
+    B2M_CUDA_TRY(ctx, d_pose.ensure(7 * static_cast<size_t>(nb)));
+    B2M_CUDA_TRY(ctx, d_params.ensure(12 * static_cast<size_t>(nb)));
+    B2M_CUDA_TRY(ctx, d_off.ensure(nb));
+    B2M_CUDA_TRY(ctx, d_xoff.ensure(nc));
+    B2M_CUDA_TRY(ctx, d_cnt.ensure(nb));
+    B2M_CUDA_TRY(ctx, d_sup.ensure(nc));
+    B2M_CUDA_TRY(ctx, d_succ.ensure(nc));
+    B2M_CUDA_TRY(ctx, d_osucc.ensure(nb));
+    B2M_CUDA_TRY(ctx, d_oinl.ensure(nb));
+    B2M_CUDA_TRY(ctx, d_ofac.ensure(nb));
+    B2M_CUDA_TRY(ctx, d_cams.ensure(nb));
+    B2M_CUDA_TRY(ctx, d_xn.ensure(pos));
+    B2M_CUDA_TRY(ctx, d_cmask.ensure(pos));
+    B2M_CUDA_TRY(ctx, d_mask.ensure(H.total));
     if (H.total > 0) {
-      A_TRY(ctx, cudaMemcpyAsync(d_px, H.px.data(), sizeof(double) * 2 * H.total, cudaMemcpyHostToDevice, st));
-      A_TRY(ctx, cudaMemcpyAsync(d_p3, H.p3.data(), sizeof(double) * 3 * H.total, cudaMemcpyHostToDevice, st));
+      B2M_CUDA_TRY(ctx, cudaMemcpyAsync(d_px, H.px.data(), sizeof(double) * 2 * H.total, cudaMemcpyHostToDevice, st));
+      B2M_CUDA_TRY(ctx, cudaMemcpyAsync(d_p3, H.p3.data(), sizeof(double) * 3 * H.total, cudaMemcpyHostToDevice, st));
     }
-    A_TRY(ctx, cudaMemcpyAsync(d_cent, H.centroid.data(), sizeof(double) * 3 * nb, cudaMemcpyHostToDevice, st));
-    A_TRY(ctx, cudaMemcpyAsync(d_fac, factors.data(), sizeof(double) * nf, cudaMemcpyHostToDevice, st));
-    A_TRY(ctx, cudaMemcpyAsync(d_off, H.off.data(), sizeof(int64_t) * nb, cudaMemcpyHostToDevice, st));
-    A_TRY(ctx, cudaMemcpyAsync(d_xoff, xoff.data(), sizeof(int64_t) * nc, cudaMemcpyHostToDevice, st));
-    A_TRY(ctx, cudaMemcpyAsync(d_cnt, H.cnt.data(), sizeof(int32_t) * nb, cudaMemcpyHostToDevice, st));
-    A_TRY(ctx, cudaMemcpyAsync(d_cams, H.cams.data(), sizeof(DevCam) * nb, cudaMemcpyHostToDevice, st));
+    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(d_cent, H.centroid.data(), sizeof(double) * 3 * nb, cudaMemcpyHostToDevice, st));
+    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(d_fac, factors.data(), sizeof(double) * nf, cudaMemcpyHostToDevice, st));
+    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(d_off, H.off.data(), sizeof(int64_t) * nb, cudaMemcpyHostToDevice, st));
+    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(d_xoff, xoff.data(), sizeof(int64_t) * nc, cudaMemcpyHostToDevice, st));
+    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(d_cnt, H.cnt.data(), sizeof(int32_t) * nb, cudaMemcpyHostToDevice, st));
+    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(d_cams, H.cams.data(), sizeof(DevCam) * nb, cudaMemcpyHostToDevice, st));
     RansacParams P{};
     P.px = d_px; P.p3 = d_p3; P.centroid = d_cent; P.off = d_off; P.cnt = d_cnt; P.xoff = d_xoff; P.cams = d_cams;
     P.xn = d_xn; P.mask = d_cmask; P.models = d_models; P.sup = d_sup; P.success = d_succ;
     P.factors = d_fac; P.n_factors = nf; P.ro = opts->ransac; P.seed = ctx->seed; P.problem_base = k0;
-    P.counters = abs_counters(ctx);
+    P.counters = ctx->d_counters + kAbsPoseCounters;
     b2m_abs_ransac_kernel<<<static_cast<unsigned>(nc), kThreads, 0, st>>>(P);
-    A_TRY(ctx, cudaGetLastError());
+    B2M_CUDA_TRY(ctx, cudaGetLastError());
     SelectParams S{};
     S.off = d_off; S.cnt = d_cnt; S.xoff = d_xoff; S.cta_mask = d_cmask; S.models = d_models; S.sup = d_sup;
     S.success = d_succ; S.centroid = d_cent; S.factors = d_fac; S.n_factors = nf;
     S.estimate_focal_length = opts->estimate_focal_length; S.cams = d_cams; S.mask = d_mask; S.pose = d_pose;
     S.params = d_params; S.out_success = d_osucc; S.out_inliers = d_oinl; S.out_factor = d_ofac;
     b2m_abs_select_kernel<<<nb, 32, 0, st>>>(S);
-    A_TRY(ctx, cudaGetLastError());
+    B2M_CUDA_TRY(ctx, cudaGetLastError());
     ctx->stats.kernel_launches += 2;
-    double* d_cov = nullptr;
     if (refine)
-      if (int rc = launch_refine(ctx, B, H, nb, d_px, d_p3, d_off, d_cnt, d_mask, d_pose, d_params, d_osucc, refine,
-                                 want_covariance, &d_cov))
+      if (int rc = launch_refine(ctx, H, nb, d_px, d_p3, d_off, d_cnt, d_mask, d_pose, d_params, d_osucc, refine,
+                                 want_covariance, d_model, d_cov))
         return rc;
     std::vector<double> h_pose(7 * static_cast<size_t>(nb)), h_params(12 * static_cast<size_t>(nb)),
         h_cov(d_cov ? 36 * static_cast<size_t>(nb) : 0);
     std::vector<int32_t> h_succ(nb), h_inl(nb), h_fac(nb);
     std::vector<uint8_t> h_mask(static_cast<size_t>(std::max<int64_t>(H.total, 1)));
-    A_TRY(ctx, cudaMemcpyAsync(h_pose.data(), d_pose, sizeof(double) * 7 * nb, cudaMemcpyDeviceToHost, st));
-    A_TRY(ctx, cudaMemcpyAsync(h_params.data(), d_params, sizeof(double) * 12 * nb, cudaMemcpyDeviceToHost, st));
-    A_TRY(ctx, cudaMemcpyAsync(h_succ.data(), d_osucc, sizeof(int32_t) * nb, cudaMemcpyDeviceToHost, st));
-    A_TRY(ctx, cudaMemcpyAsync(h_inl.data(), d_oinl, sizeof(int32_t) * nb, cudaMemcpyDeviceToHost, st));
-    A_TRY(ctx, cudaMemcpyAsync(h_fac.data(), d_ofac, sizeof(int32_t) * nb, cudaMemcpyDeviceToHost, st));
-    if (d_cov) A_TRY(ctx, cudaMemcpyAsync(h_cov.data(), d_cov, sizeof(double) * 36 * nb, cudaMemcpyDeviceToHost, st));
+    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(h_pose.data(), d_pose, sizeof(double) * 7 * nb, cudaMemcpyDeviceToHost, st));
+    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(h_params.data(), d_params, sizeof(double) * 12 * nb, cudaMemcpyDeviceToHost, st));
+    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(h_succ.data(), d_osucc, sizeof(int32_t) * nb, cudaMemcpyDeviceToHost, st));
+    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(h_inl.data(), d_oinl, sizeof(int32_t) * nb, cudaMemcpyDeviceToHost, st));
+    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(h_fac.data(), d_ofac, sizeof(int32_t) * nb, cudaMemcpyDeviceToHost, st));
+    if (d_cov) B2M_CUDA_TRY(ctx, cudaMemcpyAsync(h_cov.data(), d_cov, sizeof(double) * 36 * nb, cudaMemcpyDeviceToHost, st));
     if (H.total > 0 && inlier_masks)
-      A_TRY(ctx, cudaMemcpyAsync(h_mask.data(), d_mask, H.total, cudaMemcpyDeviceToHost, st));
-    A_TRY(ctx, cudaStreamSynchronize(st));
+      B2M_CUDA_TRY(ctx, cudaMemcpyAsync(h_mask.data(), d_mask, H.total, cudaMemcpyDeviceToHost, st));
+    B2M_CUDA_TRY(ctx, cudaStreamSynchronize(st));
     for (int k = 0; k < nb; ++k) {
       // params: the camera's parameters after estimation (focal scaled when estimating it) and refinement
       fill_result(&out[k0 + k], h_pose.data() + 7 * k, h_params.data() + 12 * k, h_succ[k], h_inl[k], h_fac[k],
@@ -1582,16 +1536,12 @@ int b2m_refine_absolute_pose_batch(b2m_ctx* ctx, const b2m_abs_pose_problem* pro
                                    const double* init_poses, const uint8_t* const* inlier_masks,
                                    const b2m_pose_refine_opts* refine, int32_t want_covariance, b2m_abs_pose_result* out) {
   if (!ctx) return B2M_EINVAL;
-  auto bad = [&](const char* msg) {
-    ctx->err = msg;
-    return B2M_EINVAL;
-  };
   if (n_problems < 0 || (n_problems > 0 && (!problems || !out || !init_poses || !inlier_masks)) || !refine)
-    return bad("[abs_pose.cu] Check Failed: problems, initial poses, inlier masks, options and out != NULL");
-  if (const char* why = check_refine_opts(refine)) return bad(why);
-  if (const char* why = check_problems(problems, n_problems)) return bad(why);
+    return fail(ctx, B2M_EINVAL, "[abs_pose.cu] Check Failed: problems, initial poses, inlier masks, options and out != NULL");
+  if (const char* why = check_refine_opts(refine)) return fail(ctx, B2M_EINVAL, why);
+  if (const char* why = check_problems(problems, n_problems)) return fail(ctx, B2M_EINVAL, why);
   for (int64_t k = 0; k < n_problems; ++k)
-    if (problems[k].n > 0 && !inlier_masks[k]) return bad("[abs_pose.cu] Check Failed: inlier_mask.size() == points2D.size()");
+    if (problems[k].n > 0 && !inlier_masks[k]) return fail(ctx, B2M_EINVAL, "[abs_pose.cu] Check Failed: inlier_mask.size() == points2D.size()");
   cudaSetDevice(ctx->device);
   cudaStream_t st = ctx->stream;
   constexpr int64_t kChunk = 4096;
@@ -1606,39 +1556,37 @@ int b2m_refine_absolute_pose_batch(b2m_ctx* ctx, const b2m_abs_pose_problem* pro
       for (int j = 0; j < cam::kMaxParams; ++j) params[12 * k + j] = H.cams[k].p[j];
       for (int64_t i = 0; i < H.cnt[k]; ++i) mask[H.off[k] + i] = inlier_masks[k0 + k][i] ? 1 : 0;
     }
-    Bufs B;
-    double *d_px, *d_p3, *d_pose, *d_params;
-    int64_t* d_off;
-    int32_t *d_cnt, *d_succ;
-    uint8_t* d_mask;
-    A_TRY(ctx, B.alloc(&d_px, 2 * H.total));
-    A_TRY(ctx, B.alloc(&d_p3, 3 * H.total));
-    A_TRY(ctx, B.alloc(&d_pose, 7 * static_cast<size_t>(nb)));
-    A_TRY(ctx, B.alloc(&d_params, 12 * static_cast<size_t>(nb)));
-    A_TRY(ctx, B.alloc(&d_off, nb));
-    A_TRY(ctx, B.alloc(&d_cnt, nb));
-    A_TRY(ctx, B.alloc(&d_succ, nb));
-    A_TRY(ctx, B.alloc(&d_mask, H.total));
+    DeviceArray<double> d_px, d_p3, d_pose, d_params, d_cov;
+    DeviceArray<int64_t> d_off;
+    DeviceArray<int32_t> d_cnt, d_succ, d_model;
+    DeviceArray<uint8_t> d_mask;
+    B2M_CUDA_TRY(ctx, d_px.ensure(2 * H.total));
+    B2M_CUDA_TRY(ctx, d_p3.ensure(3 * H.total));
+    B2M_CUDA_TRY(ctx, d_pose.ensure(7 * static_cast<size_t>(nb)));
+    B2M_CUDA_TRY(ctx, d_params.ensure(12 * static_cast<size_t>(nb)));
+    B2M_CUDA_TRY(ctx, d_off.ensure(nb));
+    B2M_CUDA_TRY(ctx, d_cnt.ensure(nb));
+    B2M_CUDA_TRY(ctx, d_succ.ensure(nb));
+    B2M_CUDA_TRY(ctx, d_mask.ensure(H.total));
     if (H.total > 0) {
-      A_TRY(ctx, cudaMemcpyAsync(d_px, H.px.data(), sizeof(double) * 2 * H.total, cudaMemcpyHostToDevice, st));
-      A_TRY(ctx, cudaMemcpyAsync(d_p3, H.p3.data(), sizeof(double) * 3 * H.total, cudaMemcpyHostToDevice, st));
-      A_TRY(ctx, cudaMemcpyAsync(d_mask, mask.data(), H.total, cudaMemcpyHostToDevice, st));
+      B2M_CUDA_TRY(ctx, cudaMemcpyAsync(d_px, H.px.data(), sizeof(double) * 2 * H.total, cudaMemcpyHostToDevice, st));
+      B2M_CUDA_TRY(ctx, cudaMemcpyAsync(d_p3, H.p3.data(), sizeof(double) * 3 * H.total, cudaMemcpyHostToDevice, st));
+      B2M_CUDA_TRY(ctx, cudaMemcpyAsync(d_mask, mask.data(), H.total, cudaMemcpyHostToDevice, st));
     }
-    A_TRY(ctx, cudaMemcpyAsync(d_pose, init_poses + 7 * k0, sizeof(double) * 7 * nb, cudaMemcpyHostToDevice, st));
-    A_TRY(ctx, cudaMemcpyAsync(d_params, params.data(), sizeof(double) * 12 * nb, cudaMemcpyHostToDevice, st));
-    A_TRY(ctx, cudaMemcpyAsync(d_off, H.off.data(), sizeof(int64_t) * nb, cudaMemcpyHostToDevice, st));
-    A_TRY(ctx, cudaMemcpyAsync(d_cnt, H.cnt.data(), sizeof(int32_t) * nb, cudaMemcpyHostToDevice, st));
-    A_TRY(ctx, cudaMemcpyAsync(d_succ, succ.data(), sizeof(int32_t) * nb, cudaMemcpyHostToDevice, st));
-    double* d_cov = nullptr;
-    if (int rc = launch_refine(ctx, B, H, nb, d_px, d_p3, d_off, d_cnt, d_mask, d_pose, d_params, d_succ, refine,
-                               want_covariance, &d_cov))
+    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(d_pose, init_poses + 7 * k0, sizeof(double) * 7 * nb, cudaMemcpyHostToDevice, st));
+    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(d_params, params.data(), sizeof(double) * 12 * nb, cudaMemcpyHostToDevice, st));
+    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(d_off, H.off.data(), sizeof(int64_t) * nb, cudaMemcpyHostToDevice, st));
+    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(d_cnt, H.cnt.data(), sizeof(int32_t) * nb, cudaMemcpyHostToDevice, st));
+    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(d_succ, succ.data(), sizeof(int32_t) * nb, cudaMemcpyHostToDevice, st));
+    if (int rc = launch_refine(ctx, H, nb, d_px, d_p3, d_off, d_cnt, d_mask, d_pose, d_params, d_succ, refine,
+                               want_covariance, d_model, d_cov))
       return rc;
     std::vector<double> h_pose(7 * static_cast<size_t>(nb)), h_cov(d_cov ? 36 * static_cast<size_t>(nb) : 0);
-    A_TRY(ctx, cudaMemcpyAsync(h_pose.data(), d_pose, sizeof(double) * 7 * nb, cudaMemcpyDeviceToHost, st));
-    A_TRY(ctx, cudaMemcpyAsync(params.data(), d_params, sizeof(double) * 12 * nb, cudaMemcpyDeviceToHost, st));
-    A_TRY(ctx, cudaMemcpyAsync(succ.data(), d_succ, sizeof(int32_t) * nb, cudaMemcpyDeviceToHost, st));
-    if (d_cov) A_TRY(ctx, cudaMemcpyAsync(h_cov.data(), d_cov, sizeof(double) * 36 * nb, cudaMemcpyDeviceToHost, st));
-    A_TRY(ctx, cudaStreamSynchronize(st));
+    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(h_pose.data(), d_pose, sizeof(double) * 7 * nb, cudaMemcpyDeviceToHost, st));
+    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(params.data(), d_params, sizeof(double) * 12 * nb, cudaMemcpyDeviceToHost, st));
+    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(succ.data(), d_succ, sizeof(int32_t) * nb, cudaMemcpyDeviceToHost, st));
+    if (d_cov) B2M_CUDA_TRY(ctx, cudaMemcpyAsync(h_cov.data(), d_cov, sizeof(double) * 36 * nb, cudaMemcpyDeviceToHost, st));
+    B2M_CUDA_TRY(ctx, cudaStreamSynchronize(st));
     for (int k = 0; k < nb; ++k) {
       int inl = 0;
       for (int64_t i = 0; i < H.cnt[k]; ++i) inl += mask[H.off[k] + i];

@@ -24,22 +24,6 @@ thread_local std::string g_noctx_err;
 
 namespace {
 
-int fail(b2m_ctx* ctx, int code, const std::string& msg) {
-  if (ctx) ctx->err = msg; else g_noctx_err = msg;
-  return code;
-}
-
-#define CU_TRY(ctx, expr)                                                                       \
-  do {                                                                                          \
-    cudaError_t _e = (expr);                                                                    \
-    if (_e != cudaSuccess) {                                                                    \
-      char _b[512];                                                                             \
-      snprintf(_b, sizeof(_b), "[%s:%d] CUDA error: %s (%s)", __FILE__, __LINE__,              \
-               cudaGetErrorString(_e), #expr);                                                  \
-      return fail(ctx, _e == cudaErrorMemoryAllocation ? B2M_ENOMEM : B2M_ECUDA, _b);            \
-    }                                                                                           \
-  } while (0)
-
 typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                     const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
                                     CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -85,22 +69,22 @@ int layout_images_impl(b2m_ctx* ctx, ImageSet& S, int n_images, const int32_t* n
   rows = std::max<int64_t>(rows, kRowPad);
   S.max_feat_pad = std::max(round_up(S.max_feat, kRowPad), kRowPad);
   S.total_rows = rows;
-  CU_TRY(ctx, cudaMalloc(&S.d_desc, static_cast<size_t>(rows) * 128));
-  CU_TRY(ctx, cudaMemsetAsync(S.d_desc, 0, static_cast<size_t>(rows) * 128, ctx->stream));
+  B2M_CUDA_TRY(ctx, S.d_desc.ensure(static_cast<size_t>(rows) * 128));
+  B2M_CUDA_TRY(ctx, cudaMemsetAsync(S.d_desc, 0, static_cast<size_t>(rows) * 128, ctx->stream));
   if (want_kpts) {
-    CU_TRY(ctx, cudaMalloc(&S.d_kpts, static_cast<size_t>(rows) * sizeof(float2)));
-    CU_TRY(ctx, cudaMemsetAsync(S.d_kpts, 0, static_cast<size_t>(rows) * sizeof(float2), ctx->stream));
+    B2M_CUDA_TRY(ctx, S.d_kpts.ensure(static_cast<size_t>(rows)));
+    B2M_CUDA_TRY(ctx, cudaMemsetAsync(S.d_kpts, 0, static_cast<size_t>(rows) * sizeof(float2), ctx->stream));
   }
   // one extra, all-zero entry behind the table: image index `n_images` = "no features" (the dummy image
   // launch_k1_filter_skip points dead pairs at)
-  CU_TRY(ctx, cudaMalloc(&S.d_row0, sizeof(int32_t) * (n_images + 1)));
-  CU_TRY(ctx, cudaMalloc(&S.d_nfeat, sizeof(int32_t) * (n_images + 1)));
-  CU_TRY(ctx, cudaMemsetAsync(S.d_row0, 0, sizeof(int32_t) * (n_images + 1), ctx->stream));
-  CU_TRY(ctx, cudaMemsetAsync(S.d_nfeat, 0, sizeof(int32_t) * (n_images + 1), ctx->stream));
+  B2M_CUDA_TRY(ctx, S.d_row0.ensure(n_images + 1));
+  B2M_CUDA_TRY(ctx, S.d_nfeat.ensure(n_images + 1));
+  B2M_CUDA_TRY(ctx, cudaMemsetAsync(S.d_row0, 0, sizeof(int32_t) * (n_images + 1), ctx->stream));
+  B2M_CUDA_TRY(ctx, cudaMemsetAsync(S.d_nfeat, 0, sizeof(int32_t) * (n_images + 1), ctx->stream));
   if (n_images > 0) {
-    CU_TRY(ctx, cudaMemcpyAsync(S.d_row0, S.row0.data(), sizeof(int32_t) * n_images, cudaMemcpyHostToDevice,
+    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(S.d_row0, S.row0.data(), sizeof(int32_t) * n_images, cudaMemcpyHostToDevice,
                                 ctx->stream));
-    CU_TRY(ctx, cudaMemcpyAsync(S.d_nfeat, S.nfeat.data(), sizeof(int32_t) * n_images, cudaMemcpyHostToDevice,
+    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(S.d_nfeat, S.nfeat.data(), sizeof(int32_t) * n_images, cudaMemcpyHostToDevice,
                                 ctx->stream));
   }
   // One TMA tensor map over the whole set: dim0 = 128 descriptor bytes, dim1 = rows; box 128 x 128,
@@ -123,55 +107,55 @@ int layout_images_impl(b2m_ctx* ctx, ImageSet& S, int n_images, const int32_t* n
 }
 
 int ensure_workspace(b2m_ctx* ctx, int batch, int32_t mstride) {
-  Workspace& W = ctx->ws;
-  if (W.batch >= batch && W.mstride >= mstride) return B2M_OK;
-  W.release();
-  batch = std::max(batch, W.batch);
-  mstride = std::max(mstride, W.mstride);
-  const size_t arena_matches = static_cast<size_t>(batch) * mstride;
-  CU_TRY(ctx, cudaMalloc(&W.d_mbuf, sizeof(int32_t) * 2 * arena_matches));
-  CU_TRY(ctx, cudaMalloc(&W.d_aux, sizeof(uint2) * 2 * arena_matches));
-  CU_TRY(ctx, cudaMalloc(&W.d_cand_rows, sizeof(int32_t) * 2 * arena_matches));
-  CU_TRY(ctx, cudaMalloc(&W.d_cand_sorted, sizeof(int32_t) * 2 * arena_matches));
-  CU_TRY(ctx, cudaMalloc(&W.d_cand_cnt, sizeof(int32_t) * 2 * batch));
-  CU_TRY(ctx, cudaMalloc(&W.d_pairs_dir1, sizeof(int32_t) * 2 * batch));
-  for (int s = 0; s < 2; ++s) {
-    CU_TRY(ctx, cudaMalloc(&W.d_arena[s], sizeof(uint2) * arena_matches));
-    CU_TRY(ctx, cudaMalloc(&W.d_cursor[s], sizeof(unsigned long long)));
-    CU_TRY(ctx, cudaMalloc(&W.d_pair_off[s], sizeof(int64_t) * batch));
-    CU_TRY(ctx, cudaMalloc(&W.d_pair_cnt[s], sizeof(int32_t) * batch));
-    CU_TRY(ctx, cudaMallocHost(&W.h_arena[s], sizeof(uint2) * arena_matches));
-    CU_TRY(ctx, cudaMallocHost(&W.h_cursor[s], sizeof(unsigned long long)));
-    CU_TRY(ctx, cudaMallocHost(&W.h_pair_off[s], sizeof(int64_t) * batch));
-    CU_TRY(ctx, cudaMallocHost(&W.h_pair_cnt[s], sizeof(int32_t) * batch));
-  }
-  W.batch = batch;
-  W.mstride = mstride;
-  return B2M_OK;
+  if (ctx->ws.batch >= batch && ctx->ws.mstride >= mstride) return B2M_OK;
+  return alloc_group(ctx->ws, [&](Workspace& W) -> int {
+    const size_t arena_matches = static_cast<size_t>(batch) * mstride;
+    B2M_CUDA_TRY(ctx, W.d_mbuf.ensure(2 * arena_matches));
+    B2M_CUDA_TRY(ctx, W.d_aux.ensure(2 * arena_matches));
+    B2M_CUDA_TRY(ctx, W.d_cand_rows.ensure(2 * arena_matches));
+    B2M_CUDA_TRY(ctx, W.d_cand_sorted.ensure(2 * arena_matches));
+    B2M_CUDA_TRY(ctx, W.d_cand_cnt.ensure(2 * batch));
+    B2M_CUDA_TRY(ctx, W.d_pairs_dir1.ensure(2 * batch));
+    for (int s = 0; s < 2; ++s) {
+      B2M_CUDA_TRY(ctx, W.d_arena[s].ensure(arena_matches));
+      B2M_CUDA_TRY(ctx, W.d_cursor[s].ensure(1));
+      B2M_CUDA_TRY(ctx, W.d_pair_off[s].ensure(batch));
+      B2M_CUDA_TRY(ctx, W.d_pair_cnt[s].ensure(batch));
+      B2M_CUDA_TRY(ctx, W.h_arena[s].ensure(arena_matches));
+      B2M_CUDA_TRY(ctx, W.h_cursor[s].ensure(1));
+      B2M_CUDA_TRY(ctx, W.h_pair_off[s].ensure(batch));
+      B2M_CUDA_TRY(ctx, W.h_pair_cnt[s].ensure(batch));
+    }
+    W.batch = batch;
+    W.mstride = mstride;
+    return B2M_OK;
+  });
 }
 
 // Scratch of the gathered column direction, sized like the workspace (worst case: every column of every pair matched).
 int ensure_gather(b2m_ctx* ctx) {
-  Workspace& W = ctx->ws;
-  if (W.d_gath_desc) return B2M_OK;
-  const size_t rows = static_cast<size_t>(W.batch) * W.mstride;
-  CU_TRY(ctx, cudaMalloc(&W.d_gath_desc, rows * 128));
-  CU_TRY(ctx, cudaMalloc(&W.d_colrank, sizeof(int32_t) * rows));
-  CU_TRY(ctx, cudaMalloc(&W.d_gath_cols, sizeof(int32_t) * rows));
-  CU_TRY(ctx, cudaMalloc(&W.d_gath_cnt, sizeof(int32_t) * W.batch));
-  CU_TRY(ctx, cudaMalloc(&W.d_gath_items, sizeof(int32_t) * 2 * (rows / kRowPad + 1)));
-  CU_TRY(ctx, cudaMalloc(&W.d_gath_n, sizeof(int32_t)));
-  PFN_encodeTiled enc = get_encode_tiled();
-  if (!enc) return fail(ctx, B2M_ECUDA, "[api.cu] cuTensorMapEncodeTiled not available from the driver");
-  cuuint64_t gdim[2] = {128, static_cast<cuuint64_t>(rows)};
-  cuuint64_t gstride[1] = {128};
-  cuuint32_t box[2] = {128, 128};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = enc(&W.tmap_gath, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, W.d_gath_desc, gdim, gstride, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return fail(ctx, B2M_ECUDA, "[api.cu] cuTensorMapEncodeTiled (gather scratch) failed");
-  return B2M_OK;
+  const Workspace& W = ctx->ws;
+  if (W.gath.desc) return B2M_OK;
+  return alloc_group(ctx->ws.gath, [&](GatherBufs& g) -> int {
+    const size_t rows = static_cast<size_t>(W.batch) * W.mstride;
+    B2M_CUDA_TRY(ctx, g.desc.ensure(rows * 128));
+    B2M_CUDA_TRY(ctx, g.colrank.ensure(rows));
+    B2M_CUDA_TRY(ctx, g.cols.ensure(rows));
+    B2M_CUDA_TRY(ctx, g.cnt.ensure(W.batch));
+    B2M_CUDA_TRY(ctx, g.items.ensure(2 * (rows / kRowPad + 1)));
+    B2M_CUDA_TRY(ctx, g.n.ensure(1));
+    PFN_encodeTiled enc = get_encode_tiled();
+    if (!enc) return fail(ctx, B2M_ECUDA, "[api.cu] cuTensorMapEncodeTiled not available from the driver");
+    cuuint64_t gdim[2] = {128, static_cast<cuuint64_t>(rows)};
+    cuuint64_t gstride[1] = {128};
+    cuuint32_t box[2] = {128, 128};
+    cuuint32_t estr[2] = {1, 1};
+    CUresult r = enc(&g.tmap, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, g.desc, gdim, gstride, box, estr,
+                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) return fail(ctx, B2M_ECUDA, "[api.cu] cuTensorMapEncodeTiled (gather scratch) failed");
+    return B2M_OK;
+  });
 }
 
 int check_sift(b2m_ctx* ctx, const b2m_sift_opts* o) {
@@ -232,12 +216,12 @@ int match_pairs_impl(b2m_ctx* ctx, ImageSet& S, const int32_t* pairs, int64_t n_
     return fail(ctx, B2M_EINVAL, "[api.cu] Check Failed: num descriptors <= SiftMatchingOptions.max_num_matches "
                                  "(truncate at upload; images the pair list does not reference are not checked)");
 
-  b2m_results* res = new (std::nothrow) b2m_results();
+  std::unique_ptr<b2m_results> res(new (std::nothrow) b2m_results());
   if (!res) return fail(ctx, B2M_ENOMEM, "[api.cu] out of host memory");
   res->pairs.assign(pairs, pairs + 2 * n_pairs);
   res->off.assign(n_pairs, 0);
   res->cnt.assign(n_pairs, 0);
-  if (tvg) verify_results_init(res, n_pairs);
+  if (tvg) verify_results_init(res.get(), n_pairs);
   if (host_cache_enabled()) {
     HostCache& hc = host_cache();
     std::lock_guard<std::mutex> lk(hc.mu);
@@ -255,10 +239,6 @@ int match_pairs_impl(b2m_ctx* ctx, ImageSet& S, const int32_t* pairs, int64_t n_
     } catch (const std::bad_alloc&) {  // only a hint
     }
   }
-  auto bail = [&](int rc) {
-    delete res;
-    return rc;
-  };
 
   // pairs per kernel batch; bounded so that the worst-case scratch of the gathered column direction
   // (batch x mstride descriptors) stays below 6 GB even for 32768-feature images
@@ -272,34 +252,17 @@ int match_pairs_impl(b2m_ctx* ctx, ImageSet& S, const int32_t* pairs, int64_t n_
   // sized for the pairs of this call, not for a full batch: a context that only ever sees small jobs stays small
   if (int rc = ensure_workspace(ctx, static_cast<int>(std::min<int64_t>(B, std::max<int64_t>(n_pairs, 1))),
                                 round_up(S.max_feat_pad, 512)))
-    return bail(rc);
+    return rc;
   if (tvg)
     if (int rc = verify_prepare(ctx, S, ctx->ws.batch, static_cast<int64_t>(ctx->ws.batch) * ctx->ws.mstride))
-      return bail(rc);
-  if (ctx->d_pairs_cap < n_pairs) {
-    if (ctx->d_pairs) cudaFree(ctx->d_pairs);
-    ctx->d_pairs = nullptr;
-    ctx->d_pairs_cap = 0;
-    cudaError_t e = cudaMalloc(&ctx->d_pairs, sizeof(int32_t) * 2 * std::max<int64_t>(n_pairs, 1));
-    if (e != cudaSuccess) return bail(fail(ctx, B2M_ENOMEM, "[api.cu] cudaMalloc(pairs) failed"));
-    ctx->d_pairs_cap = n_pairs;
-  }
+      return rc;
+  if (n_pairs > 0) B2M_CUDA_TRY(ctx, ctx->d_pairs.ensure(2 * static_cast<size_t>(n_pairs)));
   Workspace& W = ctx->ws;
   cudaStream_t st = ctx->stream;
-#define CU_TRY_R(expr)                                                                      \
-  do {                                                                                      \
-    cudaError_t _e = (expr);                                                                \
-    if (_e != cudaSuccess) {                                                                \
-      char _b[512];                                                                         \
-      snprintf(_b, sizeof(_b), "[%s:%d] CUDA error: %s (%s)", __FILE__, __LINE__,          \
-               cudaGetErrorString(_e), #expr);                                              \
-      return bail(fail(ctx, B2M_ECUDA, _b));                                                \
-    }                                                                                       \
-  } while (0)
 
   if (n_pairs > 0)
-    CU_TRY_R(cudaMemcpyAsync(ctx->d_pairs, pairs, sizeof(int32_t) * 2 * n_pairs, cudaMemcpyHostToDevice, st));
-  CU_TRY_R(cudaEventRecord(ctx->ev_t0, st));
+    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(ctx->d_pairs, pairs, sizeof(int32_t) * 2 * n_pairs, cudaMemcpyHostToDevice, st));
+  B2M_CUDA_TRY(ctx, cudaEventRecord(ctx->ev_t0, st));
   ctx->stats.last_k1_ms = 0.0;
   ctx->stats.last_k1_launches = 0;
 
@@ -314,7 +277,7 @@ int match_pairs_impl(b2m_ctx* ctx, ImageSet& S, const int32_t* pairs, int64_t n_
     const int s = static_cast<int>(b & 1);
     const int64_t p0 = b * B;
     const int nb = static_cast<int>(std::min<int64_t>(B, n_pairs - p0));
-    CU_TRY(ctx, cudaEventSynchronize(ctx->ev_k[s]));
+    B2M_CUDA_TRY(ctx, cudaEventSynchronize(ctx->ev_k[s]));
     const unsigned long long total = *W.h_cursor[s];
     {
       float k1ms = 0.f, vms = 0.f;
@@ -329,18 +292,18 @@ int match_pairs_impl(b2m_ctx* ctx, ImageSet& S, const int32_t* pairs, int64_t n_
         if (cudaEventElapsedTime(&vms, ctx->ev_k1b[s], ctx->ev_k[s]) == cudaSuccess) verify_ms += vms;
       }
     }
-    CU_TRY(ctx, cudaStreamWaitEvent(ctx->copy_stream, ctx->ev_k[s], 0));
-    CU_TRY(ctx, cudaMemcpyAsync(W.h_pair_off[s], W.d_pair_off[s], sizeof(int64_t) * nb, cudaMemcpyDeviceToHost,
+    B2M_CUDA_TRY(ctx, cudaStreamWaitEvent(ctx->copy_stream, ctx->ev_k[s], 0));
+    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(W.h_pair_off[s], W.d_pair_off[s], sizeof(int64_t) * nb, cudaMemcpyDeviceToHost,
                                 ctx->copy_stream));
-    CU_TRY(ctx, cudaMemcpyAsync(W.h_pair_cnt[s], W.d_pair_cnt[s], sizeof(int32_t) * nb, cudaMemcpyDeviceToHost,
+    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(W.h_pair_cnt[s], W.d_pair_cnt[s], sizeof(int32_t) * nb, cudaMemcpyDeviceToHost,
                                 ctx->copy_stream));
     if (total > 0)
-      CU_TRY(ctx, cudaMemcpyAsync(W.h_arena[s], W.d_arena[s], sizeof(uint2) * total, cudaMemcpyDeviceToHost,
+      B2M_CUDA_TRY(ctx, cudaMemcpyAsync(W.h_arena[s], W.d_arena[s], sizeof(uint2) * total, cudaMemcpyDeviceToHost,
                                   ctx->copy_stream));
     if (tvg)
-      if (int rc = verify_batch_download(ctx, res, s, p0, nb)) return rc;
-    CU_TRY(ctx, cudaEventRecord(ctx->ev_data[s], ctx->copy_stream));
-    CU_TRY(ctx, cudaEventSynchronize(ctx->ev_data[s]));
+      if (int rc = verify_batch_download(ctx, res.get(), s, p0, nb)) return rc;
+    B2M_CUDA_TRY(ctx, cudaEventRecord(ctx->ev_data[s], ctx->copy_stream));
+    B2M_CUDA_TRY(ctx, cudaEventSynchronize(ctx->ev_data[s]));
     const int64_t base = static_cast<int64_t>(res->matches.size() / 2);
     res->matches.resize(res->matches.size() + 2 * total);
     if (total > 0) memcpy(res->matches.data() + 2 * base, W.h_arena[s], sizeof(uint2) * total);
@@ -349,7 +312,7 @@ int match_pairs_impl(b2m_ctx* ctx, ImageSet& S, const int32_t* pairs, int64_t n_
       res->cnt[p0 + k] = W.h_pair_cnt[s][k];
     }
     if (tvg)
-      if (int rc = verify_batch_collect(ctx, res, s, p0, nb, tvg->min_num_inliers)) return rc;
+      if (int rc = verify_batch_collect(ctx, res.get(), s, p0, nb, tvg->min_num_inliers)) return rc;
     return B2M_OK;
   };
 
@@ -388,10 +351,10 @@ int match_pairs_impl(b2m_ctx* ctx, ImageSet& S, const int32_t* pairs, int64_t n_
     cp.pair_off = W.d_pair_off[bp.s];
     cp.pair_cnt = W.d_pair_cnt[bp.s];
     cp.img_row0 = S.d_row0;
-    cp.kpts = tvg ? S.d_kpts : nullptr;
+    cp.kpts = tvg ? static_cast<const float2*>(S.d_kpts) : nullptr;
     cp.pts = tvg ? static_cast<double4*>(verify_points_arena(ctx, bp.s)) : nullptr;
     cp.enable = nullptr;
-    cp.cand_cnt = ctx->exact_k1 ? nullptr : W.d_cand_cnt;   // the filter epilogue's candidate counts (not produced by K1-exact)
+    cp.cand_cnt = ctx->exact_k1 ? nullptr : static_cast<const int32_t*>(W.d_cand_cnt);   // the filter epilogue's candidate counts (not produced by K1-exact)
     return bp;
   };
   // Column direction of the cross-check: computed for the matched columns only (launch_k1_filter_gather).  The
@@ -400,8 +363,8 @@ int match_pairs_impl(b2m_ctx* ctx, ImageSet& S, const int32_t* pairs, int64_t n_
   const bool split_capable = !ctx->exact_k1 && n_dirs == 2;
   auto gather_scratch = [&]() {
     GatherScratch g;
-    g.desc = W.d_gath_desc; g.colrank = W.d_colrank; g.cols = W.d_gath_cols; g.cnt = W.d_gath_cnt;
-    g.items = W.d_gath_items; g.n_items = W.d_gath_n;
+    g.desc = W.gath.desc; g.colrank = W.gath.colrank; g.cols = W.gath.cols; g.cnt = W.gath.cnt;
+    g.items = W.gath.items; g.n_items = W.gath.n;
     return g;
   };
   // One-time comparison of the gathered schedule against the two-direction launch on one batch (returns a B2M code;
@@ -410,18 +373,12 @@ int match_pairs_impl(b2m_ctx* ctx, ImageSet& S, const int32_t* pairs, int64_t n_
     const int s = bp.s, nb = bp.nb;
     const MatchParams& mp = bp.mp;
     const CompactParams& cp = bp.cp;
-    uint2* t_arena = nullptr;
-    int64_t* t_off = nullptr;
-    int32_t *t_cnt = nullptr, *t_flag = nullptr;
-    auto drop = [&]() {
-      cudaFree(t_arena); cudaFree(t_off); cudaFree(t_cnt); cudaFree(t_flag);
-      t_arena = nullptr; t_off = nullptr; t_cnt = nullptr; t_flag = nullptr;
-    };
+    DeviceArray<uint2> t_arena;
+    DeviceArray<int64_t> t_off;
+    DeviceArray<int32_t> t_cnt, t_flag;
     const size_t arena_matches = static_cast<size_t>(W.batch) * W.mstride;
-    if (ensure_gather(ctx) != B2M_OK || cudaMalloc(&t_arena, sizeof(uint2) * arena_matches) != cudaSuccess ||
-        cudaMalloc(&t_off, sizeof(int64_t) * nb) != cudaSuccess || cudaMalloc(&t_cnt, sizeof(int32_t) * nb) != cudaSuccess ||
-        cudaMalloc(&t_flag, sizeof(int32_t)) != cudaSuccess) {
-      drop();
+    if (ensure_gather(ctx) != B2M_OK || t_arena.ensure(arena_matches) != cudaSuccess ||
+        t_off.ensure(nb) != cudaSuccess || t_cnt.ensure(nb) != cudaSuccess || t_flag.ensure(1) != cudaSuccess) {
       cudaGetLastError();
       ctx->k1_dir1_mode = B2M_K1_DIR1_FULL_NOMEM;  // no room for the scratch / comparison: stay on the validated launch
       return B2M_OK;
@@ -432,18 +389,17 @@ int match_pairs_impl(b2m_ctx* ctx, ImageSet& S, const int32_t* pairs, int64_t n_
     ct.pair_cnt = t_cnt;
     ct.kpts = nullptr;
     ct.pts = nullptr;
-    ct.colrank = W.d_colrank;
+    ct.colrank = W.gath.colrank;
     cudaError_t e = cudaMemsetAsync(W.d_cursor[s], 0, sizeof(unsigned long long), st);
     if (e == cudaSuccess)
-      e = launch_k1_filter_gather(S.tmap, W.tmap_gath, mp, S.d_desc, nb, max_strips, ctx->num_sms, gather_scratch(), st, nullptr);
+      e = launch_k1_filter_gather(S.tmap, W.gath.tmap, mp, S.d_desc, nb, max_strips, ctx->num_sms, gather_scratch(), st, nullptr);
     if (e == cudaSuccess) e = launch_crosscheck_compact(ct, nb, st);
     if (e != cudaSuccess) {
       // the gathered schedule could not even be launched (a non-sticky launch error): stay on the validated
       // launch instead of failing the call; a sticky error resurfaces at the next CUDA call anyway
       cudaGetLastError();
-      drop();
       ctx->k1_dir1_mode = B2M_K1_DIR1_FULL_MISMATCH;
-      CU_TRY_R(cudaMemsetAsync(W.d_cursor[s], 0, sizeof(unsigned long long), st));
+      B2M_CUDA_TRY(ctx, cudaMemsetAsync(W.d_cursor[s], 0, sizeof(unsigned long long), st));
       return B2M_OK;
     }
     int32_t h_flag = -1;
@@ -458,24 +414,23 @@ int match_pairs_impl(b2m_ctx* ctx, ImageSet& S, const int32_t* pairs, int64_t n_
     if (e == cudaSuccess)
       e = cudaMemcpyAsync(&h_total, W.d_cursor[s], sizeof(unsigned long long), cudaMemcpyDeviceToHost, st);
     if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-    drop();
-    if (e != cudaSuccess) CU_TRY_R(e);
+    if (e != cudaSuccess) B2M_CUDA_TRY(ctx, e);
     // a batch without a single match compares nothing: stay untested (and on the two-direction launch)
     if (h_flag != 0) ctx->k1_dir1_mode = B2M_K1_DIR1_FULL_MISMATCH;
     else if (h_total > 0) ctx->k1_dir1_mode = B2M_K1_DIR1_GATHER;
     ctx->stats.kernel_launches += 10;
-    CU_TRY_R(cudaMemsetAsync(W.d_cursor[s], 0, sizeof(unsigned long long), st));
+    B2M_CUDA_TRY(ctx, cudaMemsetAsync(W.d_cursor[s], 0, sizeof(unsigned long long), st));
     return B2M_OK;
   };
   // RANSAC + decision of a compacted batch (+ guided re-matching), then its match total to the host
   auto verify_stage = [&](const BatchParams& bp) -> int {
     const int s = bp.s, nb = bp.nb;
     if (tvg)
-      if (int rc = verify_batch_launch(ctx, S, tvg, sift, s, bp.p0, nb)) return bail(rc);
+      if (int rc = verify_batch_launch(ctx, S, tvg, sift, s, bp.p0, nb)) return rc;
     if (tvg && sift->guided_matching) {
       // K1g: re-match the verified pairs under their geometry; the result replaces the inlier matches
       GuidedSlot gs;
-      if (int rc = verify_guided_slot(ctx, s, &gs)) return bail(rc);
+      if (int rc = verify_guided_slot(ctx, s, &gs)) return rc;
       GuidedParams gp{};
       gp.kind = gs.kind;
       gp.model = gs.model;
@@ -487,10 +442,10 @@ int match_pairs_impl(b2m_ctx* ctx, ImageSet& S, const int32_t* pairs, int64_t n_
       const bool guided_full = guided_env && !strcmp(guided_env, "full");
       const bool guided_gather = n_dirs == 2 && !guided_full && ensure_gather(ctx) == B2M_OK;
       if (guided_gather)
-        CU_TRY_R(launch_k1_guided_gather(S.tmap, W.tmap_gath, bp.mp, gp, S.d_desc, nb, max_strips, gather_scratch(), st));
+        B2M_CUDA_TRY(ctx, launch_k1_guided_gather(S.tmap, W.gath.tmap, bp.mp, gp, S.d_desc, nb, max_strips, gather_scratch(), st));
       else
-        CU_TRY_R(launch_k1_guided(S.tmap, bp.mp, gp, nb, max_strips, n_dirs, st));
-      CU_TRY_R(cudaMemsetAsync(gs.cursor, 0, sizeof(unsigned long long), st));
+        B2M_CUDA_TRY(ctx, launch_k1_guided(S.tmap, bp.mp, gp, nb, max_strips, n_dirs, st));
+      B2M_CUDA_TRY(ctx, cudaMemsetAsync(gs.cursor, 0, sizeof(unsigned long long), st));
       CompactParams gc = bp.cp;
       gc.arena = gs.arena;
       gc.cursor = gs.cursor;
@@ -500,13 +455,13 @@ int match_pairs_impl(b2m_ctx* ctx, ImageSet& S, const int32_t* pairs, int64_t n_
       gc.pts = nullptr;
       gc.enable = gs.kind;
       gc.cand_cnt = nullptr;   // the guided kernel writes final matches, no candidate lists
-      gc.colrank = guided_gather ? W.d_colrank : nullptr;
-      CU_TRY_R(launch_crosscheck_compact(gc, nb, st));
-      CU_TRY_R(cudaMemcpyAsync(gs.h_cursor, gs.cursor, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+      gc.colrank = guided_gather ? static_cast<const int32_t*>(W.gath.colrank) : nullptr;
+      B2M_CUDA_TRY(ctx, launch_crosscheck_compact(gc, nb, st));
+      B2M_CUDA_TRY(ctx, cudaMemcpyAsync(gs.h_cursor, gs.cursor, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
       ctx->stats.kernel_launches += guided_gather ? 4 : 2;
     }
-    CU_TRY_R(cudaMemcpyAsync(W.h_cursor[s], W.d_cursor[s], sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
-    CU_TRY_R(cudaEventRecord(ctx->ev_k[s], st));
+    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(W.h_cursor[s], W.d_cursor[s], sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+    B2M_CUDA_TRY(ctx, cudaEventRecord(ctx->ev_k[s], st));
     return B2M_OK;
   };
   auto stopped = [&]() -> int {
@@ -514,13 +469,13 @@ int match_pairs_impl(b2m_ctx* ctx, ImageSet& S, const int32_t* pairs, int64_t n_
     cudaStreamSynchronize(ctx->aux_stream);
     cudaStreamSynchronize(ctx->copy_stream);
     ctx->stop = 0;
-    return bail(fail(ctx, B2M_ESTOPPED, "[api.cu] stopped by b2m_request_stop"));
+    return fail(ctx, B2M_ESTOPPED, "[api.cu] stopped by b2m_request_stop");
   };
 
   const double hp_t1 = now();
   bool pretested = false;
   if (n_batches > 0 && split_capable && ctx->k1_dir1_mode == B2M_K1_DIR1_UNTESTED) {
-    if (int rc = k1_selftest(batch_params(0))) return rc;  // `res` was released by the failing step
+    if (int rc = k1_selftest(batch_params(0))) return rc;
     pretested = true;
   }
   // Overlapped order (gathered schedule + verification, the exhaustive pipeline's case): the ALU-only middle of K1
@@ -533,7 +488,7 @@ int match_pairs_impl(b2m_ctx* ctx, ImageSet& S, const int32_t* pairs, int64_t n_
   pipelined = split_capable && tvg && !sift->guided_matching && n_batches >= 2 && !no_overlap &&
               (ctx->k1_dir1_mode == B2M_K1_DIR1_GATHER || ctx->k1_dir1_mode == B2M_K1_DIR1_GATHER_FORCED);
   if (pipelined) {
-    if (int rc = ensure_gather(ctx)) return bail(rc);
+    if (int rc = ensure_gather(ctx)) return rc;
     const GatherScratch g = gather_scratch();
     BatchParams prev;
     auto gemm0_time = [&](int s) {
@@ -547,26 +502,26 @@ int match_pairs_impl(b2m_ctx* ctx, ImageSet& S, const int32_t* pairs, int64_t n_
       BatchParams bp = batch_params(b);
       const int s = bp.s, nb = bp.nb;
       if (b >= 2) gemm0_time(s);  // GEMM0 of batch b - 2: complete (the host waited for RANSAC(b - 3) an iteration ago)
-      CU_TRY_R(cudaMemsetAsync(W.d_cursor[s], 0, sizeof(unsigned long long), st));
-      CU_TRY_R(cudaEventRecord(ctx->ev_k1a[s], st));
-      CU_TRY_R(launch_k1_gather_phase(0, S.tmap, W.tmap_gath, bp.mp, S.d_desc, nb, max_strips, ctx->num_sms, g, st));
-      CU_TRY_R(cudaEventRecord(ctx->ev_k1b[s], st));
-      CU_TRY_R(cudaStreamWaitEvent(ctx->aux_stream, ctx->ev_k1b[s], 0));
-      CU_TRY_R(launch_k1_gather_phase(1, S.tmap, W.tmap_gath, bp.mp, S.d_desc, nb, max_strips, ctx->num_sms, g, ctx->aux_stream));
-      CU_TRY_R(cudaEventRecord(ctx->ev_p1[s], ctx->aux_stream));
+      B2M_CUDA_TRY(ctx, cudaMemsetAsync(W.d_cursor[s], 0, sizeof(unsigned long long), st));
+      B2M_CUDA_TRY(ctx, cudaEventRecord(ctx->ev_k1a[s], st));
+      B2M_CUDA_TRY(ctx, launch_k1_gather_phase(0, S.tmap, W.gath.tmap, bp.mp, S.d_desc, nb, max_strips, ctx->num_sms, g, st));
+      B2M_CUDA_TRY(ctx, cudaEventRecord(ctx->ev_k1b[s], st));
+      B2M_CUDA_TRY(ctx, cudaStreamWaitEvent(ctx->aux_stream, ctx->ev_k1b[s], 0));
+      B2M_CUDA_TRY(ctx, launch_k1_gather_phase(1, S.tmap, W.gath.tmap, bp.mp, S.d_desc, nb, max_strips, ctx->num_sms, g, ctx->aux_stream));
+      B2M_CUDA_TRY(ctx, cudaEventRecord(ctx->ev_p1[s], ctx->aux_stream));
       if (b > 0)
         if (int rc = verify_stage(prev)) return rc;
       // Drain batch b - 2 (same slot as b) while GEMM0(b) keeps the GPU busy: its RANSAC ran an iteration ago, so the
       // host does not wait; the slot's match arena / verification outputs are next written by the compaction below.
       if (b >= 2)
-        if (int rc = finish(b - 2)) return bail(rc);
-      CU_TRY_R(cudaStreamWaitEvent(st, ctx->ev_p1[s], 0));
-      CU_TRY_R(cudaEventRecord(ctx->ev_g2a[s], st));
-      CU_TRY_R(launch_k1_gather_phase(2, S.tmap, W.tmap_gath, bp.mp, S.d_desc, nb, max_strips, ctx->num_sms, g, st));
-      CU_TRY_R(cudaEventRecord(ctx->ev_g2b[s], st));
-      CU_TRY_R(launch_k1_gather_phase(3, S.tmap, W.tmap_gath, bp.mp, S.d_desc, nb, max_strips, ctx->num_sms, g, st));
-      bp.cp.colrank = W.d_colrank;
-      CU_TRY_R(launch_crosscheck_compact(bp.cp, nb, st));
+        if (int rc = finish(b - 2)) return rc;
+      B2M_CUDA_TRY(ctx, cudaStreamWaitEvent(st, ctx->ev_p1[s], 0));
+      B2M_CUDA_TRY(ctx, cudaEventRecord(ctx->ev_g2a[s], st));
+      B2M_CUDA_TRY(ctx, launch_k1_gather_phase(2, S.tmap, W.gath.tmap, bp.mp, S.d_desc, nb, max_strips, ctx->num_sms, g, st));
+      B2M_CUDA_TRY(ctx, cudaEventRecord(ctx->ev_g2b[s], st));
+      B2M_CUDA_TRY(ctx, launch_k1_gather_phase(3, S.tmap, W.gath.tmap, bp.mp, S.d_desc, nb, max_strips, ctx->num_sms, g, st));
+      bp.cp.colrank = W.gath.colrank;
+      B2M_CUDA_TRY(ctx, launch_crosscheck_compact(bp.cp, nb, st));
       ctx->stats.kernel_launches += 7;
       ctx->stats.last_k1_launches += 1;
       ctx->stats.k1_dir1_mode = static_cast<uint64_t>(ctx->k1_dir1_mode);
@@ -582,62 +537,61 @@ int match_pairs_impl(b2m_ctx* ctx, ImageSet& S, const int32_t* pairs, int64_t n_
     const int s = bp.s, nb = bp.nb;
     MatchParams& mp = bp.mp;
     CompactParams& cp = bp.cp;
-    if (b >= 2) CU_TRY_R(cudaStreamWaitEvent(st, ctx->ev_data[s], 0));
-    CU_TRY_R(cudaMemsetAsync(W.d_cursor[s], 0, sizeof(unsigned long long), st));
+    if (b >= 2) B2M_CUDA_TRY(ctx, cudaStreamWaitEvent(st, ctx->ev_data[s], 0));
+    B2M_CUDA_TRY(ctx, cudaMemsetAsync(W.d_cursor[s], 0, sizeof(unsigned long long), st));
     if (split_capable && ctx->k1_dir1_mode == B2M_K1_DIR1_UNTESTED && !(b == 0 && pretested))
-      if (int rc = k1_selftest(bp)) return rc;  // `res` was released by the failing step
+      if (int rc = k1_selftest(bp)) return rc;
     const bool use_gather = split_capable && (ctx->k1_dir1_mode == B2M_K1_DIR1_GATHER || ctx->k1_dir1_mode == B2M_K1_DIR1_GATHER_FORCED);
     const bool use_skip = split_capable && (ctx->k1_dir1_mode == B2M_K1_DIR1_SKIP || ctx->k1_dir1_mode == B2M_K1_DIR1_SKIP_FORCED);
     if (use_gather)
-      if (int rc = ensure_gather(ctx)) return bail(rc);
-    CU_TRY_R(cudaEventRecord(ctx->ev_k1a[s], st));
+      if (int rc = ensure_gather(ctx)) return rc;
+    B2M_CUDA_TRY(ctx, cudaEventRecord(ctx->ev_k1a[s], st));
     if (ctx->exact_k1) {
-      CU_TRY_R(launch_k1_match(S.tmap, mp, nb, max_strips, n_dirs, st));
+      B2M_CUDA_TRY(ctx, launch_k1_match(S.tmap, mp, nb, max_strips, n_dirs, st));
     } else if (use_gather) {
-      CU_TRY_R(launch_k1_filter_gather(S.tmap, W.tmap_gath, mp, S.d_desc, nb, max_strips, ctx->num_sms, gather_scratch(), st,
+      B2M_CUDA_TRY(ctx, launch_k1_filter_gather(S.tmap, W.gath.tmap, mp, S.d_desc, nb, max_strips, ctx->num_sms, gather_scratch(), st,
                                        ctx->ev_k1b[s]));
-      cp.colrank = W.d_colrank;
+      cp.colrank = W.gath.colrank;
       ctx->stats.kernel_launches += 4;  // second GEMM launch, gather, two resolves instead of one
     } else if (use_skip) {
-      CU_TRY_R(launch_k1_filter_skip(S.tmap, mp, S.d_desc, nb, max_strips, ctx->num_sms, W.d_pairs_dir1, S.n_images, st,
+      B2M_CUDA_TRY(ctx, launch_k1_filter_skip(S.tmap, mp, S.d_desc, nb, max_strips, ctx->num_sms, W.d_pairs_dir1, S.n_images, st,
                                      ctx->ev_k1b[s]));
       ctx->stats.kernel_launches += 3;  // second GEMM launch, pair selection, resolve
     } else {
-      CU_TRY_R(launch_k1_filter(S.tmap, mp, S.d_desc, nb, max_strips, n_dirs, ctx->num_sms, st,
+      B2M_CUDA_TRY(ctx, launch_k1_filter(S.tmap, mp, S.d_desc, nb, max_strips, n_dirs, ctx->num_sms, st,
                                 ctx->ev_k1b[s]));
       ctx->stats.kernel_launches += 1;
     }
-    if (ctx->exact_k1) CU_TRY_R(cudaEventRecord(ctx->ev_k1b[s], st));
+    if (ctx->exact_k1) B2M_CUDA_TRY(ctx, cudaEventRecord(ctx->ev_k1b[s], st));
     ctx->stats.kernel_launches += 1;
     ctx->stats.last_k1_launches += 1;
     ctx->stats.k1_dir1_mode = static_cast<uint64_t>(ctx->k1_dir1_mode);
-    CU_TRY_R(launch_crosscheck_compact(cp, nb, st));
+    B2M_CUDA_TRY(ctx, launch_crosscheck_compact(cp, nb, st));
     ctx->stats.kernel_launches += 1;
     if (int rc = verify_stage(bp)) return rc;
     if (b > 0)
-      if (int rc = finish(b - 1)) return bail(rc);
+      if (int rc = finish(b - 1)) return rc;
   }
   }
   const double hp_t2 = now();
   if (pipelined && n_batches >= 2)
-    if (int rc = finish(n_batches - 2)) return bail(rc);
+    if (int rc = finish(n_batches - 2)) return rc;
   if (n_batches > 0)
-    if (int rc = finish(n_batches - 1)) return bail(rc);
-  CU_TRY_R(cudaEventRecord(ctx->ev_t1, st));
-  CU_TRY_R(cudaEventSynchronize(ctx->ev_t1));
+    if (int rc = finish(n_batches - 1)) return rc;
+  B2M_CUDA_TRY(ctx, cudaEventRecord(ctx->ev_t1, st));
+  B2M_CUDA_TRY(ctx, cudaEventSynchronize(ctx->ev_t1));
   float ms = 0.f;
   cudaEventElapsedTime(&ms, ctx->ev_t0, ctx->ev_t1);
   ctx->stats.last_total_ms = ms;
   if (pipelined) verify_ms = std::max(0.0, static_cast<double>(ms) - ctx->stats.last_k1_ms);
   ctx->stats.last_verify_ms = verify_ms;
   ctx->stats.last_match_ms = ms - verify_ms;
-#undef CU_TRY_R
   if (host_prof)
     fprintf(stderr, "[b2m hostprof] pairs %lld: set-up %.1f ms, launch loop %.1f ms, last batch + sync %.1f ms, device %.1f ms\n",
             static_cast<long long>(n_pairs), hp_t1 - hp_t0, hp_t2 - hp_t1, now() - hp_t2, ms);
   ctx->hint_matches = res->matches.size() / 2;
   ctx->hint_inliers = res->inliers.size() / 2;
-  *out = res;
+  *out = res.release();
   return B2M_OK;
 }
 
@@ -651,63 +605,6 @@ b2m_results::~b2m_results() {
   if (matches.capacity() > hc.matches.capacity()) matches.swap(hc.matches);
   if (inliers.capacity() > hc.inliers.capacity()) inliers.swap(hc.inliers);
 }
-
-namespace b2m {
-void ImageSet::release() {
-  if (d_desc) cudaFree(d_desc);
-  if (d_kpts) cudaFree(d_kpts);
-  if (d_row0) cudaFree(d_row0);
-  if (d_nfeat) cudaFree(d_nfeat);
-  d_desc = nullptr;
-  d_kpts = nullptr;
-  d_row0 = nullptr;
-  d_nfeat = nullptr;
-  n_images = 0;
-  nfeat.clear();
-  row0.clear();
-  cams.clear();
-  max_feat = max_feat_pad = 0;
-  total_rows = 0;
-}
-void Workspace::release() {
-  if (d_mbuf) cudaFree(d_mbuf);
-  if (d_aux) cudaFree(d_aux);
-  if (d_cand_cnt) cudaFree(d_cand_cnt);
-  if (d_cand_rows) cudaFree(d_cand_rows);
-  if (d_cand_sorted) cudaFree(d_cand_sorted);
-  if (d_pairs_dir1) cudaFree(d_pairs_dir1);
-  d_pairs_dir1 = nullptr;
-  cudaFree(d_gath_desc); cudaFree(d_colrank); cudaFree(d_gath_cols); cudaFree(d_gath_cnt); cudaFree(d_gath_items);
-  cudaFree(d_gath_n);
-  d_gath_desc = nullptr; d_colrank = nullptr; d_gath_cols = nullptr; d_gath_cnt = nullptr; d_gath_items = nullptr;
-  d_gath_n = nullptr;
-  d_cand_sorted = nullptr;
-  d_mbuf = nullptr;
-  d_aux = nullptr;
-  d_cand_cnt = nullptr;
-  d_cand_rows = nullptr;
-  for (int s = 0; s < 2; ++s) {
-    if (d_arena[s]) cudaFree(d_arena[s]);
-    if (d_cursor[s]) cudaFree(d_cursor[s]);
-    if (d_pair_off[s]) cudaFree(d_pair_off[s]);
-    if (d_pair_cnt[s]) cudaFree(d_pair_cnt[s]);
-    if (h_arena[s]) cudaFreeHost(h_arena[s]);
-    if (h_cursor[s]) cudaFreeHost(h_cursor[s]);
-    if (h_pair_off[s]) cudaFreeHost(h_pair_off[s]);
-    if (h_pair_cnt[s]) cudaFreeHost(h_pair_cnt[s]);
-    d_arena[s] = nullptr;
-    d_cursor[s] = nullptr;
-    d_pair_off[s] = nullptr;
-    d_pair_cnt[s] = nullptr;
-    h_arena[s] = nullptr;
-    h_cursor[s] = nullptr;
-    h_pair_off[s] = nullptr;
-    h_pair_cnt[s] = nullptr;
-  }
-  batch = 0;
-  mstride = 0;
-}
-}  // namespace b2m
 
 extern "C" {
 
@@ -786,7 +683,8 @@ int b2m_create(const b2m_device_cfg* cfg, b2m_ctx** out) {
              prop.minor);
     return fail(nullptr, B2M_ENODEV, b);
   }
-  b2m_ctx* ctx = new (std::nothrow) b2m_ctx();
+  // on a failure below, `ctx` and every stream, event and buffer created so far are destroyed on return
+  std::unique_ptr<b2m_ctx> ctx(new (std::nothrow) b2m_ctx());
   if (!ctx) return fail(nullptr, B2M_ENOMEM, "out of host memory");
   ctx->device = dev;
   ctx->num_sms = prop.multiProcessorCount;
@@ -796,32 +694,25 @@ int b2m_create(const b2m_device_cfg* cfg, b2m_ctx** out) {
     ctx->pair_batch_auto = false;
   }
   ctx->stats.struct_size = sizeof(b2m_stats);
-#define CU_TRY_C(expr)                                                            \
-  do {                                                                            \
-    cudaError_t _e = (expr);                                                      \
-    if (_e != cudaSuccess) {                                                      \
-      std::string m = std::string("[api.cu] CUDA error in b2m_create: ") + cudaGetErrorString(_e); \
-      delete ctx;                                                                 \
-      return fail(nullptr, B2M_ECUDA, m);                                         \
-    }                                                                             \
-  } while (0)
-  CU_TRY_C(cudaSetDevice(dev));
-  CU_TRY_C(cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking));
-  CU_TRY_C(cudaStreamCreateWithFlags(&ctx->copy_stream, cudaStreamNonBlocking));
-  CU_TRY_C(cudaStreamCreateWithFlags(&ctx->aux_stream, cudaStreamNonBlocking));
+  B2M_CUDA_TRY(nullptr, cudaSetDevice(dev));
+  B2M_CUDA_TRY(nullptr, ctx->stream.create(cudaStreamNonBlocking));
+  B2M_CUDA_TRY(nullptr, ctx->copy_stream.create(cudaStreamNonBlocking));
+  B2M_CUDA_TRY(nullptr, ctx->aux_stream.create(cudaStreamNonBlocking));
   for (int s = 0; s < 2; ++s) {
-    CU_TRY_C(cudaEventCreate(&ctx->ev_k[s]));
-    CU_TRY_C(cudaEventCreateWithFlags(&ctx->ev_data[s], cudaEventDisableTiming));
+    B2M_CUDA_TRY(nullptr, ctx->ev_k[s].create(cudaEventDefault));
+    B2M_CUDA_TRY(nullptr, ctx->ev_data[s].create(cudaEventDisableTiming));
   }
   for (int s = 0; s < 2; ++s) {
-    CU_TRY_C(cudaEventCreate(&ctx->ev_k1a[s]));
-    CU_TRY_C(cudaEventCreate(&ctx->ev_k1b[s]));
-    CU_TRY_C(cudaEventCreateWithFlags(&ctx->ev_p1[s], cudaEventDisableTiming));
-    CU_TRY_C(cudaEventCreate(&ctx->ev_g2a[s]));
-    CU_TRY_C(cudaEventCreate(&ctx->ev_g2b[s]));
+    B2M_CUDA_TRY(nullptr, ctx->ev_k1a[s].create(cudaEventDefault));
+    B2M_CUDA_TRY(nullptr, ctx->ev_k1b[s].create(cudaEventDefault));
+    B2M_CUDA_TRY(nullptr, ctx->ev_p1[s].create(cudaEventDisableTiming));
+    B2M_CUDA_TRY(nullptr, ctx->ev_g2a[s].create(cudaEventDefault));
+    B2M_CUDA_TRY(nullptr, ctx->ev_g2b[s].create(cudaEventDefault));
   }
-  CU_TRY_C(cudaEventCreate(&ctx->ev_t0));
-  CU_TRY_C(cudaEventCreate(&ctx->ev_t1));
+  B2M_CUDA_TRY(nullptr, ctx->ev_t0.create(cudaEventDefault));
+  B2M_CUDA_TRY(nullptr, ctx->ev_t1.create(cudaEventDefault));
+  B2M_CUDA_TRY(nullptr, ctx->d_counters.ensure(kNumCounters));
+  B2M_CUDA_TRY(nullptr, cudaMemset(ctx->d_counters, 0, sizeof(unsigned long long) * kNumCounters));
   // acos LUT: the float32 accept test of FindBestMatchesOneWayBruteForce depends only on the
   // integer dot product d in [0, 2^18] (clamped); tabulating it with the HOST libm makes the
   // device decisions identical to a CPU run on the same machine.
@@ -839,11 +730,10 @@ int b2m_create(const b2m_device_cfg* cfg, b2m_ctx** out) {
     if (d1 && !strcmp(d1, "full")) ctx->k1_dir1_mode = B2M_K1_DIR1_FULL_FORCED;
     if (d1 && !strcmp(d1, "skip")) ctx->k1_dir1_mode = B2M_K1_DIR1_SKIP_FORCED;
     if (d1 && !strcmp(d1, "gather")) ctx->k1_dir1_mode = B2M_K1_DIR1_GATHER_FORCED;
-    CU_TRY_C(cudaMalloc(&ctx->d_lut, sizeof(float) * lut.size()));
-    CU_TRY_C(cudaMemcpy(ctx->d_lut, lut.data(), sizeof(float) * lut.size(), cudaMemcpyHostToDevice));
+    B2M_CUDA_TRY(nullptr, ctx->d_lut.ensure(lut.size()));
+    B2M_CUDA_TRY(nullptr, cudaMemcpy(ctx->d_lut, lut.data(), sizeof(float) * lut.size(), cudaMemcpyHostToDevice));
   }
-#undef CU_TRY_C
-  *out = ctx;
+  *out = ctx.release();
   return B2M_OK;
 }
 
@@ -852,29 +742,9 @@ void b2m_destroy(b2m_ctx* ctx) {
   cudaSetDevice(ctx->device);
   cudaDeviceSynchronize();
   comm_release(ctx);
-  if (ctx->d_verify_counters) cudaFree(ctx->d_verify_counters);
-  if (ctx->d_abs_counters) cudaFree(ctx->d_abs_counters);
   tri_release(ctx);
   sift_release(ctx);
-  ctx->images.release();
-  ctx->ws.release();
   verify_release(ctx);
-  if (ctx->d_pairs) cudaFree(ctx->d_pairs);
-  if (ctx->d_lut) cudaFree(ctx->d_lut);
-  for (int s = 0; s < 2; ++s) {
-    if (ctx->ev_k[s]) cudaEventDestroy(ctx->ev_k[s]);
-    if (ctx->ev_data[s]) cudaEventDestroy(ctx->ev_data[s]);
-    if (ctx->ev_k1a[s]) cudaEventDestroy(ctx->ev_k1a[s]);
-    if (ctx->ev_k1b[s]) cudaEventDestroy(ctx->ev_k1b[s]);
-    if (ctx->ev_p1[s]) cudaEventDestroy(ctx->ev_p1[s]);
-    if (ctx->ev_g2a[s]) cudaEventDestroy(ctx->ev_g2a[s]);
-    if (ctx->ev_g2b[s]) cudaEventDestroy(ctx->ev_g2b[s]);
-  }
-  if (ctx->ev_t0) cudaEventDestroy(ctx->ev_t0);
-  if (ctx->ev_t1) cudaEventDestroy(ctx->ev_t1);
-  if (ctx->stream) cudaStreamDestroy(ctx->stream);
-  if (ctx->copy_stream) cudaStreamDestroy(ctx->copy_stream);
-  if (ctx->aux_stream) cudaStreamDestroy(ctx->aux_stream);
   delete ctx;
 }
 
@@ -891,17 +761,17 @@ static int set_images_impl(b2m_ctx* ctx, int32_t n_images, const int32_t* n_feat
   if (!ctx) return B2M_EINVAL;
   if (n_images < 0 || (n_images > 0 && (!n_feat || !desc)))
     return fail(ctx, B2M_EINVAL, "[api.cu] Check Failed: n_images >= 0 && n_feat && desc");
-  CU_TRY(ctx, cudaSetDevice(ctx->device));
+  B2M_CUDA_TRY(ctx, cudaSetDevice(ctx->device));
   ImageSet& S = ctx->images;
   if (int rc = layout_images(ctx, S, n_images, n_feat, kpts != nullptr)) return rc;
   for (int i = 0; i < n_images; ++i) {
     if (n_feat[i] == 0) continue;
     if (!desc[i]) return fail(ctx, B2M_EINVAL, "[api.cu] Check Failed: desc[i] != NULL");
-    CU_TRY(ctx, cudaMemcpyAsync(S.d_desc + static_cast<size_t>(S.row0[i]) * 128, desc[i],
+    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(S.d_desc + static_cast<size_t>(S.row0[i]) * 128, desc[i],
                                 static_cast<size_t>(n_feat[i]) * 128, cudaMemcpyHostToDevice, ctx->stream));
     if (kpts) {
       if (!kpts[i]) return fail(ctx, B2M_EINVAL, "[api.cu] Check Failed: kpts[i] != NULL");
-      CU_TRY(ctx, cudaMemcpyAsync(S.d_kpts + S.row0[i], kpts[i], static_cast<size_t>(n_feat[i]) * sizeof(float2),
+      B2M_CUDA_TRY(ctx, cudaMemcpyAsync(S.d_kpts + S.row0[i], kpts[i], static_cast<size_t>(n_feat[i]) * sizeof(float2),
                                   cudaMemcpyHostToDevice, ctx->stream));
     }
   }
@@ -910,7 +780,7 @@ static int set_images_impl(b2m_ctx* ctx, int32_t n_images, const int32_t* n_feat
       if (const char* why = camera_problem(cams[i])) return fail(ctx, B2M_EINVAL, why);
     S.cams.assign(cams, cams + n_images);
   }
-  CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+  B2M_CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
   return B2M_OK;
 }
 
@@ -926,7 +796,7 @@ static int set_images_device_impl(b2m_ctx* ctx, int32_t n_images, const int32_t*
   if (!ctx) return B2M_EINVAL;
   if (n_images < 0 || (n_images > 0 && (!n_feat || !dev_desc_packed)))
     return fail(ctx, B2M_EINVAL, "[api.cu] Check Failed: n_images >= 0 && n_feat && dev_desc_packed");
-  CU_TRY(ctx, cudaSetDevice(ctx->device));
+  B2M_CUDA_TRY(ctx, cudaSetDevice(ctx->device));
   ImageSet& S = ctx->images;
   if (int rc = layout_images(ctx, S, n_images, n_feat, dev_kpts_packed != nullptr)) return rc;
   int64_t src_row = 0;
@@ -943,10 +813,10 @@ static int set_images_device_impl(b2m_ctx* ctx, int32_t n_images, const int32_t*
       j = i + 1;
     }
     if (run > 0) {
-      CU_TRY(ctx, cudaMemcpyAsync(S.d_desc + static_cast<size_t>(S.row0[i]) * 128, src + src_row * 128,
+      B2M_CUDA_TRY(ctx, cudaMemcpyAsync(S.d_desc + static_cast<size_t>(S.row0[i]) * 128, src + src_row * 128,
                                   static_cast<size_t>(run) * 128, cudaMemcpyDeviceToDevice, ctx->stream));
       if (ksrc)
-        CU_TRY(ctx, cudaMemcpyAsync(S.d_kpts + S.row0[i], ksrc + src_row, static_cast<size_t>(run) * sizeof(float2),
+        B2M_CUDA_TRY(ctx, cudaMemcpyAsync(S.d_kpts + S.row0[i], ksrc + src_row, static_cast<size_t>(run) * sizeof(float2),
                                     cudaMemcpyDeviceToDevice, ctx->stream));
     }
     src_row += run;
@@ -957,7 +827,7 @@ static int set_images_device_impl(b2m_ctx* ctx, int32_t n_images, const int32_t*
       if (const char* why = camera_problem(cams[i])) return fail(ctx, B2M_EINVAL, why);
     S.cams.assign(cams, cams + n_images);
   }
-  CU_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+  B2M_CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
   return B2M_OK;
 }
 
@@ -985,13 +855,13 @@ static int set_images_sharded_impl(b2m_ctx* ctx, int32_t n_images, const int32_t
   if (cams)
     for (int i = 0; i < n_images; ++i)
       if (const char* why = camera_problem(cams[i])) return fail(ctx, B2M_EINVAL, why);
-  CU_TRY(ctx, cudaSetDevice(ctx->device));
+  B2M_CUDA_TRY(ctx, cudaSetDevice(ctx->device));
   ImageSet& S = ctx->images;
   const bool kp = mine->has_keypoints != 0;
   if (int rc = layout_images(ctx, S, n_images, n_feat, kp)) return rc;
   cudaStream_t st = ctx->stream;
   const cudaMemcpyKind kind = mine->location == B2M_LOC_HOST ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice;
-  CU_TRY(ctx, cudaEventRecord(ctx->ev_t0, st));
+  B2M_CUDA_TRY(ctx, cudaEventRecord(ctx->ev_t0, st));
   {  // the local shard -> its rows; runs of images without padding go in one copy
     const uint8_t* src = static_cast<const uint8_t*>(mine->desc_packed);
     const float2* ksrc = static_cast<const float2*>(mine->kpts_packed);
@@ -1006,16 +876,16 @@ static int set_images_sharded_impl(b2m_ctx* ctx, int32_t n_images, const int32_t
         j = i + 1;
       }
       if (run > 0) {
-        CU_TRY(ctx, cudaMemcpyAsync(S.d_desc + static_cast<size_t>(S.row0[i]) * 128, src + src_row * 128,
+        B2M_CUDA_TRY(ctx, cudaMemcpyAsync(S.d_desc + static_cast<size_t>(S.row0[i]) * 128, src + src_row * 128,
                                     static_cast<size_t>(run) * 128, kind, st));
         if (kp)
-          CU_TRY(ctx, cudaMemcpyAsync(S.d_kpts + S.row0[i], ksrc + src_row, static_cast<size_t>(run) * sizeof(float2), kind, st));
+          B2M_CUDA_TRY(ctx, cudaMemcpyAsync(S.d_kpts + S.row0[i], ksrc + src_row, static_cast<size_t>(run) * sizeof(float2), kind, st));
       }
       src_row += run;
       i = j;
     }
   }
-  CU_TRY(ctx, cudaEventRecord(ctx->ev_k1a[0], st));
+  B2M_CUDA_TRY(ctx, cudaEventRecord(ctx->ev_k1a[0], st));
   uint64_t recv_bytes = 0;
   if (ctx->comm && ctx->comm_size > 1) {
     // ONE all-gather of the descriptor rows (and one of the keypoint rows): rank r owns the padded rows of its images
@@ -1034,12 +904,12 @@ static int set_images_sharded_impl(b2m_ctx* ctx, int32_t n_images, const int32_t
     if (int rc = comm_allgather_regions(ctx, S.d_desc, o, l, st)) return rc;
     if (kp) {
       for (int r = 0; r < nr; ++r) { o[r] = off[r] * sizeof(float2); l[r] = len[r] * sizeof(float2); }
-      if (int rc = comm_allgather_regions(ctx, reinterpret_cast<uint8_t*>(S.d_kpts), o, l, st)) return rc;
+      if (int rc = comm_allgather_regions(ctx, reinterpret_cast<uint8_t*>(static_cast<float2*>(S.d_kpts)), o, l, st)) return rc;
     }
   }
-  CU_TRY(ctx, cudaEventRecord(ctx->ev_k1b[0], st));
+  B2M_CUDA_TRY(ctx, cudaEventRecord(ctx->ev_k1b[0], st));
   if (cams) S.cams.assign(cams, cams + n_images);
-  CU_TRY(ctx, cudaStreamSynchronize(st));
+  B2M_CUDA_TRY(ctx, cudaStreamSynchronize(st));
   float up = 0.f, ag = 0.f;
   cudaEventElapsedTime(&up, ctx->ev_t0, ctx->ev_k1a[0]);
   cudaEventElapsedTime(&ag, ctx->ev_k1a[0], ctx->ev_k1b[0]);
@@ -1149,30 +1019,17 @@ int b2m_get_stats(b2m_ctx* ctx, b2m_stats* out) {
   out->struct_size = sizeof(b2m_stats);
   out->comm_size = ctx->comm_size;
   out->comm_rank = ctx->comm_rank;
-  if (ctx->d_verify_counters) {  // kernel-side counters of the verifier (models scored, residual evaluations per kind)
-    unsigned long long h[6] = {0, 0, 0, 0, 0, 0};
-    cudaSetDevice(ctx->device);
-    if (cudaMemcpy(h, ctx->d_verify_counters, sizeof(h), cudaMemcpyDeviceToHost) == cudaSuccess)
-      for (int k = 0; k < 3; ++k) {
-        out->verify_models_scored[k] = h[k];
-        out->verify_residuals[k] = h[3 + k];
-      }
-  }
-  if (ctx->d_abs_counters) {  // same for the absolute pose estimator
-    unsigned long long h[2] = {0, 0};
-    cudaSetDevice(ctx->device);
-    if (cudaMemcpy(h, ctx->d_abs_counters, sizeof(h), cudaMemcpyDeviceToHost) == cudaSuccess) {
-      out->abs_pose_models_scored = h[0];
-      out->abs_pose_residuals = h[1];
+  unsigned long long h[kNumCounters];  // kernel-side counters: models scored, residual evaluations
+  cudaSetDevice(ctx->device);
+  if (cudaMemcpy(h, ctx->d_counters, sizeof(h), cudaMemcpyDeviceToHost) == cudaSuccess) {
+    for (int k = 0; k < 3; ++k) {
+      out->verify_models_scored[k] = h[kVerifyCounters + k];
+      out->verify_residuals[k] = h[kVerifyCounters + 3 + k];
     }
-  }
-  {
-    unsigned long long h[2] = {0, 0};
-    cudaSetDevice(ctx->device);
-    if (tri_counters(ctx, h)) {  // and for triangulation
-      out->tri_models_scored = h[0];
-      out->tri_residuals = h[1];
-    }
+    out->abs_pose_models_scored = h[kAbsPoseCounters];
+    out->abs_pose_residuals = h[kAbsPoseCounters + 1];
+    out->tri_models_scored = h[kTriCounters];
+    out->tri_residuals = h[kTriCounters + 1];
   }
   return B2M_OK;
 }
@@ -1180,16 +1037,8 @@ int b2m_reset_stats(b2m_ctx* ctx) {
   if (!ctx) return B2M_EINVAL;
   memset(&ctx->stats, 0, sizeof(ctx->stats));
   ctx->stats.struct_size = sizeof(b2m_stats);
-  if (ctx->d_verify_counters) {
-    cudaSetDevice(ctx->device);
-    cudaMemset(ctx->d_verify_counters, 0, sizeof(unsigned long long) * 6);
-  }
-  if (ctx->d_abs_counters) {
-    cudaSetDevice(ctx->device);
-    cudaMemset(ctx->d_abs_counters, 0, sizeof(unsigned long long) * 2);
-  }
   cudaSetDevice(ctx->device);
-  tri_reset_counters(ctx);
+  cudaMemset(ctx->d_counters, 0, sizeof(unsigned long long) * kNumCounters);
   ctx->stats.k1_dir1_mode = static_cast<uint64_t>(ctx->k1_dir1_mode);  // a property of the context, not a counter
   return B2M_OK;
 }

@@ -10,6 +10,7 @@
 
 #include "../../include/b200match.h"
 #include "camera_models.h"
+#include "cuda_owned.cuh"
 
 namespace b2m {
 
@@ -35,47 +36,56 @@ struct ImageSet {
   int32_t max_feat = 0;      // max valid rows
   int32_t max_feat_pad = 0;  // max padded rows
   int64_t total_rows = 0;    // padded rows over all images
-  uint8_t* d_desc = nullptr;
-  float2* d_kpts = nullptr;  // indexed by padded row, or nullptr
-  int32_t* d_row0 = nullptr;
-  int32_t* d_nfeat = nullptr;
+  DeviceArray<uint8_t> d_desc;
+  DeviceArray<float2> d_kpts;  // indexed by padded row, or empty
+  DeviceArray<int32_t> d_row0;
+  DeviceArray<int32_t> d_nfeat;
   std::vector<b2m_camera> cams;
   uint64_t generation = 0;  // bumped by every b2m_set_images*: consumers caching per-set state (device cameras)
                             // key on this, not on d_desc (the allocator may hand the same address out again)
   CUtensorMap tmap{};       // box 128 bytes x 128 rows
-  void release();
+  void release() { *this = ImageSet(); }
+};
+
+// Scratch of the gathered column direction (launch_k1_filter_gather), allocated on first use.
+struct GatherBufs {
+  DeviceArray<uint8_t> desc;    // [batch x mstride x 128]
+  DeviceArray<int32_t> colrank; // [batch][mstride]
+  DeviceArray<int32_t> cols;    // [batch][mstride]
+  DeviceArray<int32_t> cnt;     // [batch]
+  DeviceArray<int32_t> items;   // [batch x mstride / 256][2]
+  DeviceArray<int32_t> n;       // [1]
+  CUtensorMap tmap{};
 };
 
 struct Workspace {
   int batch = 0;
   int32_t mstride = 0;
-  int32_t* d_mbuf = nullptr;
-  uint2* d_aux = nullptr;          // K1 v2: (best, S1) per candidate row
-  int32_t* d_cand_cnt = nullptr;   // K1 v2: [batch][2]
-  int32_t* d_cand_rows = nullptr;  // K1 v2: [batch][2][mstride]
-  int32_t* d_cand_sorted = nullptr;
-  int32_t* d_pairs_dir1 = nullptr; // [batch][2] swapped / dummy pairs of launch_k1_filter_skip
-  // gathered column direction (launch_k1_filter_gather), allocated on first use
-  uint8_t* d_gath_desc = nullptr;  // [batch x mstride x 128]
-  int32_t* d_colrank = nullptr;    // [batch][mstride]
-  int32_t* d_gath_cols = nullptr;  // [batch][mstride]
-  int32_t* d_gath_cnt = nullptr;   // [batch]
-  int32_t* d_gath_items = nullptr; // [batch x mstride / 256][2]
-  int32_t* d_gath_n = nullptr;     // [1]
-  CUtensorMap tmap_gath{};
-  uint2* d_arena[2] = {nullptr, nullptr};
-  unsigned long long* d_cursor[2] = {nullptr, nullptr};
-  int64_t* d_pair_off[2] = {nullptr, nullptr};
-  int32_t* d_pair_cnt[2] = {nullptr, nullptr};
-  uint2* h_arena[2] = {nullptr, nullptr};
-  unsigned long long* h_cursor[2] = {nullptr, nullptr};
-  int64_t* h_pair_off[2] = {nullptr, nullptr};
-  int32_t* h_pair_cnt[2] = {nullptr, nullptr};
-  void release();
+  DeviceArray<int32_t> d_mbuf;
+  DeviceArray<uint2> d_aux;           // K1 v2: (best, S1) per candidate row
+  DeviceArray<int32_t> d_cand_cnt;    // K1 v2: [batch][2]
+  DeviceArray<int32_t> d_cand_rows;   // K1 v2: [batch][2][mstride]
+  DeviceArray<int32_t> d_cand_sorted;
+  DeviceArray<int32_t> d_pairs_dir1;  // [batch][2] swapped / dummy pairs of launch_k1_filter_skip
+  GatherBufs gath;
+  DeviceArray<uint2> d_arena[2];
+  DeviceArray<unsigned long long> d_cursor[2];
+  DeviceArray<int64_t> d_pair_off[2];
+  DeviceArray<int32_t> d_pair_cnt[2];
+  PinnedArray<uint2> h_arena[2];
+  PinnedArray<unsigned long long> h_cursor[2];
+  PinnedArray<int64_t> h_pair_off[2];
+  PinnedArray<int32_t> h_pair_cnt[2];
 };
 
 // message of a failing call that has no context to carry it (b2m_create, b2m_comm_get_unique_id)
 extern thread_local std::string g_noctx_err;
+
+// Indices into b2m_ctx::d_counters, the kernel-side counters behind b2m_stats: models scored, then residual evaluations.
+constexpr int kVerifyCounters = 0;    // [6]: per model kind E, F, H (verify.cu)
+constexpr int kAbsPoseCounters = 6;   // [2] (abs_pose.cu)
+constexpr int kTriCounters = 8;       // [2] (triangulation.cu)
+constexpr int kNumCounters = 10;
 
 }  // namespace b2m
 
@@ -94,21 +104,21 @@ struct b2m_ctx {
   bool pair_batch_auto = true;  // no explicit b2m_device_cfg.pair_batch: the batch scales with the image size (api.cu)
   int pair_batch = 4096;  // pairs per kernel batch: ~380 verifiable pairs x 3 model kinds per launch keep the RANSAC
                           // kernels at several CTAs per SM
-  cudaStream_t stream = nullptr;
-  cudaStream_t copy_stream = nullptr;
-  cudaEvent_t ev_k[2] = {nullptr, nullptr};
-  cudaEvent_t ev_data[2] = {nullptr, nullptr};
-  cudaEvent_t ev_t0 = nullptr, ev_t1 = nullptr;
-  cudaEvent_t ev_k1a[2] = {nullptr, nullptr}, ev_k1b[2] = {nullptr, nullptr};
+  b2m::Stream stream;
+  b2m::Stream copy_stream;
+  b2m::Event ev_k[2];
+  b2m::Event ev_data[2];
+  b2m::Event ev_t0, ev_t1;
+  b2m::Event ev_k1a[2], ev_k1b[2];
   // overlapped schedule (api.cu): exact resolve + gather of batch b run on `aux_stream` next to the RANSAC kernels of
   // batch b - 1; ev_p1 = that work done, ev_g2a / ev_g2b bracket the gathered GEMM (timing)
-  cudaStream_t aux_stream = nullptr;
-  cudaEvent_t ev_p1[2] = {nullptr, nullptr}, ev_g2a[2] = {nullptr, nullptr}, ev_g2b[2] = {nullptr, nullptr};
-  float* d_lut = nullptr;
+  b2m::Stream aux_stream;
+  b2m::Event ev_p1[2], ev_g2a[2], ev_g2b[2];
+  b2m::DeviceArray<float> d_lut;
+  b2m::DeviceArray<unsigned long long> d_counters;  // [kNumCounters], zeroed by b2m_create and b2m_reset_stats
   b2m::ImageSet images;
   b2m::Workspace ws;
-  int32_t* d_pairs = nullptr;
-  int64_t d_pairs_cap = 0;
+  b2m::DeviceArray<int32_t> d_pairs;
   std::string err;
   volatile int stop = 0;
   bool exact_k1 = false;  // use the exact top-2 epilogue (K1 v1) instead of filter + resolve (K1 v2)
@@ -119,17 +129,18 @@ struct b2m_ctx {
   // multi-GPU (comm.cu): the NCCL communicator this context joined, or nullptr
   void* comm = nullptr;          // ncclComm_t
   int comm_size = 1, comm_rank = 0;
-  unsigned long long* d_verify_counters = nullptr;  // [6]: models scored / residual evaluations per kind (verify.cu)
-  unsigned long long* d_abs_counters = nullptr;     // [2]: models scored / residual evaluations (abs_pose.cu)
-  void* tri_state = nullptr;     // b2m::TriState (triangulation.cu): pinned staging, device buffers, counters
+  void* tri_state = nullptr;     // b2m::TriState (triangulation.cu): pinned staging and device buffers
   void* sift_state = nullptr;    // b2m::SiftState (sift.cu): pyramid, gradient and keypoint buffers
 };
 
 namespace b2m {
+// Sets the error message of `ctx` (nullptr: of the calling thread) and returns `code`.
+inline int fail(b2m_ctx* ctx, int code, const std::string& msg) {
+  if (ctx) ctx->err = msg; else g_noctx_err = msg;
+  return code;
+}
 // triangulation.cu
 void tri_release(b2m_ctx* ctx);
-bool tri_counters(b2m_ctx* ctx, unsigned long long* out);  // [2]: models scored, residual evaluations
-void tri_reset_counters(b2m_ctx* ctx);
 // sift.cu
 void sift_release(b2m_ctx* ctx);
 }  // namespace b2m

@@ -538,55 +538,30 @@ __global__ void __launch_bounds__(32 * kDescWarps) b2m_sift_descriptor_kernel(co
 }
 
 // ---- host side ---------------------------------------------------------------------------------------------------
-#define S_TRY(ctx, expr)                                                                            \
-  do {                                                                                              \
-    cudaError_t _e = (expr);                                                                        \
-    if (_e != cudaSuccess) {                                                                        \
-      (ctx)->err = std::string("[sift.cu:") + std::to_string(__LINE__) + "] CUDA error: " +       \
-                   cudaGetErrorString(_e) + " (" #expr ")";                                        \
-      return B2M_ECUDA;                                                                             \
-    }                                                                                               \
-  } while (0)
+// Buffers of the Gaussian pyramid: sized by the largest first octave and the number of levels, replaced together.
+struct SiftPyramid {
+  int64_t cap_px = 0;
+  int cap_levels = 0;
+  DeviceArray<uint8_t> d_img;
+  DeviceArray<float> d_G, d_D, d_T, d_U;
+};
+
+// Fixed-size buffers, allocated (and the exp table uploaded) by the first call.
+struct SiftTables {
+  DeviceArray<int> d_total, d_nang;
+  DeviceArray<double> d_ang;
+  DeviceArray<Kp> d_kp;
+  DeviceArray<float> d_taps;
+};
 
 struct SiftState {
-  int64_t cap_px = 0, cap_grad = 0, cap_blocks = 0, cap_ent = 0;
-  int cap_levels = 0;
-  uint8_t* d_img = nullptr;
-  float *d_G = nullptr, *d_D = nullptr, *d_T = nullptr, *d_U = nullptr, *d_taps = nullptr;
-  float2* d_grad = nullptr;
-  int *d_counts = nullptr, *d_offs = nullptr, *d_total = nullptr, *d_nang = nullptr;
-  Kp* d_kp = nullptr;
-  double* d_ang = nullptr;
-  DescEntry* d_ent = nullptr;
-  float* d_kout = nullptr;
-  uint8_t* d_dout = nullptr;
-  bool table = false;
-  void release_px() {
-    for (void* p : {static_cast<void*>(d_img), static_cast<void*>(d_G), static_cast<void*>(d_D), static_cast<void*>(d_T),
-                    static_cast<void*>(d_U)})
-      if (p) cudaFree(p);
-    d_img = nullptr;
-    d_G = d_D = d_T = d_U = nullptr;
-    cap_px = 0;
-    cap_levels = 0;
-  }
-  void release() {
-    release_px();
-    for (void* p : {static_cast<void*>(d_grad), static_cast<void*>(d_counts), static_cast<void*>(d_offs),
-                    static_cast<void*>(d_total), static_cast<void*>(d_nang), static_cast<void*>(d_kp),
-                    static_cast<void*>(d_ang), static_cast<void*>(d_ent), static_cast<void*>(d_kout),
-                    static_cast<void*>(d_dout), static_cast<void*>(d_taps)})
-      if (p) cudaFree(p);
-    d_grad = nullptr;
-    d_counts = d_offs = d_total = d_nang = nullptr;
-    d_kp = nullptr;
-    d_ang = nullptr;
-    d_ent = nullptr;
-    d_kout = nullptr;
-    d_dout = nullptr;
-    d_taps = nullptr;
-    cap_grad = cap_blocks = cap_ent = 0;
-  }
+  SiftPyramid px;
+  SiftTables tab;
+  DeviceArray<float2> d_grad;
+  DeviceArray<int> d_counts, d_offs;
+  DeviceArray<DescEntry> d_ent;
+  DeviceArray<float> d_kout;
+  DeviceArray<uint8_t> d_dout;
 };
 
 // _vl_sift_smooth's kernel: half-width max(ceil(4 sigma), 1), fp32 taps normalised by their fp32 running sum
@@ -632,17 +607,17 @@ int extract_one(b2m_ctx* ctx, SiftState* S, const b2m_image& im, const b2m_extra
   dims(o_min, &w0, &h0);
   const int64_t A0 = static_cast<int64_t>(w0) * h0;
   // base level
-  S_TRY(ctx, cudaMemcpy2DAsync(S->d_img, W, im.data, im.stride, W, H, cudaMemcpyHostToDevice, st));
-  float* G = S->d_G;
+  B2M_CUDA_TRY(ctx, cudaMemcpy2DAsync(S->px.d_img, W, im.data, im.stride, W, H, cudaMemcpyHostToDevice, st));
+  float* G = S->px.d_G;
   float* base = G;  // level s = -1
   {
-    float* a = o_min < 0 ? S->d_T : (o_min > 0 ? S->d_U : base);
-    b2m_sift_to_float_kernel<<<blocks_for(static_cast<int64_t>(W) * H, 256), 256, 0, st>>>(S->d_img, W, W, H, a);
+    float* a = o_min < 0 ? S->px.d_T : (o_min > 0 ? S->px.d_U : base);
+    b2m_sift_to_float_kernel<<<blocks_for(static_cast<int64_t>(W) * H, 256), 256, 0, st>>>(S->px.d_img, W, W, H, a);
     ctx->stats.kernel_launches += 1;
     if (o_min < 0) {
       int w = W, h = H;
       for (int k = 0; k < -o_min; ++k) {
-        float* dst = (k == -o_min - 1) ? base : (a == S->d_T ? S->d_U : S->d_T);
+        float* dst = (k == -o_min - 1) ? base : (a == S->px.d_T ? S->px.d_U : S->px.d_T);
         b2m_sift_upsample_kernel<<<blocks_for(4LL * w * h, 256), 256, 0, st>>>(a, w, h, dst);
         ctx->stats.kernel_launches += 1;
         a = dst;
@@ -654,15 +629,15 @@ int extract_one(b2m_ctx* ctx, SiftState* S, const b2m_image& im, const b2m_extra
       ctx->stats.kernel_launches += 1;
     }
   }
-  S_TRY(ctx, cudaGetLastError());
+  B2M_CUDA_TRY(ctx, cudaGetLastError());
   auto blur = [&](const float* in, int w, int h, int f, float* out, const float* prev, float* dog) {
     const int64_t n = static_cast<int64_t>(w) * h;
     const int R = tap_r[f];
     const dim3 bv((w + 31) / 32, (h + kBlurRowsV - 1) / kBlurRowsV), bh((w + kBlurColsH - 1) / kBlurColsH, (h + 7) / 8);
     b2m_sift_blur_v_kernel<<<bv, dim3(32, 8), sizeof(float) * (2 * R + 1 + 32 * (kBlurRowsV + 2 * R)), st>>>(
-        in, w, h, S->d_taps + tap_off[f], R, S->d_T);
+        in, w, h, S->tab.d_taps + tap_off[f], R, S->px.d_T);
     b2m_sift_blur_h_dog_kernel<<<bh, dim3(32, 8), sizeof(float) * (2 * R + 1 + 8 * (kBlurColsH + 2 * R)), st>>>(
-        S->d_T, w, h, S->d_taps + tap_off[f], R, out,
+        S->px.d_T, w, h, S->tab.d_taps + tap_off[f], R, out,
                                                                    prev, dog);
     ctx->stats.kernel_launches += 2;
   };
@@ -670,7 +645,7 @@ int extract_one(b2m_ctx* ctx, SiftState* S, const b2m_image& im, const b2m_extra
   OctTab T{};
   T.o_min = o_min;
   int64_t goff = 0;
-  S_TRY(ctx, cudaMemsetAsync(S->d_total, 0, sizeof(int), st));
+  B2M_CUDA_TRY(ctx, cudaMemsetAsync(S->tab.d_total, 0, sizeof(int), st));
   const int nlev = Sr + 3;
   const int n_oct = num_octaves_built(W, H, op);
   for (int o = o_min; o < o_min + n_oct; ++o) {
@@ -680,13 +655,13 @@ int extract_one(b2m_ctx* ctx, SiftState* S, const b2m_image& im, const b2m_extra
     if (o > o_min) {  // level S - 1 of the previous octave at even indices (no extra smoothing: sa == sb)
       int pw, ph;
       dims(o - 1, &pw, &ph);
-      b2m_sift_subsample_kernel<<<blocks_for(A, 256), 256, 0, st>>>(G + static_cast<int64_t>(Sr) * A0, pw, 2, w, h, S->d_U);
-      S_TRY(ctx, cudaMemcpyAsync(G, S->d_U, sizeof(float) * A, cudaMemcpyDeviceToDevice, st));
+      b2m_sift_subsample_kernel<<<blocks_for(A, 256), 256, 0, st>>>(G + static_cast<int64_t>(Sr) * A0, pw, 2, w, h, S->px.d_U);
+      B2M_CUDA_TRY(ctx, cudaMemcpyAsync(G, S->px.d_U, sizeof(float) * A, cudaMemcpyDeviceToDevice, st));
       ctx->stats.kernel_launches += 1;
     }
     for (int s = 1; s < nlev; ++s)  // level s - 1 of VLFeat's numbering; DoG s - 2 = G[s] - G[s - 1]
-      blur(G + (s - 1) * A0, w, h, s, G + s * A0, G + (s - 1) * A0, S->d_D + (s - 1) * A);
-    S_TRY(ctx, cudaGetLastError());
+      blur(G + (s - 1) * A0, w, h, s, G + s * A0, G + (s - 1) * A0, S->px.d_D + (s - 1) * A);
+    B2M_CUDA_TRY(ctx, cudaGetLastError());
     T.w[o - o_min] = w;
     T.h[o - o_min] = h;
     T.goff[o - o_min] = goff;
@@ -696,7 +671,7 @@ int extract_one(b2m_ctx* ctx, SiftState* S, const b2m_image& im, const b2m_extra
     ctx->stats.kernel_launches += Sr;
     goff += Sr * A;
     DetectParams P;
-    P.dog = S->d_D;
+    P.dog = S->px.d_D;
     P.w = w;
     P.h = h;
     P.S = Sr;
@@ -707,20 +682,20 @@ int extract_one(b2m_ctx* ctx, SiftState* S, const b2m_image& im, const b2m_extra
     P.n = static_cast<int64_t>(Sr) * (w - 2) * (h - 2);
     const unsigned nb = blocks_for(P.n, kDetectThreads);
     b2m_sift_detect_count_kernel<<<nb, kDetectThreads, 0, st>>>(P, S->d_counts);
-    b2m_sift_scan_kernel<<<1, 1024, 0, st>>>(S->d_counts, static_cast<int>(nb), S->d_offs, S->d_total);
-    b2m_sift_detect_write_kernel<<<nb, kDetectThreads, 0, st>>>(P, S->d_offs, S->d_kp);
+    b2m_sift_scan_kernel<<<1, 1024, 0, st>>>(S->d_counts, static_cast<int>(nb), S->d_offs, S->tab.d_total);
+    b2m_sift_detect_write_kernel<<<nb, kDetectThreads, 0, st>>>(P, S->d_offs, S->tab.d_kp);
     ctx->stats.kernel_launches += 3;
-    S_TRY(ctx, cudaGetLastError());
+    B2M_CUDA_TRY(ctx, cudaGetLastError());
   }
   int total = 0;
-  S_TRY(ctx, cudaMemcpyAsync(&total, S->d_total, sizeof(int), cudaMemcpyDeviceToHost, st));
-  S_TRY(ctx, cudaStreamSynchronize(st));
+  B2M_CUDA_TRY(ctx, cudaMemcpyAsync(&total, S->tab.d_total, sizeof(int), cudaMemcpyDeviceToHost, st));
+  B2M_CUDA_TRY(ctx, cudaStreamSynchronize(st));
   if (total > kKpCap) {
     ctx->err = "[sift.cu] more than 2^20 keypoints in one image before the max_num_features cut";
     return B2M_ENOMEM;
   }
   std::vector<Kp> kp(total);
-  if (total) S_TRY(ctx, cudaMemcpy(kp.data(), S->d_kp, sizeof(Kp) * total, cudaMemcpyDeviceToHost));
+  if (total) B2M_CUDA_TRY(ctx, cudaMemcpy(kp.data(), S->tab.d_kp, sizeof(Kp) * total, cudaMemcpyDeviceToHost));
   // max_num_features: (octave, level) runs from the coarsest down; the run that passes the limit is kept whole
   std::vector<int> run_start;
   for (int i = 0; i < total; ++i)
@@ -741,13 +716,13 @@ int extract_one(b2m_ctx* ctx, SiftState* S, const b2m_image& im, const b2m_extra
   std::vector<int> nang(nk, 1);
   std::vector<double> ang(4 * static_cast<size_t>(nk), 0.0);
   if (nk && !op.upright) {
-    b2m_sift_orientation_kernel<<<blocks_for(nk, kOriWarps), 32 * kOriWarps, 0, st>>>(S->d_kp + first, nk, T, S->d_grad,
-                                                                                    S->d_nang, S->d_ang);
+    b2m_sift_orientation_kernel<<<blocks_for(nk, kOriWarps), 32 * kOriWarps, 0, st>>>(S->tab.d_kp + first, nk, T, S->d_grad,
+                                                                                    S->tab.d_nang, S->tab.d_ang);
     ctx->stats.kernel_launches += 1;
-    S_TRY(ctx, cudaGetLastError());
-    S_TRY(ctx, cudaMemcpyAsync(nang.data(), S->d_nang, sizeof(int) * nk, cudaMemcpyDeviceToHost, st));
-    S_TRY(ctx, cudaMemcpyAsync(ang.data(), S->d_ang, sizeof(double) * 4 * nk, cudaMemcpyDeviceToHost, st));
-    S_TRY(ctx, cudaStreamSynchronize(st));
+    B2M_CUDA_TRY(ctx, cudaGetLastError());
+    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(nang.data(), S->tab.d_nang, sizeof(int) * nk, cudaMemcpyDeviceToHost, st));
+    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(ang.data(), S->tab.d_ang, sizeof(double) * 4 * nk, cudaMemcpyDeviceToHost, st));
+    B2M_CUDA_TRY(ctx, cudaStreamSynchronize(st));
   }
   std::vector<DescEntry> ent;
   for (int k = 0; k < nk; ++k)
@@ -757,27 +732,17 @@ int extract_one(b2m_ctx* ctx, SiftState* S, const b2m_image& im, const b2m_extra
   F->kpts.resize(4 * (f0 + ne));
   F->desc.resize(128 * (f0 + ne));
   if (ne) {
-    if (ne > S->cap_ent) {
-      if (S->d_ent) cudaFree(S->d_ent);
-      if (S->d_kout) cudaFree(S->d_kout);
-      if (S->d_dout) cudaFree(S->d_dout);
-      S->d_ent = nullptr;
-      S->d_kout = nullptr;
-      S->d_dout = nullptr;
-      S->cap_ent = 0;
-      S_TRY(ctx, cudaMalloc(&S->d_ent, sizeof(DescEntry) * ne));
-      S_TRY(ctx, cudaMalloc(&S->d_kout, sizeof(float) * 4 * ne));
-      S_TRY(ctx, cudaMalloc(&S->d_dout, 128 * static_cast<size_t>(ne)));
-      S->cap_ent = ne;
-    }
-    S_TRY(ctx, cudaMemcpyAsync(S->d_ent, ent.data(), sizeof(DescEntry) * ne, cudaMemcpyHostToDevice, st));
+    B2M_CUDA_TRY(ctx, S->d_ent.ensure(ne));
+    B2M_CUDA_TRY(ctx, S->d_kout.ensure(4 * static_cast<size_t>(ne)));
+    B2M_CUDA_TRY(ctx, S->d_dout.ensure(128 * static_cast<size_t>(ne)));
+    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(S->d_ent, ent.data(), sizeof(DescEntry) * ne, cudaMemcpyHostToDevice, st));
     b2m_sift_descriptor_kernel<<<blocks_for(ne, kDescWarps), 32 * kDescWarps, 0, st>>>(
-        S->d_kp, S->d_ent, ne, T, S->d_grad, op.normalization == B2M_NORMALIZATION_L2, S->d_kout, S->d_dout);
+        S->tab.d_kp, S->d_ent, ne, T, S->d_grad, op.normalization == B2M_NORMALIZATION_L2, S->d_kout, S->d_dout);
     ctx->stats.kernel_launches += 1;
-    S_TRY(ctx, cudaGetLastError());
-    S_TRY(ctx, cudaMemcpyAsync(F->kpts.data() + 4 * f0, S->d_kout, sizeof(float) * 4 * ne, cudaMemcpyDeviceToHost, st));
-    S_TRY(ctx, cudaMemcpyAsync(F->desc.data() + 128 * f0, S->d_dout, 128 * static_cast<size_t>(ne), cudaMemcpyDeviceToHost, st));
-    S_TRY(ctx, cudaStreamSynchronize(st));
+    B2M_CUDA_TRY(ctx, cudaGetLastError());
+    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(F->kpts.data() + 4 * f0, S->d_kout, sizeof(float) * 4 * ne, cudaMemcpyDeviceToHost, st));
+    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(F->desc.data() + 128 * f0, S->d_dout, 128 * static_cast<size_t>(ne), cudaMemcpyDeviceToHost, st));
+    B2M_CUDA_TRY(ctx, cudaStreamSynchronize(st));
   }
   F->off.push_back(static_cast<int64_t>(f0) + ne);
   ctx->stats.sift_images += 1;
@@ -789,12 +754,8 @@ int extract_one(b2m_ctx* ctx, SiftState* S, const b2m_image& im, const b2m_extra
 }  // namespace
 
 void sift_release(b2m_ctx* ctx) {
-  if (ctx && ctx->sift_state) {
-    SiftState* s = static_cast<SiftState*>(ctx->sift_state);
-    s->release();
-    delete s;
-    ctx->sift_state = nullptr;
-  }
+  delete static_cast<SiftState*>(ctx->sift_state);
+  ctx->sift_state = nullptr;
 }
 
 }  // namespace b2m
@@ -822,41 +783,37 @@ void b2m_extract_opts_default(b2m_extract_opts* o) {
 int b2m_extract_features_batch(b2m_ctx* ctx, const b2m_image* images, int32_t n, const b2m_extract_opts* opts,
                                b2m_features** out) {
   if (!ctx) return B2M_EINVAL;
-  auto bad = [&](const std::string& msg) {
-    ctx->err = msg;
-    return B2M_EINVAL;
-  };
-  if (!out || !opts || n < 0 || (n > 0 && !images)) return bad("[sift.cu] Check Failed: images, options and out != NULL");
+  if (!out || !opts || n < 0 || (n > 0 && !images)) return fail(ctx, B2M_EINVAL, "[sift.cu] Check Failed: images, options and out != NULL");
   *out = nullptr;
   if (opts->struct_size != sizeof(b2m_extract_opts))
-    return bad("[sift.cu] Check Failed: b2m_extract_opts.struct_size == sizeof(b2m_extract_opts)");
+    return fail(ctx, B2M_EINVAL, "[sift.cu] Check Failed: b2m_extract_opts.struct_size == sizeof(b2m_extract_opts)");
   const b2m_extract_opts& o = *opts;
   // SiftExtractionOptions::Check (U:feature/sift.cc)
-  if (!(o.max_image_size > 0)) return bad("[sift.cc] Check Failed: max_image_size > 0");
-  if (!(o.max_num_features > 0)) return bad("[sift.cc] Check Failed: max_num_features > 0");
-  if (!(o.octave_resolution > 0)) return bad("[sift.cc] Check Failed: octave_resolution > 0");
-  if (!(o.peak_threshold > 0.0)) return bad("[sift.cc] Check Failed: peak_threshold > 0");
-  if (!(o.edge_threshold > 0.0)) return bad("[sift.cc] Check Failed: edge_threshold > 0");
-  if (!(o.max_num_orientations > 0)) return bad("[sift.cc] Check Failed: max_num_orientations > 0");
-  if (!(o.num_octaves > 0)) return bad("[sift.cu] Check Failed: num_octaves > 0");
-  if (!(o.first_octave >= -3 && o.first_octave <= 16)) return bad("[sift.cu] Check Failed: -3 <= first_octave <= 16");
+  if (!(o.max_image_size > 0)) return fail(ctx, B2M_EINVAL, "[sift.cc] Check Failed: max_image_size > 0");
+  if (!(o.max_num_features > 0)) return fail(ctx, B2M_EINVAL, "[sift.cc] Check Failed: max_num_features > 0");
+  if (!(o.octave_resolution > 0)) return fail(ctx, B2M_EINVAL, "[sift.cc] Check Failed: octave_resolution > 0");
+  if (!(o.peak_threshold > 0.0)) return fail(ctx, B2M_EINVAL, "[sift.cc] Check Failed: peak_threshold > 0");
+  if (!(o.edge_threshold > 0.0)) return fail(ctx, B2M_EINVAL, "[sift.cc] Check Failed: edge_threshold > 0");
+  if (!(o.max_num_orientations > 0)) return fail(ctx, B2M_EINVAL, "[sift.cc] Check Failed: max_num_orientations > 0");
+  if (!(o.num_octaves > 0)) return fail(ctx, B2M_EINVAL, "[sift.cu] Check Failed: num_octaves > 0");
+  if (!(o.first_octave >= -3 && o.first_octave <= 16)) return fail(ctx, B2M_EINVAL, "[sift.cu] Check Failed: -3 <= first_octave <= 16");
   if (o.normalization != B2M_NORMALIZATION_L1_ROOT && o.normalization != B2M_NORMALIZATION_L2)
-    return bad("[sift.cu] Check Failed: normalization is L1_ROOT or L2");
+    return fail(ctx, B2M_EINVAL, "[sift.cu] Check Failed: normalization is L1_ROOT or L2");
   if (o.estimate_affine_shape || o.domain_size_pooling)
-    return bad("[sift.cu] Check Failed: estimate_affine_shape and domain_size_pooling (the covariant path) are not supported");
-  if (o.darkness_adaptivity) return bad("[sift.cu] Check Failed: darkness_adaptivity (SiftGPU only) is not supported");
+    return fail(ctx, B2M_EINVAL, "[sift.cu] Check Failed: estimate_affine_shape and domain_size_pooling (the covariant path) are not supported");
+  if (o.darkness_adaptivity) return fail(ctx, B2M_EINVAL, "[sift.cu] Check Failed: darkness_adaptivity (SiftGPU only) is not supported");
   int64_t max_a0 = 0, need_grad = 1;
   int max_w = 0, max_h = 0;
   for (int32_t i = 0; i < n; ++i) {
     const b2m_image& im = images[i];
     if (!im.data || im.width <= 0 || im.height <= 0 || im.stride < im.width)
-      return bad("[sift.cu] Check Failed: image " + std::to_string(i) + " is non-empty with stride >= width");
+      return fail(ctx, B2M_EINVAL, "[sift.cu] Check Failed: image " + std::to_string(i) + " is non-empty with stride >= width");
     if (im.width > o.max_image_size || im.height > o.max_image_size)
-      return bad("[sift.h] Check Failed: image " + std::to_string(i) + " within max_image_size");
+      return fail(ctx, B2M_EINVAL, "[sift.h] Check Failed: image " + std::to_string(i) + " within max_image_size");
     const int f = o.first_octave;
     const int64_t a0 = f < 0 ? (static_cast<int64_t>(im.width) << -f) * (static_cast<int64_t>(im.height) << -f)
                              : static_cast<int64_t>(im.width >> f) * (im.height >> f);
-    if (a0 > (int64_t(1) << 30)) return bad("[sift.cu] Check Failed: first octave of at most 2^30 pixels");
+    if (a0 > (int64_t(1) << 30)) return fail(ctx, B2M_EINVAL, "[sift.cu] Check Failed: first octave of at most 2^30 pixels");
     max_a0 = std::max(max_a0, a0);
     // gradients of every octave stay resident until the descriptors are done: S levels per octave
     int64_t areas = 0;
@@ -872,47 +829,42 @@ int b2m_extract_features_batch(b2m_ctx* ctx, const b2m_image* images, int32_t n,
   cudaSetDevice(ctx->device);
   if (!ctx->sift_state) ctx->sift_state = new SiftState();
   SiftState* S = static_cast<SiftState*>(ctx->sift_state);
-  if (!S->table) {
-    double tab[258];
-    for (int k = 0; k < 257; ++k) tab[k] = std::exp(-static_cast<double>(k) * (25.0 / 256));
-    tab[257] = 0.0;
-    S_TRY(ctx, cudaMemcpyToSymbol(c_expn, tab, sizeof(tab)));
-    S_TRY(ctx, cudaMalloc(&S->d_total, sizeof(int)));
-    S_TRY(ctx, cudaMalloc(&S->d_nang, sizeof(int) * kKpCap));
-    S_TRY(ctx, cudaMalloc(&S->d_ang, sizeof(double) * 4 * kKpCap));
-    S_TRY(ctx, cudaMalloc(&S->d_kp, sizeof(Kp) * kKpCap));
-    S_TRY(ctx, cudaMalloc(&S->d_taps, sizeof(float) * 65536));
-    S->table = true;
+  if (!S->tab.d_taps) {
+    const int rc = alloc_group(S->tab, [&](SiftTables& t) -> int {
+      double tab[258];
+      for (int k = 0; k < 257; ++k) tab[k] = std::exp(-static_cast<double>(k) * (25.0 / 256));
+      tab[257] = 0.0;
+      B2M_CUDA_TRY(ctx, cudaMemcpyToSymbol(c_expn, tab, sizeof(tab)));
+      B2M_CUDA_TRY(ctx, t.d_total.ensure(1));
+      B2M_CUDA_TRY(ctx, t.d_nang.ensure(kKpCap));
+      B2M_CUDA_TRY(ctx, t.d_ang.ensure(4 * kKpCap));
+      B2M_CUDA_TRY(ctx, t.d_kp.ensure(kKpCap));
+      B2M_CUDA_TRY(ctx, t.d_taps.ensure(65536));
+      return B2M_OK;
+    });
+    if (rc) return rc;
   }
   const int nlev = o.octave_resolution + 3;
   const int64_t img_px = static_cast<int64_t>(max_w) * max_h;
   const int64_t need_px = std::max(max_a0, img_px);
-  if (n > 0 && (need_px > S->cap_px || nlev > S->cap_levels)) {
-    S->release_px();
-    S_TRY(ctx, cudaMalloc(&S->d_img, need_px));
-    S_TRY(ctx, cudaMalloc(&S->d_G, sizeof(float) * nlev * need_px));
-    S_TRY(ctx, cudaMalloc(&S->d_D, sizeof(float) * (nlev - 1) * need_px));
-    S_TRY(ctx, cudaMalloc(&S->d_T, sizeof(float) * need_px));
-    S_TRY(ctx, cudaMalloc(&S->d_U, sizeof(float) * need_px));
-    S->cap_px = need_px;
-    S->cap_levels = nlev;
+  if (n > 0 && (need_px > S->px.cap_px || nlev > S->px.cap_levels)) {
+    const int rc = alloc_group(S->px, [&](SiftPyramid& p) -> int {
+      B2M_CUDA_TRY(ctx, p.d_img.ensure(need_px));
+      B2M_CUDA_TRY(ctx, p.d_G.ensure(static_cast<size_t>(nlev) * need_px));
+      B2M_CUDA_TRY(ctx, p.d_D.ensure(static_cast<size_t>(nlev - 1) * need_px));
+      B2M_CUDA_TRY(ctx, p.d_T.ensure(need_px));
+      B2M_CUDA_TRY(ctx, p.d_U.ensure(need_px));
+      p.cap_px = need_px;
+      p.cap_levels = nlev;
+      return B2M_OK;
+    });
+    if (rc) return rc;
   }
   const int64_t need_blocks = (static_cast<int64_t>(o.octave_resolution) * max_a0 + kDetectThreads - 1) / kDetectThreads + 1;
-  if (n > 0 && need_grad > S->cap_grad) {
-    if (S->d_grad) cudaFree(S->d_grad);
-    S->d_grad = nullptr;
-    S->cap_grad = 0;
-    S_TRY(ctx, cudaMalloc(&S->d_grad, sizeof(float2) * need_grad));
-    S->cap_grad = need_grad;
-  }
-  if (n > 0 && need_blocks > S->cap_blocks) {
-    if (S->d_counts) cudaFree(S->d_counts);
-    if (S->d_offs) cudaFree(S->d_offs);
-    S->d_counts = S->d_offs = nullptr;
-    S->cap_blocks = 0;
-    S_TRY(ctx, cudaMalloc(&S->d_counts, sizeof(int) * need_blocks));
-    S_TRY(ctx, cudaMalloc(&S->d_offs, sizeof(int) * need_blocks));
-    S->cap_blocks = need_blocks;
+  if (n > 0) {
+    B2M_CUDA_TRY(ctx, S->d_grad.ensure(need_grad));
+    B2M_CUDA_TRY(ctx, S->d_counts.ensure(need_blocks));
+    B2M_CUDA_TRY(ctx, S->d_offs.ensure(need_blocks));
   }
   // filters: [0] the first level's (0 taps when sa <= sb), [s] level s - 1 of VLFeat's numbering from level s - 2
   const int Sr = o.octave_resolution;
@@ -936,12 +888,12 @@ int b2m_extract_features_batch(b2m_ctx* ctx, const b2m_image* images, int32_t n,
       taps.insert(taps.end(), g.begin(), g.end());
     }
   }
-  if (taps.size() > 65536) return bad("[sift.cu] Check Failed: Gaussian filters of at most 65536 taps in all");
+  if (taps.size() > 65536) return fail(ctx, B2M_EINVAL, "[sift.cu] Check Failed: Gaussian filters of at most 65536 taps in all");
   // the blur tiles stage 32 x (64 + 2R) samples in the 48 KB of default shared memory
   if (*std::max_element(tap_r.begin(), tap_r.end()) > kMaxBlurR)
-    return bad("[sift.cu] Check Failed: Gaussian half-width <= " + std::to_string(kMaxBlurR) +
+    return fail(ctx, B2M_EINVAL, "[sift.cu] Check Failed: Gaussian half-width <= " + std::to_string(kMaxBlurR) +
                " (octave_resolution and first_octave give a smoothing this wide)");
-  S_TRY(ctx, cudaMemcpy(S->d_taps, taps.data(), sizeof(float) * std::max<size_t>(taps.size(), 1), cudaMemcpyHostToDevice));
+  B2M_CUDA_TRY(ctx, cudaMemcpy(S->tab.d_taps, taps.data(), sizeof(float) * std::max<size_t>(taps.size(), 1), cudaMemcpyHostToDevice));
   b2m_features* F = new b2m_features();
   F->off.push_back(0);
   for (int32_t i = 0; i < n; ++i) {

@@ -441,88 +441,40 @@ __global__ void __launch_bounds__(32 * kWarps) b2m_tri_ransac_kernel(const TriPa
   }
 }
 
-#define T_TRY(ctx, expr)                                                                    \
-  do {                                                                                      \
-    cudaError_t _e = (expr);                                                                \
-    if (_e != cudaSuccess) {                                                                \
-      char _b[512];                                                                         \
-      snprintf(_b, sizeof(_b), "[%s:%d] CUDA error: %s (%s)", __FILE__, __LINE__,          \
-               cudaGetErrorString(_e), #expr);                                              \
-      (ctx)->err = _b;                                                                      \
-      return _e == cudaErrorMemoryAllocation ? B2M_ENOMEM : B2M_ECUDA;                      \
-    }                                                                                       \
-  } while (0)
-
 // Chunk limits: results do not depend on them (tracks are independent).
 constexpr int64_t kChunkTracks = int64_t(1) << 15;
 constexpr int64_t kChunkObs = int64_t(1) << 21;
 
 }  // namespace
 
-// Pinned staging and device buffers of the triangulation path, kept by the context between calls and grown on demand.
-struct TriState {
-  int64_t cap_tracks = 0, cap_obs = 0, cap_images = 0;
+// Pinned staging and device buffers of one chunk of tracks, replaced together when a call needs more.
+struct TriChunkBufs {
+  int64_t cap_tracks = 0, cap_obs = 0;
   // pinned host staging
-  double* h_pts = nullptr;
-  int32_t* h_img = nullptr;
-  int64_t* h_off = nullptr;
-  int32_t* h_order = nullptr;
-  double* h_xyz = nullptr;
-  int32_t* h_inl = nullptr;
-  uint8_t* h_succ = nullptr;
-  uint8_t* h_mask = nullptr;
+  PinnedArray<double> h_pts;
+  PinnedArray<int32_t> h_img;
+  PinnedArray<int64_t> h_off;
+  PinnedArray<int32_t> h_order;
+  PinnedArray<double> h_xyz;
+  PinnedArray<int32_t> h_inl;
+  PinnedArray<uint8_t> h_succ;
+  PinnedArray<uint8_t> h_mask;
   // device
-  double *d_pts = nullptr, *d_xyz = nullptr, *d_cams = nullptr, *d_centers = nullptr;
-  int32_t *d_img = nullptr, *d_order = nullptr, *d_inl = nullptr, *d_scratch = nullptr;
-  int64_t* d_off = nullptr;
-  uint8_t *d_succ = nullptr, *d_mask = nullptr;
-  unsigned long long* d_counters = nullptr;
+  DeviceArray<double> d_pts, d_xyz;
+  DeviceArray<int32_t> d_img, d_order, d_inl, d_scratch;
+  DeviceArray<int64_t> d_off;
+  DeviceArray<uint8_t> d_succ, d_mask;
+};
 
-  void release_tracks_obs() {
-    for (void* q : {static_cast<void*>(h_pts), static_cast<void*>(h_img), static_cast<void*>(h_off),
-                    static_cast<void*>(h_order), static_cast<void*>(h_xyz), static_cast<void*>(h_inl),
-                    static_cast<void*>(h_succ), static_cast<void*>(h_mask)})
-      if (q) cudaFreeHost(q);
-    for (void* q : {static_cast<void*>(d_pts), static_cast<void*>(d_xyz), static_cast<void*>(d_img),
-                    static_cast<void*>(d_order), static_cast<void*>(d_inl), static_cast<void*>(d_scratch),
-                    static_cast<void*>(d_off), static_cast<void*>(d_succ), static_cast<void*>(d_mask)})
-      if (q) cudaFree(q);
-    h_pts = nullptr; h_img = nullptr; h_off = nullptr; h_order = nullptr; h_xyz = nullptr; h_inl = nullptr;
-    h_succ = nullptr; h_mask = nullptr;
-    d_pts = nullptr; d_xyz = nullptr; d_img = nullptr; d_order = nullptr; d_inl = nullptr; d_scratch = nullptr;
-    d_off = nullptr; d_succ = nullptr; d_mask = nullptr;
-    cap_tracks = cap_obs = 0;
-  }
-  void release() {
-    release_tracks_obs();
-    if (d_cams) cudaFree(d_cams);
-    if (d_centers) cudaFree(d_centers);
-    if (d_counters) cudaFree(d_counters);
-    d_cams = d_centers = nullptr;
-    d_counters = nullptr;
-    cap_images = 0;
-  }
+// The buffers of the triangulation path, kept by the context between calls and grown on demand.
+struct TriState {
+  TriChunkBufs chunk;
+  DeviceArray<double> d_cams, d_centers;  // per image
 };
 
 void tri_release(b2m_ctx* ctx) {
-  if (ctx && ctx->tri_state) {
-    TriState* s = static_cast<TriState*>(ctx->tri_state);
-    s->release();
-    delete s;
-    ctx->tri_state = nullptr;
-  }
-}
-
-// kernel-side counters (models scored, residual evaluations), zero when the path was never used
-bool tri_counters(b2m_ctx* ctx, unsigned long long* out) {
-  TriState* s = static_cast<TriState*>(ctx->tri_state);
-  if (!s || !s->d_counters) return false;
-  return cudaMemcpy(out, s->d_counters, sizeof(unsigned long long) * 2, cudaMemcpyDeviceToHost) == cudaSuccess;
-}
-
-void tri_reset_counters(b2m_ctx* ctx) {
-  TriState* s = static_cast<TriState*>(ctx->tri_state);
-  if (s && s->d_counters) cudaMemset(s->d_counters, 0, sizeof(unsigned long long) * 2);
+  delete static_cast<TriState*>(ctx->tri_state);
+  ctx->tri_state = nullptr;
 }
 
 namespace {
@@ -531,41 +483,35 @@ int ensure_state(b2m_ctx* ctx, int64_t tracks, int64_t obs, int64_t images, TriS
   if (!ctx->tri_state) ctx->tri_state = new TriState();
   TriState* s = static_cast<TriState*>(ctx->tri_state);
   *out = s;
-  if (!s->d_counters) {
-    T_TRY(ctx, cudaMalloc(&s->d_counters, sizeof(unsigned long long) * 2));
-    T_TRY(ctx, cudaMemset(s->d_counters, 0, sizeof(unsigned long long) * 2));
+  if (tracks > s->chunk.cap_tracks || obs > s->chunk.cap_obs) {
+    const int rc = alloc_group(s->chunk, [&](TriChunkBufs& b) -> int {
+      const int64_t T = std::max<int64_t>(tracks, 1), M = std::max<int64_t>(obs, 1);
+      B2M_CUDA_TRY(ctx, b.h_pts.ensure(2 * M));
+      B2M_CUDA_TRY(ctx, b.h_img.ensure(M));
+      B2M_CUDA_TRY(ctx, b.h_off.ensure(T + 1));
+      B2M_CUDA_TRY(ctx, b.h_order.ensure(T));
+      B2M_CUDA_TRY(ctx, b.h_xyz.ensure(3 * T));
+      B2M_CUDA_TRY(ctx, b.h_inl.ensure(T));
+      B2M_CUDA_TRY(ctx, b.h_succ.ensure(T));
+      B2M_CUDA_TRY(ctx, b.h_mask.ensure(M));
+      B2M_CUDA_TRY(ctx, b.d_pts.ensure(2 * M));
+      B2M_CUDA_TRY(ctx, b.d_img.ensure(M));
+      B2M_CUDA_TRY(ctx, b.d_off.ensure(T + 1));
+      B2M_CUDA_TRY(ctx, b.d_order.ensure(T));
+      B2M_CUDA_TRY(ctx, b.d_xyz.ensure(3 * T));
+      B2M_CUDA_TRY(ctx, b.d_inl.ensure(T));
+      B2M_CUDA_TRY(ctx, b.d_succ.ensure(T));
+      B2M_CUDA_TRY(ctx, b.d_mask.ensure(M));
+      B2M_CUDA_TRY(ctx, b.d_scratch.ensure(M));
+      b.cap_tracks = T;
+      b.cap_obs = M;
+      return B2M_OK;
+    });
+    if (rc) return rc;
   }
-  if (tracks > s->cap_tracks || obs > s->cap_obs) {
-    s->release_tracks_obs();
-    const int64_t T = std::max<int64_t>(tracks, 1), M = std::max<int64_t>(obs, 1);
-    T_TRY(ctx, cudaHostAlloc(&s->h_pts, sizeof(double) * 2 * M, cudaHostAllocDefault));
-    T_TRY(ctx, cudaHostAlloc(&s->h_img, sizeof(int32_t) * M, cudaHostAllocDefault));
-    T_TRY(ctx, cudaHostAlloc(&s->h_off, sizeof(int64_t) * (T + 1), cudaHostAllocDefault));
-    T_TRY(ctx, cudaHostAlloc(&s->h_order, sizeof(int32_t) * T, cudaHostAllocDefault));
-    T_TRY(ctx, cudaHostAlloc(&s->h_xyz, sizeof(double) * 3 * T, cudaHostAllocDefault));
-    T_TRY(ctx, cudaHostAlloc(&s->h_inl, sizeof(int32_t) * T, cudaHostAllocDefault));
-    T_TRY(ctx, cudaHostAlloc(&s->h_succ, T, cudaHostAllocDefault));
-    T_TRY(ctx, cudaHostAlloc(&s->h_mask, M, cudaHostAllocDefault));
-    T_TRY(ctx, cudaMalloc(&s->d_pts, sizeof(double) * 2 * M));
-    T_TRY(ctx, cudaMalloc(&s->d_img, sizeof(int32_t) * M));
-    T_TRY(ctx, cudaMalloc(&s->d_off, sizeof(int64_t) * (T + 1)));
-    T_TRY(ctx, cudaMalloc(&s->d_order, sizeof(int32_t) * T));
-    T_TRY(ctx, cudaMalloc(&s->d_xyz, sizeof(double) * 3 * T));
-    T_TRY(ctx, cudaMalloc(&s->d_inl, sizeof(int32_t) * T));
-    T_TRY(ctx, cudaMalloc(&s->d_succ, T));
-    T_TRY(ctx, cudaMalloc(&s->d_mask, M));
-    T_TRY(ctx, cudaMalloc(&s->d_scratch, sizeof(int32_t) * M));
-    s->cap_tracks = T;
-    s->cap_obs = M;
-  }
-  if (images > s->cap_images) {
-    if (s->d_cams) cudaFree(s->d_cams);
-    if (s->d_centers) cudaFree(s->d_centers);
-    s->d_cams = s->d_centers = nullptr;
-    s->cap_images = 0;
-    T_TRY(ctx, cudaMalloc(&s->d_cams, sizeof(double) * 12 * images));
-    T_TRY(ctx, cudaMalloc(&s->d_centers, sizeof(double) * 3 * images));
-    s->cap_images = images;
+  if (images > 0) {
+    B2M_CUDA_TRY(ctx, s->d_cams.ensure(12 * images));
+    B2M_CUDA_TRY(ctx, s->d_centers.ensure(3 * images));
   }
   return B2M_OK;
 }
@@ -590,36 +536,32 @@ int b2m_estimate_triangulation_batch(b2m_ctx* ctx, int64_t n_tracks, const int64
                                      const double* cams_from_world, const b2m_tri_opts* opts, double* xyz,
                                      int32_t* num_inliers, uint8_t* success, uint8_t* inlier_mask) {
   if (!ctx) return B2M_EINVAL;
-  auto bad = [&](const std::string& msg) {
-    ctx->err = msg;
-    return B2M_EINVAL;
-  };
   if (!opts || n_tracks < 0 || (n_tracks > 0 && (!track_offsets || !xyz || !num_inliers || !success)))
-    return bad("[triangulation.cu] Check Failed: track_offsets, options and outputs != NULL");
+    return fail(ctx, B2M_EINVAL, "[triangulation.cu] Check Failed: track_offsets, options and outputs != NULL");
   if (opts->struct_size != sizeof(b2m_tri_opts) || opts->ransac.struct_size != sizeof(b2m_ransac_opts))
-    return bad("[triangulation.cu] Check Failed: b2m_tri_opts.struct_size == sizeof(b2m_tri_opts)");
+    return fail(ctx, B2M_EINVAL, "[triangulation.cu] Check Failed: b2m_tri_opts.struct_size == sizeof(b2m_tri_opts)");
   // EstimateTriangulationOptions::Check, RANSACOptions::Check (U:estimators/triangulation.h, U:optim/ransac.h)
   const b2m_ransac_opts& ro = opts->ransac;
-  if (!(opts->min_tri_angle >= 0.0)) return bad("[triangulation.h] Check Failed: min_tri_angle >= 0");
-  if (!(ro.max_error > 0.0)) return bad("[ransac.h] Check Failed: max_error > 0");
+  if (!(opts->min_tri_angle >= 0.0)) return fail(ctx, B2M_EINVAL, "[triangulation.h] Check Failed: min_tri_angle >= 0");
+  if (!(ro.max_error > 0.0)) return fail(ctx, B2M_EINVAL, "[ransac.h] Check Failed: max_error > 0");
   if (!(ro.min_inlier_ratio >= 0.0 && ro.min_inlier_ratio <= 1.0))
-    return bad("[ransac.h] Check Failed: min_inlier_ratio in [0, 1]");
-  if (!(ro.confidence >= 0.0 && ro.confidence <= 1.0)) return bad("[ransac.h] Check Failed: confidence in [0, 1]");
-  if (!(ro.min_num_trials <= ro.max_num_trials)) return bad("[ransac.h] Check Failed: min_num_trials <= max_num_trials");
+    return fail(ctx, B2M_EINVAL, "[ransac.h] Check Failed: min_inlier_ratio in [0, 1]");
+  if (!(ro.confidence >= 0.0 && ro.confidence <= 1.0)) return fail(ctx, B2M_EINVAL, "[ransac.h] Check Failed: confidence in [0, 1]");
+  if (!(ro.min_num_trials <= ro.max_num_trials)) return fail(ctx, B2M_EINVAL, "[ransac.h] Check Failed: min_num_trials <= max_num_trials");
   if (n_tracks == 0) return B2M_OK;
-  if (track_offsets[0] != 0) return bad("[triangulation.cu] Check Failed: track_offsets[0] == 0");
+  if (track_offsets[0] != 0) return fail(ctx, B2M_EINVAL, "[triangulation.cu] Check Failed: track_offsets[0] == 0");
   for (int64_t k = 0; k < n_tracks; ++k)
     if (!(track_offsets[k + 1] - track_offsets[k] >= 2))  // THROW_CHECK_GE(point_data.size(), 2)
-      return bad("[triangulation.cc] Check Failed: point_data.size() >= 2 (track " + std::to_string(k) + ")");
+      return fail(ctx, B2M_EINVAL, "[triangulation.cc] Check Failed: point_data.size() >= 2 (track " + std::to_string(k) + ")");
   const int64_t M = track_offsets[n_tracks];
   if (!points_normalized || !image_idx || !cams_from_world)
-    return bad("[triangulation.cu] Check Failed: points, image indices and cameras != NULL");
+    return fail(ctx, B2M_EINVAL, "[triangulation.cu] Check Failed: points, image indices and cameras != NULL");
   for (int64_t i = 0; i < M; ++i)
     if (image_idx[i] < 0 || image_idx[i] >= n_images)
-      return bad("[triangulation.cu] Check Failed: 0 <= image_idx < n_images (observation " + std::to_string(i) + ")");
+      return fail(ctx, B2M_EINVAL, "[triangulation.cu] Check Failed: 0 <= image_idx < n_images (observation " + std::to_string(i) + ")");
   for (int64_t k = 0; k < n_tracks; ++k)
     if (track_offsets[k + 1] - track_offsets[k] > INT32_MAX)
-      return bad("[triangulation.cu] Check Failed: observations per track < 2^31");
+      return fail(ctx, B2M_EINVAL, "[triangulation.cu] Check Failed: observations per track < 2^31");
 
   cudaSetDevice(ctx->device);
   cudaStream_t st = ctx->stream;
@@ -648,28 +590,28 @@ int b2m_estimate_triangulation_batch(b2m_ctx* ctx, int64_t n_tracks, const int64
   }
   TriState* S = nullptr;
   if (int rc = ensure_state(ctx, cap_t, cap_o, n_images, &S)) return rc;
-  T_TRY(ctx, cudaMemcpyAsync(S->d_cams, cams_from_world, sizeof(double) * 12 * n_images, cudaMemcpyHostToDevice, st));
-  T_TRY(ctx, cudaMemcpyAsync(S->d_centers, centers.data(), sizeof(double) * 3 * n_images, cudaMemcpyHostToDevice, st));
+  B2M_CUDA_TRY(ctx, cudaMemcpyAsync(S->d_cams, cams_from_world, sizeof(double) * 12 * n_images, cudaMemcpyHostToDevice, st));
+  B2M_CUDA_TRY(ctx, cudaMemcpyAsync(S->d_centers, centers.data(), sizeof(double) * 3 * n_images, cudaMemcpyHostToDevice, st));
   std::vector<int32_t> order;
   for (size_t c = 0; c + 1 < starts.size(); ++c) {
     if (ctx->stop) return B2M_ESTOPPED;
     const int64_t k0 = starts[c], k1 = starts[c + 1];
     const int nb = static_cast<int>(k1 - k0);
     const int64_t o0 = track_offsets[k0], mo = track_offsets[k1] - o0;
-    memcpy(S->h_pts, points_normalized + 2 * o0, sizeof(double) * 2 * mo);
-    memcpy(S->h_img, image_idx + o0, sizeof(int32_t) * mo);
-    for (int k = 0; k <= nb; ++k) S->h_off[k] = track_offsets[k0 + k] - o0;
+    memcpy(S->chunk.h_pts, points_normalized + 2 * o0, sizeof(double) * 2 * mo);
+    memcpy(S->chunk.h_img, image_idx + o0, sizeof(int32_t) * mo);
+    for (int k = 0; k <= nb; ++k) S->chunk.h_off[k] = track_offsets[k0 + k] - o0;
     order.resize(nb);
     std::iota(order.begin(), order.end(), 0);
     std::stable_sort(order.begin(), order.end(),
-                     [&](int32_t a, int32_t b) { return S->h_off[a + 1] - S->h_off[a] > S->h_off[b + 1] - S->h_off[b]; });
-    memcpy(S->h_order, order.data(), sizeof(int32_t) * nb);
-    T_TRY(ctx, cudaMemcpyAsync(S->d_pts, S->h_pts, sizeof(double) * 2 * mo, cudaMemcpyHostToDevice, st));
-    T_TRY(ctx, cudaMemcpyAsync(S->d_img, S->h_img, sizeof(int32_t) * mo, cudaMemcpyHostToDevice, st));
-    T_TRY(ctx, cudaMemcpyAsync(S->d_off, S->h_off, sizeof(int64_t) * (nb + 1), cudaMemcpyHostToDevice, st));
-    T_TRY(ctx, cudaMemcpyAsync(S->d_order, S->h_order, sizeof(int32_t) * nb, cudaMemcpyHostToDevice, st));
+                     [&](int32_t a, int32_t b) { return S->chunk.h_off[a + 1] - S->chunk.h_off[a] > S->chunk.h_off[b + 1] - S->chunk.h_off[b]; });
+    memcpy(S->chunk.h_order, order.data(), sizeof(int32_t) * nb);
+    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(S->chunk.d_pts, S->chunk.h_pts, sizeof(double) * 2 * mo, cudaMemcpyHostToDevice, st));
+    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(S->chunk.d_img, S->chunk.h_img, sizeof(int32_t) * mo, cudaMemcpyHostToDevice, st));
+    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(S->chunk.d_off, S->chunk.h_off, sizeof(int64_t) * (nb + 1), cudaMemcpyHostToDevice, st));
+    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(S->chunk.d_order, S->chunk.h_order, sizeof(int32_t) * nb, cudaMemcpyHostToDevice, st));
     TriParams P{};
-    P.pts = S->d_pts; P.img = S->d_img; P.off = S->d_off; P.order = S->d_order;
+    P.pts = S->chunk.d_pts; P.img = S->chunk.d_img; P.off = S->chunk.d_off; P.order = S->chunk.d_order;
     P.cams = S->d_cams; P.centers = S->d_centers; P.nb = nb;
     P.max_residual = ro.max_error * ro.max_error;
     P.min_tri_angle = opts->min_tri_angle;
@@ -677,20 +619,20 @@ int b2m_estimate_triangulation_batch(b2m_ctx* ctx, int64_t n_tracks, const int64
     P.multiplier = ro.dyn_num_trials_multiplier;
     P.max_trials = max_trials;
     P.min_num_trials = static_cast<double>(ro.min_num_trials);
-    P.xyz = S->d_xyz; P.num_inliers = S->d_inl; P.success = S->d_succ; P.mask = S->d_mask; P.scratch = S->d_scratch;
-    P.counters = S->d_counters;
+    P.xyz = S->chunk.d_xyz; P.num_inliers = S->chunk.d_inl; P.success = S->chunk.d_succ; P.mask = S->chunk.d_mask; P.scratch = S->chunk.d_scratch;
+    P.counters = ctx->d_counters + kTriCounters;
     b2m_tri_ransac_kernel<<<static_cast<unsigned>((nb + kWarps - 1) / kWarps), 32 * kWarps, 0, st>>>(P);
-    T_TRY(ctx, cudaGetLastError());
+    B2M_CUDA_TRY(ctx, cudaGetLastError());
     ctx->stats.kernel_launches += 1;
-    T_TRY(ctx, cudaMemcpyAsync(S->h_xyz, S->d_xyz, sizeof(double) * 3 * nb, cudaMemcpyDeviceToHost, st));
-    T_TRY(ctx, cudaMemcpyAsync(S->h_inl, S->d_inl, sizeof(int32_t) * nb, cudaMemcpyDeviceToHost, st));
-    T_TRY(ctx, cudaMemcpyAsync(S->h_succ, S->d_succ, nb, cudaMemcpyDeviceToHost, st));
-    if (inlier_mask) T_TRY(ctx, cudaMemcpyAsync(S->h_mask, S->d_mask, mo, cudaMemcpyDeviceToHost, st));
-    T_TRY(ctx, cudaStreamSynchronize(st));
-    memcpy(xyz + 3 * k0, S->h_xyz, sizeof(double) * 3 * nb);
-    memcpy(num_inliers + k0, S->h_inl, sizeof(int32_t) * nb);
-    memcpy(success + k0, S->h_succ, nb);
-    if (inlier_mask) memcpy(inlier_mask + o0, S->h_mask, mo);
+    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(S->chunk.h_xyz, S->chunk.d_xyz, sizeof(double) * 3 * nb, cudaMemcpyDeviceToHost, st));
+    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(S->chunk.h_inl, S->chunk.d_inl, sizeof(int32_t) * nb, cudaMemcpyDeviceToHost, st));
+    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(S->chunk.h_succ, S->chunk.d_succ, nb, cudaMemcpyDeviceToHost, st));
+    if (inlier_mask) B2M_CUDA_TRY(ctx, cudaMemcpyAsync(S->chunk.h_mask, S->chunk.d_mask, mo, cudaMemcpyDeviceToHost, st));
+    B2M_CUDA_TRY(ctx, cudaStreamSynchronize(st));
+    memcpy(xyz + 3 * k0, S->chunk.h_xyz, sizeof(double) * 3 * nb);
+    memcpy(num_inliers + k0, S->chunk.h_inl, sizeof(int32_t) * nb);
+    memcpy(success + k0, S->chunk.h_succ, nb);
+    if (inlier_mask) memcpy(inlier_mask + o0, S->chunk.h_mask, mo);
   }
   return B2M_OK;
 }

@@ -724,8 +724,8 @@ __global__ void __launch_bounds__(kRansacThreads, KindBlocks<KIND>::v) b2m_ransa
 // The three model kinds are independent problems: E and F go to two side streams so that their
 // (few, long) CTAs fill the tail of the H kernel instead of serialising behind it.
 struct RansacStreams {
-  cudaStream_t side[2] = {nullptr, nullptr};
-  cudaEvent_t fork = nullptr, join[2] = {nullptr, nullptr};
+  Stream side[2];
+  Event fork, join[2];
 };
 
 // ---- relative pose (TwoViewGeometryOptions.compute_relative_pose; pose.h) --------------------------------
@@ -1197,109 +1197,72 @@ __global__ void __launch_bounds__(256) b2m_decide_kernel(const VerifyParams P) {
 
 // ---- host side --------------------------------------------------------------------------------
 
-struct VerifyState {
+// Guided matching (lazily allocated): hand-over arrays + a second match arena per slot
+struct GuidedBufs {
+  DeviceArray<int32_t> d_guided_kind;
+  DeviceArray<float> d_guided_model;
+  DeviceArray<uint2> d_garena[2];
+  DeviceArray<unsigned long long> d_gcursor[2];
+  DeviceArray<int64_t> d_goff[2];
+  DeviceArray<int32_t> d_gcnt[2];
+  PinnedArray<uint2> h_garena[2];
+  PinnedArray<unsigned long long> h_gcursor[2];
+  PinnedArray<int64_t> h_goff[2];
+  PinnedArray<int32_t> h_gcnt[2];
+};
+
+// Relative pose of one slot (compute_relative_pose), lazily allocated
+struct PoseBufs {
+  DeviceArray<double> d_pose;  // [batch][8] qvec, tvec, tri_angle
+  DeviceArray<int32_t> d_pose_valid;
+  PinnedArray<double> h_pose;
+  PinnedArray<int32_t> h_pose_valid;
+};
+
+// Everything sized by the batch: replaced as a whole when the workspace grows.
+struct VerifyBatch {
   int batch = 0;
   int64_t arena_cap = 0;
-  double4* d_pts[2] = {nullptr, nullptr};
-  uint8_t* d_mask = nullptr;      // [3][arena_cap], shared by both slots (stream-ordered)
-  double* d_models[2] = {nullptr, nullptr};
-  int32_t* d_sup = nullptr;
-  int32_t* d_success = nullptr;
-  int32_t* d_config[2] = {nullptr, nullptr};
-  int32_t* d_inl_cnt[2] = {nullptr, nullptr};
-  uint2* d_inliers[2] = {nullptr, nullptr};
-  // guided matching (lazily allocated): hand-over arrays + a second match arena per slot
-  int32_t* d_guided_kind = nullptr;
-  float* d_guided_model = nullptr;
-  uint2* d_garena[2] = {nullptr, nullptr};
-  unsigned long long* d_gcursor[2] = {nullptr, nullptr};
-  int64_t* d_goff[2] = {nullptr, nullptr};
-  int32_t* d_gcnt[2] = {nullptr, nullptr};
-  uint2* h_garena[2] = {nullptr, nullptr};
-  unsigned long long* h_gcursor[2] = {nullptr, nullptr};
-  int64_t* h_goff[2] = {nullptr, nullptr};
-  int32_t* h_gcnt[2] = {nullptr, nullptr};
+  DeviceArray<double4> d_pts[2];
+  DeviceArray<uint8_t> d_mask;  // [3][arena_cap], shared by both slots (stream-ordered)
+  DeviceArray<double> d_models[2];
+  DeviceArray<int32_t> d_sup;
+  DeviceArray<int32_t> d_success;
+  DeviceArray<int32_t> d_config[2];
+  DeviceArray<int32_t> d_inl_cnt[2];
+  DeviceArray<uint2> d_inliers[2];
+  PinnedArray<double> h_models[2];
+  PinnedArray<int32_t> h_config[2];
+  PinnedArray<int32_t> h_inl_cnt[2];
+  PinnedArray<uint2> h_inliers[2];
+  DeviceArray<double> d_e_scratch;       // E kernel: [batch][128][90] null spaces / models (five_point_warp.cuh)
+  GuidedBufs guided;
   bool guided_on[2] = {false, false};
-  double* h_models[2] = {nullptr, nullptr};
-  int32_t* h_config[2] = {nullptr, nullptr};
-  int32_t* h_inl_cnt[2] = {nullptr, nullptr};
-  uint2* h_inliers[2] = {nullptr, nullptr};
-  DevCamera* d_cams = nullptr;
-  // relative pose (compute_relative_pose), lazily allocated
-  double* d_pose[2] = {nullptr, nullptr};        // [batch][8] qvec, tvec, tri_angle
-  int32_t* d_pose_valid[2] = {nullptr, nullptr};
-  double* h_pose[2] = {nullptr, nullptr};
-  int32_t* h_pose_valid[2] = {nullptr, nullptr};
-  double* d_angles = nullptr;                    // [arena_cap] triangulation-angle scratch
+  PoseBufs pose[2];
+  DeviceArray<double> d_angles;          // [arena_cap] triangulation-angle scratch, lazily allocated
   bool pose_on[2] = {false, false};
-  double* d_e_scratch = nullptr;                 // E kernel: [batch][128][90] null spaces / models (five_point_warp.cuh)
-  DevDistortion* d_dist = nullptr;               // per image, only when any_distorted
-  double4* d_pts_undist[2] = {nullptr, nullptr}; // E-kernel input per slot, lazily allocated
+  DeviceArray<double4> d_pts_undist[2];  // E-kernel input per slot, lazily allocated
+};
+
+// The cameras of the resident image set, kept while the set stays.
+struct VerifyCams {
+  DeviceArray<DevCamera> d_cams;
+  DeviceArray<DevDistortion> d_dist;  // per image, only when any_distorted
   bool any_distorted = false;
-  unsigned long long* d_prof = nullptr;
-  RansacStreams rs;
   int n_cams = 0;
   uint64_t cams_of = 0;  // ImageSet::generation the cameras were uploaded for
-  void release() {
-    for (int s = 0; s < 2; ++s) {
-      cudaFree(d_pts[s]); cudaFree(d_models[s]); cudaFree(d_config[s]); cudaFree(d_inl_cnt[s]); cudaFree(d_inliers[s]);
-      cudaFreeHost(h_models[s]); cudaFreeHost(h_config[s]); cudaFreeHost(h_inl_cnt[s]); cudaFreeHost(h_inliers[s]);
-      d_pts[s] = nullptr; d_models[s] = nullptr; d_config[s] = nullptr; d_inl_cnt[s] = nullptr; d_inliers[s] = nullptr;
-      h_models[s] = nullptr; h_config[s] = nullptr; h_inl_cnt[s] = nullptr; h_inliers[s] = nullptr;
-    }
-    cudaFree(d_mask); cudaFree(d_sup); cudaFree(d_success); cudaFree(d_cams);
-    for (int s = 0; s < 2; ++s) {
-      cudaFree(d_pose[s]); cudaFree(d_pose_valid[s]); cudaFreeHost(h_pose[s]); cudaFreeHost(h_pose_valid[s]);
-      d_pose[s] = nullptr; d_pose_valid[s] = nullptr; h_pose[s] = nullptr; h_pose_valid[s] = nullptr;
-      pose_on[s] = false;
-    }
-    cudaFree(d_angles);
-    d_angles = nullptr;
-    cudaFree(d_e_scratch);
-    d_e_scratch = nullptr;
-    cudaFree(d_dist); cudaFree(d_pts_undist[0]); cudaFree(d_pts_undist[1]);
-    d_dist = nullptr; d_pts_undist[0] = d_pts_undist[1] = nullptr; any_distorted = false;
-    cudaFree(d_guided_kind); cudaFree(d_guided_model);
-    d_guided_kind = nullptr; d_guided_model = nullptr;
-    for (int s = 0; s < 2; ++s) {
-      cudaFree(d_garena[s]); cudaFree(d_gcursor[s]); cudaFree(d_goff[s]); cudaFree(d_gcnt[s]);
-      cudaFreeHost(h_garena[s]); cudaFreeHost(h_gcursor[s]); cudaFreeHost(h_goff[s]); cudaFreeHost(h_gcnt[s]);
-      d_garena[s] = nullptr; d_gcursor[s] = nullptr; d_goff[s] = nullptr; d_gcnt[s] = nullptr;
-      h_garena[s] = nullptr; h_gcursor[s] = nullptr; h_goff[s] = nullptr; h_gcnt[s] = nullptr;
-      guided_on[s] = false;
-    }
-    d_mask = nullptr; d_sup = nullptr; d_success = nullptr; d_cams = nullptr;
-    batch = 0; arena_cap = 0; n_cams = 0; cams_of = 0;
-  }
+};
+
+struct VerifyState {
+  VerifyBatch w;
+  VerifyCams c;
+  RansacStreams rs;
+  DeviceArray<unsigned long long> d_prof;
 };
 
 VerifyState* vstate(b2m_ctx* ctx) {
   if (!ctx->verify_state) ctx->verify_state = new VerifyState();
   return static_cast<VerifyState*>(ctx->verify_state);
-}
-
-#define V_TRY(ctx, expr)                                                                    \
-  do {                                                                                      \
-    cudaError_t _e = (expr);                                                                \
-    if (_e != cudaSuccess) {                                                                \
-      char _b[512];                                                                         \
-      snprintf(_b, sizeof(_b), "[%s:%d] CUDA error: %s (%s)", __FILE__, __LINE__,          \
-               cudaGetErrorString(_e), #expr);                                              \
-      (ctx)->err = _b;                                                                      \
-      return _e == cudaErrorMemoryAllocation ? B2M_ENOMEM : B2M_ECUDA;                      \
-    }                                                                                       \
-  } while (0)
-
-unsigned long long* verify_counters(b2m_ctx* ctx) {
-  if (!ctx->d_verify_counters) {
-    if (cudaMalloc(&ctx->d_verify_counters, sizeof(unsigned long long) * 6) != cudaSuccess) {
-      cudaGetLastError();
-      ctx->d_verify_counters = nullptr;
-      return nullptr;
-    }
-    cudaMemset(ctx->d_verify_counters, 0, sizeof(unsigned long long) * 6);
-  }
-  return ctx->d_verify_counters;
 }
 
 DevCamera to_dev(const b2m_camera& c) {
@@ -1321,98 +1284,91 @@ DevDistortion to_dist(const b2m_camera& c) {
 
 int ensure_verify_ws(b2m_ctx* ctx, int batch, int64_t arena_cap) {
   VerifyState* V = vstate(ctx);
-  if (V->batch >= batch && V->arena_cap >= arena_cap) return B2M_OK;
-  DevCamera* keep_cams = V->d_cams;
-  const int keep_n = V->n_cams;
-  const uint64_t keep_of = V->cams_of;
-  DevDistortion* keep_dist = V->d_dist;
-  const bool keep_any = V->any_distorted;
-  V->d_cams = nullptr;
-  V->d_dist = nullptr;
-  V->release();
-  V->d_cams = keep_cams; V->n_cams = keep_n; V->cams_of = keep_of;
-  V->d_dist = keep_dist; V->any_distorted = keep_any;
-  for (int s = 0; s < 2; ++s) {
-    V_TRY(ctx, cudaMalloc(&V->d_pts[s], sizeof(double4) * arena_cap));
-    V_TRY(ctx, cudaMalloc(&V->d_models[s], sizeof(double) * 27 * batch));
-    V_TRY(ctx, cudaMalloc(&V->d_config[s], sizeof(int32_t) * batch));
-    V_TRY(ctx, cudaMalloc(&V->d_inl_cnt[s], sizeof(int32_t) * batch));
-    V_TRY(ctx, cudaMalloc(&V->d_inliers[s], sizeof(uint2) * arena_cap));
-    V_TRY(ctx, cudaMallocHost(&V->h_models[s], sizeof(double) * 27 * batch));
-    V_TRY(ctx, cudaMallocHost(&V->h_config[s], sizeof(int32_t) * batch));
-    V_TRY(ctx, cudaMallocHost(&V->h_inl_cnt[s], sizeof(int32_t) * batch));
-    V_TRY(ctx, cudaMallocHost(&V->h_inliers[s], sizeof(uint2) * arena_cap));
-  }
-  V_TRY(ctx, cudaMalloc(&V->d_mask, 3 * arena_cap));
-  V_TRY(ctx, cudaMalloc(&V->d_e_scratch, sizeof(double) * kEStride * kRansacThreads * static_cast<size_t>(batch)));
-  V_TRY(ctx, cudaMalloc(&V->d_sup, sizeof(int32_t) * 3 * batch));
-  V_TRY(ctx, cudaMalloc(&V->d_success, sizeof(int32_t) * 3 * batch));
-  V->batch = batch;
-  V->arena_cap = arena_cap;
-  return B2M_OK;
+  if (V->w.batch >= batch && V->w.arena_cap >= arena_cap) return B2M_OK;
+  return alloc_group(V->w, [&](VerifyBatch& w) -> int {
+    for (int s = 0; s < 2; ++s) {
+      B2M_CUDA_TRY(ctx, w.d_pts[s].ensure(arena_cap));
+      B2M_CUDA_TRY(ctx, w.d_models[s].ensure(27 * static_cast<size_t>(batch)));
+      B2M_CUDA_TRY(ctx, w.d_config[s].ensure(batch));
+      B2M_CUDA_TRY(ctx, w.d_inl_cnt[s].ensure(batch));
+      B2M_CUDA_TRY(ctx, w.d_inliers[s].ensure(arena_cap));
+      B2M_CUDA_TRY(ctx, w.h_models[s].ensure(27 * static_cast<size_t>(batch)));
+      B2M_CUDA_TRY(ctx, w.h_config[s].ensure(batch));
+      B2M_CUDA_TRY(ctx, w.h_inl_cnt[s].ensure(batch));
+      B2M_CUDA_TRY(ctx, w.h_inliers[s].ensure(arena_cap));
+    }
+    B2M_CUDA_TRY(ctx, w.d_mask.ensure(3 * arena_cap));
+    B2M_CUDA_TRY(ctx, w.d_e_scratch.ensure(static_cast<size_t>(kEStride) * kRansacThreads * batch));
+    B2M_CUDA_TRY(ctx, w.d_sup.ensure(3 * static_cast<size_t>(batch)));
+    B2M_CUDA_TRY(ctx, w.d_success.ensure(3 * static_cast<size_t>(batch)));
+    w.batch = batch;
+    w.arena_cap = arena_cap;
+    return B2M_OK;
+  });
 }
 
 }  // namespace
 
 void* verify_points_arena(b2m_ctx* ctx, int s) {
   VerifyState* V = vstate(ctx);
-  return V->d_pts[s];
+  return V->w.d_pts[s];
 }
 
 int verify_prepare(b2m_ctx* ctx, ImageSet& S, int batch, int64_t arena_cap) {
   if (int rc = ensure_verify_ws(ctx, batch, arena_cap)) return rc;
   VerifyState* V = vstate(ctx);
-  if (V->cams_of != S.generation || V->n_cams != S.n_images) {
-    cudaFree(V->d_cams);
-    V->d_cams = nullptr;
+  if (V->c.cams_of == S.generation && V->c.n_cams == S.n_images) return B2M_OK;
+  return alloc_group(V->c, [&](VerifyCams& c) -> int {
     std::vector<DevCamera> dc(S.n_images);
     for (int i = 0; i < S.n_images; ++i) dc[i] = to_dev(S.cams[i]);
-    V_TRY(ctx, cudaMalloc(&V->d_cams, sizeof(DevCamera) * std::max(1, S.n_images)));
-    V_TRY(ctx, cudaMemcpyAsync(V->d_cams, dc.data(), sizeof(DevCamera) * S.n_images, cudaMemcpyHostToDevice,
-                               ctx->stream));
-    cudaFree(V->d_dist);
-    V->d_dist = nullptr;
-    V->any_distorted = false;
-    for (const DevCamera& c : dc) V->any_distorted = V->any_distorted || c.distorted;
+    B2M_CUDA_TRY(ctx, c.d_cams.ensure(S.n_images));
+    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(c.d_cams, dc.data(), sizeof(DevCamera) * S.n_images, cudaMemcpyHostToDevice,
+                                      ctx->stream));
+    for (const DevCamera& d : dc) c.any_distorted = c.any_distorted || d.distorted;
     std::vector<DevDistortion> dd;
-    if (V->any_distorted) {
+    if (c.any_distorted) {
       dd.resize(S.n_images);
       for (int i = 0; i < S.n_images; ++i) dd[i] = to_dist(S.cams[i]);
-      V_TRY(ctx, cudaMalloc(&V->d_dist, sizeof(DevDistortion) * S.n_images));
-      V_TRY(ctx, cudaMemcpyAsync(V->d_dist, dd.data(), sizeof(DevDistortion) * S.n_images, cudaMemcpyHostToDevice,
-                                 ctx->stream));
+      B2M_CUDA_TRY(ctx, c.d_dist.ensure(S.n_images));
+      B2M_CUDA_TRY(ctx, cudaMemcpyAsync(c.d_dist, dd.data(), sizeof(DevDistortion) * S.n_images, cudaMemcpyHostToDevice,
+                                        ctx->stream));
     }
-    V_TRY(ctx, cudaStreamSynchronize(ctx->stream));
-    V->n_cams = S.n_images;
-    V->cams_of = S.generation;
-  }
-  return B2M_OK;
+    B2M_CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+    c.n_cams = S.n_images;
+    c.cams_of = S.generation;
+    return B2M_OK;
+  });
 }
 
 int verify_guided_slot(b2m_ctx* ctx, int s, GuidedSlot* out) {
-  VerifyState* V = vstate(ctx);
-  if (!V->d_guided_kind) {
-    V_TRY(ctx, cudaMalloc(&V->d_guided_kind, sizeof(int32_t) * V->batch));
-    V_TRY(ctx, cudaMalloc(&V->d_guided_model, sizeof(float) * 9 * V->batch));
-    for (int k = 0; k < 2; ++k) {
-      V_TRY(ctx, cudaMalloc(&V->d_garena[k], sizeof(uint2) * V->arena_cap));
-      V_TRY(ctx, cudaMalloc(&V->d_gcursor[k], sizeof(unsigned long long)));
-      V_TRY(ctx, cudaMalloc(&V->d_goff[k], sizeof(int64_t) * V->batch));
-      V_TRY(ctx, cudaMalloc(&V->d_gcnt[k], sizeof(int32_t) * V->batch));
-      V_TRY(ctx, cudaMallocHost(&V->h_garena[k], sizeof(uint2) * V->arena_cap));
-      V_TRY(ctx, cudaMallocHost(&V->h_gcursor[k], sizeof(unsigned long long)));
-      V_TRY(ctx, cudaMallocHost(&V->h_goff[k], sizeof(int64_t) * V->batch));
-      V_TRY(ctx, cudaMallocHost(&V->h_gcnt[k], sizeof(int32_t) * V->batch));
-    }
+  VerifyBatch& w = vstate(ctx)->w;
+  GuidedBufs& g = w.guided;
+  if (!g.d_guided_kind) {
+    const int rc = alloc_group(g, [&](GuidedBufs& g) -> int {
+      B2M_CUDA_TRY(ctx, g.d_guided_kind.ensure(w.batch));
+      B2M_CUDA_TRY(ctx, g.d_guided_model.ensure(9 * static_cast<size_t>(w.batch)));
+      for (int k = 0; k < 2; ++k) {
+        B2M_CUDA_TRY(ctx, g.d_garena[k].ensure(w.arena_cap));
+        B2M_CUDA_TRY(ctx, g.d_gcursor[k].ensure(1));
+        B2M_CUDA_TRY(ctx, g.d_goff[k].ensure(w.batch));
+        B2M_CUDA_TRY(ctx, g.d_gcnt[k].ensure(w.batch));
+        B2M_CUDA_TRY(ctx, g.h_garena[k].ensure(w.arena_cap));
+        B2M_CUDA_TRY(ctx, g.h_gcursor[k].ensure(1));
+        B2M_CUDA_TRY(ctx, g.h_goff[k].ensure(w.batch));
+        B2M_CUDA_TRY(ctx, g.h_gcnt[k].ensure(w.batch));
+      }
+      return B2M_OK;
+    });
+    if (rc) return rc;
   }
-  out->kind = V->d_guided_kind;
-  out->model = V->d_guided_model;
-  out->arena = V->d_garena[s];
-  out->cursor = V->d_gcursor[s];
-  out->off = V->d_goff[s];
-  out->cnt = V->d_gcnt[s];
-  out->h_cursor = V->h_gcursor[s];
-  V->guided_on[s] = true;
+  out->kind = g.d_guided_kind;
+  out->model = g.d_guided_model;
+  out->arena = g.d_garena[s];
+  out->cursor = g.d_gcursor[s];
+  out->off = g.d_goff[s];
+  out->cnt = g.d_gcnt[s];
+  out->h_cursor = g.h_gcursor[s];
+  w.guided_on[s] = true;
   return B2M_OK;
 }
 
@@ -1435,22 +1391,22 @@ int verify_batch_launch(b2m_ctx* ctx, ImageSet& S, const b2m_tvg_opts* tvg, cons
   P.pairs = ctx->d_pairs + 2 * p0;
   P.pair_off = W.d_pair_off[s];
   P.pair_cnt = W.d_pair_cnt[s];
-  P.pts = V->d_pts[s];
+  P.pts = V->w.d_pts[s];
   P.matches = W.d_arena[s];
-  P.cams = V->d_cams;
-  P.mask = V->d_mask;
-  P.arena_cap = V->arena_cap;
-  P.models = V->d_models[s];
-  P.sup_cnt = V->d_sup;
-  P.success = V->d_success;
-  P.config = V->d_config[s];
-  P.inl_cnt = V->d_inl_cnt[s];
-  P.inliers = V->d_inliers[s];
+  P.cams = V->c.d_cams;
+  P.mask = V->w.d_mask;
+  P.arena_cap = V->w.arena_cap;
+  P.models = V->w.d_models[s];
+  P.sup_cnt = V->w.d_sup;
+  P.success = V->w.d_success;
+  P.config = V->w.d_config[s];
+  P.inl_cnt = V->w.d_inl_cnt[s];
+  P.inliers = V->w.d_inliers[s];
   P.opt = *tvg;
   P.seed = ctx->seed;
   P.single_kind = -1;
   P.force_calibrated = -1;
-  V->guided_on[s] = false;
+  V->w.guided_on[s] = false;
   P.guided_min_inliers = -1;
   if (sift && sift->guided_matching) {
     GuidedSlot gs;
@@ -1460,41 +1416,49 @@ int verify_batch_launch(b2m_ctx* ctx, ImageSet& S, const b2m_tvg_opts* tvg, cons
     P.guided_min_inliers = tvg->min_num_inliers;
   }
   if (!V->d_prof && getenv("B2M_PROF")) {
-    cudaMalloc(&V->d_prof, sizeof(unsigned long long) * 24);
+    V->d_prof.ensure(24);
     cudaMemset(V->d_prof, 0, sizeof(unsigned long long) * 24);
   }
   P.prof = V->d_prof;
-  P.counters = verify_counters(ctx);
-  P.e_scratch = V->d_e_scratch;
+  P.counters = ctx->d_counters + kVerifyCounters;
+  P.e_scratch = V->w.d_e_scratch;
   P.lo_eig_thread = lo_eig_thread_mode();
   if (!V->rs.side[0]) {
-    V_TRY(ctx, cudaStreamCreateWithFlags(&V->rs.side[0], cudaStreamNonBlocking));
-    V_TRY(ctx, cudaStreamCreateWithFlags(&V->rs.side[1], cudaStreamNonBlocking));
-    V_TRY(ctx, cudaEventCreateWithFlags(&V->rs.fork, cudaEventDisableTiming));
-    V_TRY(ctx, cudaEventCreateWithFlags(&V->rs.join[0], cudaEventDisableTiming));
-    V_TRY(ctx, cudaEventCreateWithFlags(&V->rs.join[1], cudaEventDisableTiming));
+    const int rc = alloc_group(V->rs, [&](RansacStreams& r) -> int {
+      B2M_CUDA_TRY(ctx, r.side[0].create(cudaStreamNonBlocking));
+      B2M_CUDA_TRY(ctx, r.side[1].create(cudaStreamNonBlocking));
+      B2M_CUDA_TRY(ctx, r.fork.create(cudaEventDisableTiming));
+      B2M_CUDA_TRY(ctx, r.join[0].create(cudaEventDisableTiming));
+      B2M_CUDA_TRY(ctx, r.join[1].create(cudaEventDisableTiming));
+      return B2M_OK;
+    });
+    if (rc) return rc;
   }
   const double4* pts_E = nullptr;
-  if (V->any_distorted) {  // distortion models: the E kernel reads undistorted points (row V9)
-    if (!V->d_pts_undist[s]) V_TRY(ctx, cudaMalloc(&V->d_pts_undist[s], sizeof(double4) * V->arena_cap));
-    b2m_undistort_kernel<<<nb, 256, 0, ctx->stream>>>(P, V->d_dist, V->d_pts_undist[s]);
-    V_TRY(ctx, cudaGetLastError());
+  if (V->c.any_distorted) {  // distortion models: the E kernel reads undistorted points (row V9)
+    B2M_CUDA_TRY(ctx, V->w.d_pts_undist[s].ensure(V->w.arena_cap));
+    b2m_undistort_kernel<<<nb, 256, 0, ctx->stream>>>(P, V->c.d_dist, V->w.d_pts_undist[s]);
+    B2M_CUDA_TRY(ctx, cudaGetLastError());
     ctx->stats.kernel_launches += 1;
-    pts_E = V->d_pts_undist[s];
+    pts_E = V->w.d_pts_undist[s];
   }
-  V_TRY(ctx, launch_ransac(P, nb, ctx->stream, &V->rs, pts_E));
+  B2M_CUDA_TRY(ctx, launch_ransac(P, nb, ctx->stream, &V->rs, pts_E));
   ctx->stats.kernel_launches += 2;
   b2m_decide_kernel<<<nb, 256, 0, ctx->stream>>>(P);
-  V_TRY(ctx, cudaGetLastError());
+  B2M_CUDA_TRY(ctx, cudaGetLastError());
   ctx->stats.kernel_launches += 2;
-  V->pose_on[s] = false;
+  V->w.pose_on[s] = false;
   if (tvg->compute_relative_pose) {  // EstimateTwoViewGeometryPose on the verified pairs of the batch
-    if (!V->d_angles) V_TRY(ctx, cudaMalloc(&V->d_angles, sizeof(double) * V->arena_cap));
-    if (!V->d_pose[s]) {
-      V_TRY(ctx, cudaMalloc(&V->d_pose[s], sizeof(double) * 8 * V->batch));
-      V_TRY(ctx, cudaMalloc(&V->d_pose_valid[s], sizeof(int32_t) * V->batch));
-      V_TRY(ctx, cudaMallocHost(&V->h_pose[s], sizeof(double) * 8 * V->batch));
-      V_TRY(ctx, cudaMallocHost(&V->h_pose_valid[s], sizeof(int32_t) * V->batch));
+    B2M_CUDA_TRY(ctx, V->w.d_angles.ensure(V->w.arena_cap));
+    if (!V->w.pose[s].d_pose) {
+      const int rc = alloc_group(V->w.pose[s], [&](PoseBufs& q) -> int {
+        B2M_CUDA_TRY(ctx, q.d_pose.ensure(8 * static_cast<size_t>(V->w.batch)));
+        B2M_CUDA_TRY(ctx, q.d_pose_valid.ensure(V->w.batch));
+        B2M_CUDA_TRY(ctx, q.h_pose.ensure(8 * static_cast<size_t>(V->w.batch)));
+        B2M_CUDA_TRY(ctx, q.h_pose_valid.ensure(V->w.batch));
+        return B2M_OK;
+      });
+      if (rc) return rc;
     }
     PoseParams Q{};
     Q.pairs = P.pairs;
@@ -1504,16 +1468,16 @@ int verify_batch_launch(b2m_ctx* ctx, ImageSet& S, const b2m_tvg_opts* tvg, cons
     Q.inliers = P.inliers;
     Q.models = P.models;
     Q.cams = P.cams;
-    Q.dist = V->any_distorted ? V->d_dist : nullptr;
+    Q.dist = V->c.any_distorted ? static_cast<const DevDistortion*>(V->c.d_dist) : nullptr;
     Q.kpts = S.d_kpts;
     Q.img_row0 = S.d_row0;
-    Q.angles = V->d_angles;
-    Q.out = V->d_pose[s];
-    Q.out_valid = V->d_pose_valid[s];
+    Q.angles = V->w.d_angles;
+    Q.out = V->w.pose[s].d_pose;
+    Q.out_valid = V->w.pose[s].d_pose_valid;
     b2m_pose_kernel<<<nb, 256, 0, ctx->stream>>>(Q);
-    V_TRY(ctx, cudaGetLastError());
+    B2M_CUDA_TRY(ctx, cudaGetLastError());
     ctx->stats.kernel_launches += 1;
-    V->pose_on[s] = true;
+    V->w.pose_on[s] = true;
   }
   return B2M_OK;
 }
@@ -1522,28 +1486,28 @@ int verify_batch_download(b2m_ctx* ctx, b2m_results*, int s, int64_t, int nb) {
   VerifyState* V = vstate(ctx);
   Workspace& W = ctx->ws;
   const unsigned long long total = *W.h_cursor[s];
-  V_TRY(ctx, cudaMemcpyAsync(V->h_models[s], V->d_models[s], sizeof(double) * 27 * nb, cudaMemcpyDeviceToHost,
+  B2M_CUDA_TRY(ctx, cudaMemcpyAsync(V->w.h_models[s], V->w.d_models[s], sizeof(double) * 27 * nb, cudaMemcpyDeviceToHost,
                              ctx->copy_stream));
-  V_TRY(ctx, cudaMemcpyAsync(V->h_config[s], V->d_config[s], sizeof(int32_t) * nb, cudaMemcpyDeviceToHost,
+  B2M_CUDA_TRY(ctx, cudaMemcpyAsync(V->w.h_config[s], V->w.d_config[s], sizeof(int32_t) * nb, cudaMemcpyDeviceToHost,
                              ctx->copy_stream));
-  V_TRY(ctx, cudaMemcpyAsync(V->h_inl_cnt[s], V->d_inl_cnt[s], sizeof(int32_t) * nb, cudaMemcpyDeviceToHost,
+  B2M_CUDA_TRY(ctx, cudaMemcpyAsync(V->w.h_inl_cnt[s], V->w.d_inl_cnt[s], sizeof(int32_t) * nb, cudaMemcpyDeviceToHost,
                              ctx->copy_stream));
   if (total > 0)
-    V_TRY(ctx, cudaMemcpyAsync(V->h_inliers[s], V->d_inliers[s], sizeof(uint2) * total, cudaMemcpyDeviceToHost,
+    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(V->w.h_inliers[s], V->w.d_inliers[s], sizeof(uint2) * total, cudaMemcpyDeviceToHost,
                                ctx->copy_stream));
-  if (V->pose_on[s]) {
-    V_TRY(ctx, cudaMemcpyAsync(V->h_pose[s], V->d_pose[s], sizeof(double) * 8 * nb, cudaMemcpyDeviceToHost, ctx->copy_stream));
-    V_TRY(ctx, cudaMemcpyAsync(V->h_pose_valid[s], V->d_pose_valid[s], sizeof(int32_t) * nb, cudaMemcpyDeviceToHost,
+  if (V->w.pose_on[s]) {
+    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(V->w.pose[s].h_pose, V->w.pose[s].d_pose, sizeof(double) * 8 * nb, cudaMemcpyDeviceToHost, ctx->copy_stream));
+    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(V->w.pose[s].h_pose_valid, V->w.pose[s].d_pose_valid, sizeof(int32_t) * nb, cudaMemcpyDeviceToHost,
                                ctx->copy_stream));
   }
-  if (V->guided_on[s]) {
-    const unsigned long long gtotal = *V->h_gcursor[s];
-    V_TRY(ctx, cudaMemcpyAsync(V->h_goff[s], V->d_goff[s], sizeof(int64_t) * nb, cudaMemcpyDeviceToHost,
+  if (V->w.guided_on[s]) {
+    const unsigned long long gtotal = *V->w.guided.h_gcursor[s];
+    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(V->w.guided.h_goff[s], V->w.guided.d_goff[s], sizeof(int64_t) * nb, cudaMemcpyDeviceToHost,
                                ctx->copy_stream));
-    V_TRY(ctx, cudaMemcpyAsync(V->h_gcnt[s], V->d_gcnt[s], sizeof(int32_t) * nb, cudaMemcpyDeviceToHost,
+    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(V->w.guided.h_gcnt[s], V->w.guided.d_gcnt[s], sizeof(int32_t) * nb, cudaMemcpyDeviceToHost,
                                ctx->copy_stream));
     if (gtotal > 0)
-      V_TRY(ctx, cudaMemcpyAsync(V->h_garena[s], V->d_garena[s], sizeof(uint2) * gtotal, cudaMemcpyDeviceToHost,
+      B2M_CUDA_TRY(ctx, cudaMemcpyAsync(V->w.guided.h_garena[s], V->w.guided.d_garena[s], sizeof(uint2) * gtotal, cudaMemcpyDeviceToHost,
                                  ctx->copy_stream));
   }
   return B2M_OK;
@@ -1554,13 +1518,13 @@ int verify_batch_collect(b2m_ctx* ctx, b2m_results* res, int s, int64_t p0, int 
   Workspace& W = ctx->ws;
   for (int k = 0; k < nb; ++k) {
     const int64_t p = p0 + k;
-    int cfg = V->h_config[s][k];
-    int ni = V->h_inl_cnt[s][k];
-    const uint2* inl_src = V->h_inliers[s] + W.h_pair_off[s][k];
-    if (V->guided_on[s] && V->h_gcnt[s][k] >= 0) {
+    int cfg = V->w.h_config[s][k];
+    int ni = V->w.h_inl_cnt[s][k];
+    const uint2* inl_src = V->w.h_inliers[s] + W.h_pair_off[s][k];
+    if (V->w.guided_on[s] && V->w.guided.h_gcnt[s][k] >= 0) {
       // guided matching replaced TwoViewGeometry::inlier_matches (U:feature/sift.cc MatchGuidedSiftFeaturesCPU)
-      ni = V->h_gcnt[s][k];
-      inl_src = V->h_garena[s] + V->h_goff[s][k];
+      ni = V->w.guided.h_gcnt[s][k];
+      inl_src = V->w.guided.h_garena[s] + V->w.guided.h_goff[s][k];
     }
     // FeatureMatcherController::Match write rule (row P3): raw matches below min_num_inliers are
     // stored empty (the verifier never ran: default TwoViewGeometry); geometries with fewer than
@@ -1574,15 +1538,15 @@ int verify_batch_collect(b2m_ctx* ctx, b2m_results* res, int s, int64_t p0, int 
       cfg = B2M_UNDEFINED;
       ni = 0;
     }
-    if (V->pose_on[s]) {
+    if (V->w.pose_on[s]) {
       if (res->poses.empty()) {
         const size_t np = res->config.size();
         res->poses.assign(8 * np, 0.0);
         for (size_t q = 0; q < np; ++q) res->poses[8 * q] = 1.0;
         res->pose_valid.assign(np, 0);
       }
-      if (ni > 0 && V->h_pose_valid[s][k]) {
-        memcpy(res->poses.data() + 8 * p, V->h_pose[s] + 8 * k, sizeof(double) * 8);
+      if (ni > 0 && V->w.pose[s].h_pose_valid[k]) {
+        memcpy(res->poses.data() + 8 * p, V->w.pose[s].h_pose + 8 * k, sizeof(double) * 8);
         res->pose_valid[p] = 1;
       }
     }
@@ -1595,29 +1559,25 @@ int verify_batch_collect(b2m_ctx* ctx, b2m_results* res, int s, int64_t p0, int 
       res->inliers.resize(at + 2 * static_cast<size_t>(ni));
       memcpy(res->inliers.data() + at, src, sizeof(uint2) * ni);
       res->model_idx[p] = static_cast<int32_t>(res->models.size() / 27);
-      res->models.insert(res->models.end(), V->h_models[s] + 27 * k, V->h_models[s] + 27 * k + 27);
+      res->models.insert(res->models.end(), V->w.h_models[s] + 27 * k, V->w.h_models[s] + 27 * k + 27);
     }
   }
   return B2M_OK;
 }
 
 void verify_release(b2m_ctx* ctx) {
-  if (ctx->verify_state) {
-    VerifyState* V = static_cast<VerifyState*>(ctx->verify_state);
-    if (V->d_prof) {
-      unsigned long long h[24];
-      cudaMemcpy(h, V->d_prof, sizeof(h), cudaMemcpyDeviceToHost);
-      const char* names[8] = {"solve", "score", "exact_support", "lo_accumulate", "lo_solve", "lo_score", "final", "-"};
-      for (int k = 0; k < 3; ++k)
-        for (int j = 0; j < 7; ++j)
-          fprintf(stderr, "[b2m prof] kind %d %-14s %10.3f Mcycles\n", k, names[j], h[k * 8 + j] / 1e6);
-      cudaFree(V->d_prof);
-      V->d_prof = nullptr;
-    }
-    V->release();
-    delete V;
-    ctx->verify_state = nullptr;
+  VerifyState* V = static_cast<VerifyState*>(ctx->verify_state);
+  if (!V) return;
+  if (V->d_prof) {
+    unsigned long long h[24];
+    cudaMemcpy(h, V->d_prof, sizeof(h), cudaMemcpyDeviceToHost);
+    const char* names[8] = {"solve", "score", "exact_support", "lo_accumulate", "lo_solve", "lo_score", "final", "-"};
+    for (int k = 0; k < 3; ++k)
+      for (int j = 0; j < 7; ++j)
+        fprintf(stderr, "[b2m prof] kind %d %-14s %10.3f Mcycles\n", k, names[j], h[k * 8 + j] / 1e6);
   }
+  delete V;
+  ctx->verify_state = nullptr;
 }
 
 // ---- stand-alone estimators ------------------------------------------------------------------
@@ -1625,27 +1585,21 @@ void verify_release(b2m_ctx* ctx) {
 namespace {
 
 struct Single {
-  double4* d_pts = nullptr;
-  uint2* d_matches = nullptr;
-  uint2* d_inliers = nullptr;
-  uint8_t* d_mask = nullptr;
-  DevCamera* d_cams = nullptr;
-  int32_t* d_i32 = nullptr;   // pairs[2], cnt[1], sup[3], success[3], config[1], inl_cnt[1]
-  int64_t* d_off = nullptr;
-  double* d_models = nullptr;
-  DevDistortion* d_dist = nullptr;  // only when a camera has distortion
-  double4* d_pts_undist = nullptr;
-  double* d_e_scratch = nullptr;    // E kernel scratch, [problems][128][90]
+  DeviceArray<double4> d_pts;
+  DeviceArray<uint2> d_matches;
+  DeviceArray<uint2> d_inliers;
+  DeviceArray<uint8_t> d_mask;
+  DeviceArray<DevCamera> d_cams;
+  DeviceArray<int32_t> d_i32;   // pairs[2], cnt[1], sup[3], success[3], config[1], inl_cnt[1]
+  DeviceArray<int64_t> d_off;
+  DeviceArray<double> d_models;
+  DeviceArray<DevDistortion> d_dist;  // only when a camera has distortion
+  DeviceArray<double4> d_pts_undist;
+  DeviceArray<double> d_e_scratch;    // E kernel scratch, [problems][128][90]
   // compute_relative_pose
-  double *d_p1 = nullptr, *d_p2 = nullptr, *d_angles = nullptr, *d_pose = nullptr;
-  int64_t *d_p1_off = nullptr, *d_p2_off = nullptr;
-  int32_t* d_pose_valid = nullptr;
-  ~Single() {
-    cudaFree(d_pts); cudaFree(d_matches); cudaFree(d_inliers); cudaFree(d_mask); cudaFree(d_cams);
-    cudaFree(d_i32); cudaFree(d_off); cudaFree(d_models); cudaFree(d_dist); cudaFree(d_pts_undist); cudaFree(d_e_scratch);
-    cudaFree(d_p1); cudaFree(d_p2); cudaFree(d_angles); cudaFree(d_pose); cudaFree(d_p1_off); cudaFree(d_p2_off);
-    cudaFree(d_pose_valid);
-  }
+  DeviceArray<double> d_p1, d_p2, d_angles, d_pose;
+  DeviceArray<int64_t> d_p1_off, d_p2_off;
+  DeviceArray<int32_t> d_pose_valid;
 };
 
 // Stand-alone estimator calls with compute_relative_pose: upload the callers' point arrays (concatenated over the
@@ -1654,28 +1608,28 @@ struct Single {
 int launch_pose_standalone(b2m_ctx* ctx, Single& G, const VerifyParams& P, int nb, int64_t cap, const std::vector<double>& p1,
                            const std::vector<double>& p2, const std::vector<int64_t>& off1, const std::vector<int64_t>& off2,
                            const b2m_camera* const* cams, int n_cams, cudaStream_t st) {
-  V_TRY(ctx, cudaMalloc(&G.d_p1, sizeof(double) * std::max<size_t>(p1.size(), 2)));
-  V_TRY(ctx, cudaMalloc(&G.d_p2, sizeof(double) * std::max<size_t>(p2.size(), 2)));
-  V_TRY(ctx, cudaMalloc(&G.d_p1_off, sizeof(int64_t) * nb));
-  V_TRY(ctx, cudaMalloc(&G.d_p2_off, sizeof(int64_t) * nb));
-  V_TRY(ctx, cudaMalloc(&G.d_angles, sizeof(double) * cap));
-  V_TRY(ctx, cudaMalloc(&G.d_pose, sizeof(double) * 8 * nb));
-  V_TRY(ctx, cudaMalloc(&G.d_pose_valid, sizeof(int32_t) * nb));
+  B2M_CUDA_TRY(ctx, G.d_p1.ensure(std::max<size_t>(p1.size(), 2)));
+  B2M_CUDA_TRY(ctx, G.d_p2.ensure(std::max<size_t>(p2.size(), 2)));
+  B2M_CUDA_TRY(ctx, G.d_p1_off.ensure(nb));
+  B2M_CUDA_TRY(ctx, G.d_p2_off.ensure(nb));
+  B2M_CUDA_TRY(ctx, G.d_angles.ensure(cap));
+  B2M_CUDA_TRY(ctx, G.d_pose.ensure(8 * nb));
+  B2M_CUDA_TRY(ctx, G.d_pose_valid.ensure(nb));
   if (!G.d_dist) {  // undistort_for_E uploads the models only when it had to; the pose kernel needs them as well
     bool any = false;
     for (int i = 0; i < n_cams; ++i) any = any || cam::has_distortion(cams[i]->model);
     if (any) {
       std::vector<DevDistortion> dd(n_cams);
       for (int i = 0; i < n_cams; ++i) dd[i] = to_dist(*cams[i]);
-      V_TRY(ctx, cudaMalloc(&G.d_dist, sizeof(DevDistortion) * n_cams));
-      V_TRY(ctx, cudaMemcpy(G.d_dist, dd.data(), sizeof(DevDistortion) * n_cams, cudaMemcpyHostToDevice));
+      B2M_CUDA_TRY(ctx, G.d_dist.ensure(n_cams));
+      B2M_CUDA_TRY(ctx, cudaMemcpy(G.d_dist, dd.data(), sizeof(DevDistortion) * n_cams, cudaMemcpyHostToDevice));
     }
   }
   // synchronous copies: the host vectors are the caller's locals
-  if (!p1.empty()) V_TRY(ctx, cudaMemcpy(G.d_p1, p1.data(), sizeof(double) * p1.size(), cudaMemcpyHostToDevice));
-  if (!p2.empty()) V_TRY(ctx, cudaMemcpy(G.d_p2, p2.data(), sizeof(double) * p2.size(), cudaMemcpyHostToDevice));
-  V_TRY(ctx, cudaMemcpy(G.d_p1_off, off1.data(), sizeof(int64_t) * nb, cudaMemcpyHostToDevice));
-  V_TRY(ctx, cudaMemcpy(G.d_p2_off, off2.data(), sizeof(int64_t) * nb, cudaMemcpyHostToDevice));
+  if (!p1.empty()) B2M_CUDA_TRY(ctx, cudaMemcpy(G.d_p1, p1.data(), sizeof(double) * p1.size(), cudaMemcpyHostToDevice));
+  if (!p2.empty()) B2M_CUDA_TRY(ctx, cudaMemcpy(G.d_p2, p2.data(), sizeof(double) * p2.size(), cudaMemcpyHostToDevice));
+  B2M_CUDA_TRY(ctx, cudaMemcpy(G.d_p1_off, off1.data(), sizeof(int64_t) * nb, cudaMemcpyHostToDevice));
+  B2M_CUDA_TRY(ctx, cudaMemcpy(G.d_p2_off, off2.data(), sizeof(int64_t) * nb, cudaMemcpyHostToDevice));
   PoseParams Q{};
   Q.pairs = P.pairs;
   Q.pair_off = P.pair_off;
@@ -1693,7 +1647,7 @@ int launch_pose_standalone(b2m_ctx* ctx, Single& G, const VerifyParams& P, int n
   Q.out = G.d_pose;
   Q.out_valid = G.d_pose_valid;
   b2m_pose_kernel<<<nb, 256, 0, st>>>(Q);
-  V_TRY(ctx, cudaGetLastError());
+  B2M_CUDA_TRY(ctx, cudaGetLastError());
   ctx->stats.kernel_launches += 1;
   return B2M_OK;
 }
@@ -1719,12 +1673,12 @@ int undistort_for_E(b2m_ctx* ctx, Single& G, const VerifyParams& P, const b2m_ca
   if (!any) return B2M_OK;
   std::vector<DevDistortion> dd(n_cams);
   for (int i = 0; i < n_cams; ++i) dd[i] = to_dist(*cams[i]);
-  V_TRY(ctx, cudaMalloc(&G.d_dist, sizeof(DevDistortion) * n_cams));
-  V_TRY(ctx, cudaMalloc(&G.d_pts_undist, sizeof(double4) * cap));
+  B2M_CUDA_TRY(ctx, G.d_dist.ensure(n_cams));
+  B2M_CUDA_TRY(ctx, G.d_pts_undist.ensure(cap));
   // synchronous copy: `dd` is a local that must not be read after this function returns
-  V_TRY(ctx, cudaMemcpy(G.d_dist, dd.data(), sizeof(DevDistortion) * n_cams, cudaMemcpyHostToDevice));
+  B2M_CUDA_TRY(ctx, cudaMemcpy(G.d_dist, dd.data(), sizeof(DevDistortion) * n_cams, cudaMemcpyHostToDevice));
   b2m_undistort_kernel<<<nb, 256, 0, st>>>(P, G.d_dist, G.d_pts_undist);
-  V_TRY(ctx, cudaGetLastError());
+  B2M_CUDA_TRY(ctx, cudaGetLastError());
   ctx->stats.kernel_launches += 1;
   *pts_E = G.d_pts_undist;
   return B2M_OK;
@@ -1738,26 +1692,26 @@ int run_single(b2m_ctx* ctx, const std::vector<double4>& pts, const std::vector<
                const double* raw2 = nullptr, int64_t n2 = 0) {
   const int64_t m = static_cast<int64_t>(pts.size());
   const int64_t cap = std::max<int64_t>(m, 1);
-  V_TRY(ctx, cudaMalloc(&G.d_pts, sizeof(double4) * cap));
-  V_TRY(ctx, cudaMalloc(&G.d_matches, sizeof(uint2) * cap));
-  V_TRY(ctx, cudaMalloc(&G.d_inliers, sizeof(uint2) * cap));
-  V_TRY(ctx, cudaMalloc(&G.d_mask, 3 * cap));
-  V_TRY(ctx, cudaMalloc(&G.d_cams, sizeof(DevCamera) * 2));
-  V_TRY(ctx, cudaMalloc(&G.d_i32, sizeof(int32_t) * 16));
-  V_TRY(ctx, cudaMalloc(&G.d_off, sizeof(int64_t)));
-  V_TRY(ctx, cudaMalloc(&G.d_models, sizeof(double) * 27));
-  V_TRY(ctx, cudaMalloc(&G.d_e_scratch, sizeof(double) * kEStride * kRansacThreads));
+  B2M_CUDA_TRY(ctx, G.d_pts.ensure(cap));
+  B2M_CUDA_TRY(ctx, G.d_matches.ensure(cap));
+  B2M_CUDA_TRY(ctx, G.d_inliers.ensure(cap));
+  B2M_CUDA_TRY(ctx, G.d_mask.ensure(3 * cap));
+  B2M_CUDA_TRY(ctx, G.d_cams.ensure(2));
+  B2M_CUDA_TRY(ctx, G.d_i32.ensure(16));
+  B2M_CUDA_TRY(ctx, G.d_off.ensure(1));
+  B2M_CUDA_TRY(ctx, G.d_models.ensure(27));
+  B2M_CUDA_TRY(ctx, G.d_e_scratch.ensure(static_cast<size_t>(kEStride) * kRansacThreads));
   const int32_t i32[16] = {0, 1, static_cast<int32_t>(m), 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
   const int64_t off0 = 0;
   cudaStream_t st = ctx->stream;
   if (m > 0) {
-    V_TRY(ctx, cudaMemcpyAsync(G.d_pts, pts.data(), sizeof(double4) * m, cudaMemcpyHostToDevice, st));
-    V_TRY(ctx, cudaMemcpyAsync(G.d_matches, matches.data(), sizeof(uint2) * m, cudaMemcpyHostToDevice, st));
+    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(G.d_pts, pts.data(), sizeof(double4) * m, cudaMemcpyHostToDevice, st));
+    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(G.d_matches, matches.data(), sizeof(uint2) * m, cudaMemcpyHostToDevice, st));
   }
-  V_TRY(ctx, cudaMemcpyAsync(G.d_cams, cams, sizeof(DevCamera) * 2, cudaMemcpyHostToDevice, st));
-  V_TRY(ctx, cudaMemcpyAsync(G.d_i32, i32, sizeof(i32), cudaMemcpyHostToDevice, st));
-  V_TRY(ctx, cudaMemcpyAsync(G.d_off, &off0, sizeof(int64_t), cudaMemcpyHostToDevice, st));
-  V_TRY(ctx, cudaMemsetAsync(G.d_models, 0, sizeof(double) * 27, st));
+  B2M_CUDA_TRY(ctx, cudaMemcpyAsync(G.d_cams, cams, sizeof(DevCamera) * 2, cudaMemcpyHostToDevice, st));
+  B2M_CUDA_TRY(ctx, cudaMemcpyAsync(G.d_i32, i32, sizeof(i32), cudaMemcpyHostToDevice, st));
+  B2M_CUDA_TRY(ctx, cudaMemcpyAsync(G.d_off, &off0, sizeof(int64_t), cudaMemcpyHostToDevice, st));
+  B2M_CUDA_TRY(ctx, cudaMemsetAsync(G.d_models, 0, sizeof(double) * 27, st));
   P = VerifyParams{};
   P.pairs = G.d_i32;
   P.pair_cnt = G.d_i32 + 2;
@@ -1776,27 +1730,27 @@ int run_single(b2m_ctx* ctx, const std::vector<double4>& pts, const std::vector<
   P.opt = opt;
   P.seed = ctx->seed;
   P.single_kind = single_kind;
-  P.counters = verify_counters(ctx);
+  P.counters = ctx->d_counters + kVerifyCounters;
   P.e_scratch = G.d_e_scratch;
   P.lo_eig_thread = lo_eig_thread_mode();
   if (single_kind >= 0) {
-    V_TRY(ctx, launch_ransac(P, 1, st));
+    B2M_CUDA_TRY(ctx, launch_ransac(P, 1, st));
   } else {
     const double4* pts_E = nullptr;
     if (full_cams)
       if (int rc = undistort_for_E(ctx, G, P, full_cams, 2, 1, cap, st, &pts_E)) return rc;
-    V_TRY(ctx, launch_ransac(P, 1, st, nullptr, pts_E));
+    B2M_CUDA_TRY(ctx, launch_ransac(P, 1, st, nullptr, pts_E));
     ctx->stats.kernel_launches += 2;
     b2m_decide_kernel<<<1, 256, 0, st>>>(P);
     ctx->stats.kernel_launches += 1;
     if (opt.compute_relative_pose && full_cams) {
-      V_TRY(ctx, cudaGetLastError());
+      B2M_CUDA_TRY(ctx, cudaGetLastError());
       const std::vector<double> p1(raw1, raw1 + 2 * n1), p2(raw2, raw2 + 2 * n2);
       const std::vector<int64_t> zero(1, 0);
       if (int rc = launch_pose_standalone(ctx, G, P, 1, cap, p1, p2, zero, zero, full_cams, 2, st)) return rc;
     }
   }
-  V_TRY(ctx, cudaGetLastError());
+  B2M_CUDA_TRY(ctx, cudaGetLastError());
   ctx->stats.kernel_launches += 1;
   return B2M_OK;
 }
@@ -1840,26 +1794,22 @@ static int estimate_tvg_once(b2m_ctx* ctx, const b2m_camera* cam1, const double*
                              const b2m_camera* cam2, const double* points2, int64_t n2, const uint32_t* matches,
                              int64_t m, const b2m_tvg_opts* opts, b2m_tvg_result* out, uint32_t* inlier_matches) {
   if (!ctx) return B2M_EINVAL;
-  auto bad = [&](const char* msg) {
-    ctx->err = msg;
-    return B2M_EINVAL;
-  };
-  if (!cam1 || !cam2 || !opts || !out) return bad("[verify.cu] Check Failed: cameras, options and out != NULL");
-  if (const char* why = camera_problem(*cam1)) return bad(why);
-  if (const char* why = camera_problem(*cam2)) return bad(why);
-  if (n1 < 0 || n2 < 0 || (n1 > 0 && !points1) || (n2 > 0 && !points2)) return bad("[verify.cu] Check Failed: points");
+  if (!cam1 || !cam2 || !opts || !out) return fail(ctx, B2M_EINVAL, "[verify.cu] Check Failed: cameras, options and out != NULL");
+  if (const char* why = camera_problem(*cam1)) return fail(ctx, B2M_EINVAL, why);
+  if (const char* why = camera_problem(*cam2)) return fail(ctx, B2M_EINVAL, why);
+  if (n1 < 0 || n2 < 0 || (n1 > 0 && !points1) || (n2 > 0 && !points2)) return fail(ctx, B2M_EINVAL, "[verify.cu] Check Failed: points");
   if (!matches) {  // identity matching (R:estimators/two_view_geometry.h:136-142)
-    if (n1 != n2) return bad("[verify.cu] Check Failed: points1.size() == points2.size()");
+    if (n1 != n2) return fail(ctx, B2M_EINVAL, "[verify.cu] Check Failed: points1.size() == points2.size()");
     m = n1;
   }
-  if (m < 0) return bad("[verify.cu] Check Failed: m >= 0");
+  if (m < 0) return fail(ctx, B2M_EINVAL, "[verify.cu] Check Failed: m >= 0");
   cudaSetDevice(ctx->device);
   std::vector<double4> pts(m);
   std::vector<uint2> mm(m);
   for (int64_t i = 0; i < m; ++i) {
     const uint32_t a = matches ? matches[2 * i] : static_cast<uint32_t>(i);
     const uint32_t b = matches ? matches[2 * i + 1] : static_cast<uint32_t>(i);
-    if (a >= n1 || b >= n2) return bad("[verify.cu] Check Failed: match index < number of points");
+    if (a >= n1 || b >= n2) return fail(ctx, B2M_EINVAL, "[verify.cu] Check Failed: match index < number of points");
     pts[i] = make_double4(points1[2 * a], points1[2 * a + 1], points2[2 * b], points2[2 * b + 1]);
     mm[i] = make_uint2(a, b);
   }
@@ -1872,13 +1822,13 @@ static int estimate_tvg_once(b2m_ctx* ctx, const b2m_camera* cam1, const double*
   double models[27];
   double h_pose[8] = {1, 0, 0, 0, 0, 0, 0, 0};
   int32_t h_pose_valid = 0;
-  V_TRY(ctx, cudaMemcpyAsync(i32, G.d_i32, sizeof(i32), cudaMemcpyDeviceToHost, ctx->stream));
-  V_TRY(ctx, cudaMemcpyAsync(models, G.d_models, sizeof(models), cudaMemcpyDeviceToHost, ctx->stream));
+  B2M_CUDA_TRY(ctx, cudaMemcpyAsync(i32, G.d_i32, sizeof(i32), cudaMemcpyDeviceToHost, ctx->stream));
+  B2M_CUDA_TRY(ctx, cudaMemcpyAsync(models, G.d_models, sizeof(models), cudaMemcpyDeviceToHost, ctx->stream));
   if (G.d_pose) {
-    V_TRY(ctx, cudaMemcpyAsync(h_pose, G.d_pose, sizeof(h_pose), cudaMemcpyDeviceToHost, ctx->stream));
-    V_TRY(ctx, cudaMemcpyAsync(&h_pose_valid, G.d_pose_valid, sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
+    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(h_pose, G.d_pose, sizeof(h_pose), cudaMemcpyDeviceToHost, ctx->stream));
+    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(&h_pose_valid, G.d_pose_valid, sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
   }
-  V_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+  B2M_CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
   memset(out, 0, sizeof(*out));
   out->struct_size = sizeof(*out);
   out->config = i32[9];
@@ -1889,7 +1839,7 @@ static int estimate_tvg_once(b2m_ctx* ctx, const b2m_camera* cam1, const double*
   memcpy(out->F, models + 9, sizeof(double) * 9);
   memcpy(out->H, models + 18, sizeof(double) * 9);
   if (out->n_inliers > 0 && inlier_matches) {
-    V_TRY(ctx, cudaMemcpy(inlier_matches, G.d_inliers, sizeof(uint2) * out->n_inliers, cudaMemcpyDeviceToHost));
+    B2M_CUDA_TRY(ctx, cudaMemcpy(inlier_matches, G.d_inliers, sizeof(uint2) * out->n_inliers, cudaMemcpyDeviceToHost));
   }
   return B2M_OK;
 }
@@ -1907,21 +1857,12 @@ int b2m_estimate_two_view_geometry(b2m_ctx* ctx, const b2m_camera* cam1, const d
   if (!ctx) return B2M_EINVAL;
   if (!opts || !opts->multiple_models)
     return estimate_tvg_once(ctx, cam1, points1, n1, cam2, points2, n2, matches, m, opts, out, inlier_matches);
-  if (!out) {
-    ctx->err = "[verify.cu] Check Failed: out != NULL";
-    return B2M_EINVAL;
-  }
+  if (!out) return fail(ctx, B2M_EINVAL, "[verify.cu] Check Failed: out != NULL");
   if (!matches) {
-    if (n1 != n2) {
-      ctx->err = "[verify.cu] Check Failed: points1.size() == points2.size()";
-      return B2M_EINVAL;
-    }
+    if (n1 != n2) return fail(ctx, B2M_EINVAL, "[verify.cu] Check Failed: points1.size() == points2.size()");
     m = n1;
   }
-  if (m < 0) {
-    ctx->err = "[verify.cu] Check Failed: m >= 0";
-    return B2M_EINVAL;
-  }
+  if (m < 0) return fail(ctx, B2M_EINVAL, "[verify.cu] Check Failed: m >= 0");
   std::vector<uint32_t> remaining(static_cast<size_t>(m) * 2);
   for (int64_t i = 0; i < m; ++i) {
     remaining[2 * i] = matches ? matches[2 * i] : static_cast<uint32_t>(i);
@@ -1985,23 +1926,19 @@ int b2m_estimate_two_view_geometry_batch(b2m_ctx* ctx, const b2m_tvg_problem* pr
                                          const b2m_tvg_opts* opts, b2m_tvg_result* out,
                                          uint32_t* const* inlier_matches) {
   if (!ctx) return B2M_EINVAL;
-  auto bad = [&](const char* msg) {
-    ctx->err = msg;
-    return B2M_EINVAL;
-  };
   if (n_problems < 0 || (n_problems > 0 && (!problems || !out)) || !opts)
-    return bad("[verify.cu] Check Failed: problems, options and out != NULL");
+    return fail(ctx, B2M_EINVAL, "[verify.cu] Check Failed: problems, options and out != NULL");
   if (opts->multiple_models)
-    return bad("[verify.cu] multiple_models: use b2m_estimate_two_view_geometry (the per-problem loop is sequential)");
+    return fail(ctx, B2M_EINVAL, "[verify.cu] multiple_models: use b2m_estimate_two_view_geometry (the per-problem loop is sequential)");
   for (int64_t k = 0; k < n_problems; ++k) {
     const b2m_tvg_problem& q = problems[k];
     if (q.n1 < 0 || q.n2 < 0 || (q.n1 > 0 && !q.points1) || (q.n2 > 0 && !q.points2))
-      return bad("[verify.cu] Check Failed: points");
-    if (!q.matches && q.n1 != q.n2) return bad("[verify.cu] Check Failed: points1.size() == points2.size()");
-    if (q.matches && q.m < 0) return bad("[verify.cu] Check Failed: m >= 0");
-    if ((q.matches ? q.m : q.n1) > INT32_MAX) return bad("[verify.cu] Check Failed: matches per problem < 2^31");
-    if (const char* why = camera_problem(q.cam1)) return bad(why);
-    if (const char* why = camera_problem(q.cam2)) return bad(why);
+      return fail(ctx, B2M_EINVAL, "[verify.cu] Check Failed: points");
+    if (!q.matches && q.n1 != q.n2) return fail(ctx, B2M_EINVAL, "[verify.cu] Check Failed: points1.size() == points2.size()");
+    if (q.matches && q.m < 0) return fail(ctx, B2M_EINVAL, "[verify.cu] Check Failed: m >= 0");
+    if ((q.matches ? q.m : q.n1) > INT32_MAX) return fail(ctx, B2M_EINVAL, "[verify.cu] Check Failed: matches per problem < 2^31");
+    if (const char* why = camera_problem(q.cam1)) return fail(ctx, B2M_EINVAL, why);
+    if (const char* why = camera_problem(q.cam2)) return fail(ctx, B2M_EINVAL, why);
   }
   cudaSetDevice(ctx->device);
   cudaStream_t st = ctx->stream;
@@ -2036,7 +1973,7 @@ int b2m_estimate_two_view_geometry_batch(b2m_ctx* ctx, const b2m_tvg_problem* pr
       for (int64_t i = 0; i < m; ++i) {
         const uint32_t a = q.matches ? q.matches[2 * i] : static_cast<uint32_t>(i);
         const uint32_t b = q.matches ? q.matches[2 * i + 1] : static_cast<uint32_t>(i);
-        if (a >= q.n1 || b >= q.n2) return bad("[verify.cu] Check Failed: match index < number of points");
+        if (a >= q.n1 || b >= q.n2) return fail(ctx, B2M_EINVAL, "[verify.cu] Check Failed: match index < number of points");
         pts.push_back(make_double4(q.points1[2 * a], q.points1[2 * a + 1], q.points2[2 * b], q.points2[2 * b + 1]));
         mm.push_back(make_uint2(a, b));
       }
@@ -2045,26 +1982,26 @@ int b2m_estimate_two_view_geometry_batch(b2m_ctx* ctx, const b2m_tvg_problem* pr
     const int64_t cap = std::max<int64_t>(total, 1);
     Single G;  // owns the arenas; the per-problem scalars live in one int32 block (see the offsets below)
     int32_t* d_i32 = nullptr;  // pairs[2nb] cnt[nb] sup[3nb] success[3nb] config[nb] inl_cnt[nb]
-    V_TRY(ctx, cudaMalloc(&G.d_pts, sizeof(double4) * cap));
-    V_TRY(ctx, cudaMalloc(&G.d_matches, sizeof(uint2) * cap));
-    V_TRY(ctx, cudaMalloc(&G.d_inliers, sizeof(uint2) * cap));
-    V_TRY(ctx, cudaMalloc(&G.d_mask, 3 * cap));
-    V_TRY(ctx, cudaMalloc(&G.d_cams, sizeof(DevCamera) * 2 * nb));
-    V_TRY(ctx, cudaMalloc(&G.d_i32, sizeof(int32_t) * 11 * nb));
-    V_TRY(ctx, cudaMalloc(&G.d_off, sizeof(int64_t) * nb));
-    V_TRY(ctx, cudaMalloc(&G.d_models, sizeof(double) * 27 * nb));
-    V_TRY(ctx, cudaMalloc(&G.d_e_scratch, sizeof(double) * kEStride * kRansacThreads * static_cast<size_t>(nb)));
+    B2M_CUDA_TRY(ctx, G.d_pts.ensure(cap));
+    B2M_CUDA_TRY(ctx, G.d_matches.ensure(cap));
+    B2M_CUDA_TRY(ctx, G.d_inliers.ensure(cap));
+    B2M_CUDA_TRY(ctx, G.d_mask.ensure(3 * cap));
+    B2M_CUDA_TRY(ctx, G.d_cams.ensure(2 * nb));
+    B2M_CUDA_TRY(ctx, G.d_i32.ensure(11 * nb));
+    B2M_CUDA_TRY(ctx, G.d_off.ensure(nb));
+    B2M_CUDA_TRY(ctx, G.d_models.ensure(27 * nb));
+    B2M_CUDA_TRY(ctx, G.d_e_scratch.ensure(static_cast<size_t>(kEStride) * kRansacThreads * nb));
     d_i32 = G.d_i32;
     if (total > 0) {
-      V_TRY(ctx, cudaMemcpyAsync(G.d_pts, pts.data(), sizeof(double4) * total, cudaMemcpyHostToDevice, st));
-      V_TRY(ctx, cudaMemcpyAsync(G.d_matches, mm.data(), sizeof(uint2) * total, cudaMemcpyHostToDevice, st));
+      B2M_CUDA_TRY(ctx, cudaMemcpyAsync(G.d_pts, pts.data(), sizeof(double4) * total, cudaMemcpyHostToDevice, st));
+      B2M_CUDA_TRY(ctx, cudaMemcpyAsync(G.d_matches, mm.data(), sizeof(uint2) * total, cudaMemcpyHostToDevice, st));
     }
-    V_TRY(ctx, cudaMemcpyAsync(G.d_cams, cams.data(), sizeof(DevCamera) * 2 * nb, cudaMemcpyHostToDevice, st));
-    V_TRY(ctx, cudaMemsetAsync(d_i32, 0, sizeof(int32_t) * 11 * nb, st));
-    V_TRY(ctx, cudaMemcpyAsync(d_i32, pairs.data(), sizeof(int32_t) * 2 * nb, cudaMemcpyHostToDevice, st));
-    V_TRY(ctx, cudaMemcpyAsync(d_i32 + 2 * nb, cnt.data(), sizeof(int32_t) * nb, cudaMemcpyHostToDevice, st));
-    V_TRY(ctx, cudaMemcpyAsync(G.d_off, off.data(), sizeof(int64_t) * nb, cudaMemcpyHostToDevice, st));
-    V_TRY(ctx, cudaMemsetAsync(G.d_models, 0, sizeof(double) * 27 * nb, st));
+    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(G.d_cams, cams.data(), sizeof(DevCamera) * 2 * nb, cudaMemcpyHostToDevice, st));
+    B2M_CUDA_TRY(ctx, cudaMemsetAsync(d_i32, 0, sizeof(int32_t) * 11 * nb, st));
+    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(d_i32, pairs.data(), sizeof(int32_t) * 2 * nb, cudaMemcpyHostToDevice, st));
+    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(d_i32 + 2 * nb, cnt.data(), sizeof(int32_t) * nb, cudaMemcpyHostToDevice, st));
+    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(G.d_off, off.data(), sizeof(int64_t) * nb, cudaMemcpyHostToDevice, st));
+    B2M_CUDA_TRY(ctx, cudaMemsetAsync(G.d_models, 0, sizeof(double) * 27 * nb, st));
     VerifyParams P = VerifyParams{};
     P.pairs = d_i32;
     P.pair_cnt = d_i32 + 2 * nb;
@@ -2083,14 +2020,14 @@ int b2m_estimate_two_view_geometry_batch(b2m_ctx* ctx, const b2m_tvg_problem* pr
     P.opt = *opts;
     P.seed = ctx->seed;
     P.single_kind = -1;
-    P.counters = verify_counters(ctx);
+    P.counters = ctx->d_counters + kVerifyCounters;
       P.e_scratch = G.d_e_scratch;
     P.lo_eig_thread = lo_eig_thread_mode();
     const double4* pts_E = nullptr;
     if (int rc = undistort_for_E(ctx, G, P, full_cams.data(), 2 * nb, nb, cap, st, &pts_E)) return rc;
-    V_TRY(ctx, launch_ransac(P, nb, st, nullptr, pts_E));
+    B2M_CUDA_TRY(ctx, launch_ransac(P, nb, st, nullptr, pts_E));
     b2m_decide_kernel<<<nb, 256, 0, st>>>(P);
-    V_TRY(ctx, cudaGetLastError());
+    B2M_CUDA_TRY(ctx, cudaGetLastError());
     ctx->stats.kernel_launches += 4;
     if (opts->compute_relative_pose)
       if (int rc = launch_pose_standalone(ctx, G, P, nb, cap, raw1, raw2, raw1_off, raw2_off, full_cams.data(), 2 * nb, st))
@@ -2098,17 +2035,17 @@ int b2m_estimate_two_view_geometry_batch(b2m_ctx* ctx, const b2m_tvg_problem* pr
     std::vector<double> h_pose(static_cast<size_t>(8) * nb, 0.0);
     std::vector<int32_t> h_pose_valid(nb, 0);
     if (G.d_pose) {
-      V_TRY(ctx, cudaMemcpyAsync(h_pose.data(), G.d_pose, sizeof(double) * 8 * nb, cudaMemcpyDeviceToHost, st));
-      V_TRY(ctx, cudaMemcpyAsync(h_pose_valid.data(), G.d_pose_valid, sizeof(int32_t) * nb, cudaMemcpyDeviceToHost, st));
+      B2M_CUDA_TRY(ctx, cudaMemcpyAsync(h_pose.data(), G.d_pose, sizeof(double) * 8 * nb, cudaMemcpyDeviceToHost, st));
+      B2M_CUDA_TRY(ctx, cudaMemcpyAsync(h_pose_valid.data(), G.d_pose_valid, sizeof(int32_t) * nb, cudaMemcpyDeviceToHost, st));
     }
     std::vector<int32_t> h_i32(static_cast<size_t>(11) * nb);
     std::vector<double> h_models(static_cast<size_t>(27) * nb);
     std::vector<uint2> h_inl(static_cast<size_t>(cap));
-    V_TRY(ctx, cudaMemcpyAsync(h_i32.data(), d_i32, sizeof(int32_t) * 11 * nb, cudaMemcpyDeviceToHost, st));
-    V_TRY(ctx, cudaMemcpyAsync(h_models.data(), G.d_models, sizeof(double) * 27 * nb, cudaMemcpyDeviceToHost, st));
+    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(h_i32.data(), d_i32, sizeof(int32_t) * 11 * nb, cudaMemcpyDeviceToHost, st));
+    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(h_models.data(), G.d_models, sizeof(double) * 27 * nb, cudaMemcpyDeviceToHost, st));
     if (total > 0 && inlier_matches)
-      V_TRY(ctx, cudaMemcpyAsync(h_inl.data(), G.d_inliers, sizeof(uint2) * total, cudaMemcpyDeviceToHost, st));
-    V_TRY(ctx, cudaStreamSynchronize(st));
+      B2M_CUDA_TRY(ctx, cudaMemcpyAsync(h_inl.data(), G.d_inliers, sizeof(uint2) * total, cudaMemcpyDeviceToHost, st));
+    B2M_CUDA_TRY(ctx, cudaStreamSynchronize(st));
     for (int k = 0; k < nb; ++k) {
       b2m_tvg_result& r = out[k0 + k];
       memset(&r, 0, sizeof(r));
@@ -2133,13 +2070,9 @@ int b2m_ransac_model(b2m_ctx* ctx, int32_t kind, const double* points1, const do
                      const b2m_ransac_opts* opts, double* out_model, uint8_t* inlier_mask, int64_t* num_inliers,
                      int32_t* success) {
   if (!ctx) return B2M_EINVAL;
-  auto bad = [&](const char* msg) {
-    ctx->err = msg;
-    return B2M_EINVAL;
-  };
-  if (kind < 0 || kind > 2) return bad("[verify.cu] Check Failed: kind in {0 (E), 1 (F), 2 (H)}");
-  if (!opts || !out_model || !num_inliers || !success) return bad("[verify.cu] Check Failed: outputs != NULL");
-  if (m < 0 || (m > 0 && (!points1 || !points2))) return bad("[verify.cu] Check Failed: points");
+  if (kind < 0 || kind > 2) return fail(ctx, B2M_EINVAL, "[verify.cu] Check Failed: kind in {0 (E), 1 (F), 2 (H)}");
+  if (!opts || !out_model || !num_inliers || !success) return fail(ctx, B2M_EINVAL, "[verify.cu] Check Failed: outputs != NULL");
+  if (m < 0 || (m > 0 && (!points1 || !points2))) return fail(ctx, B2M_EINVAL, "[verify.cu] Check Failed: points");
   cudaSetDevice(ctx->device);
   std::vector<double4> pts(m);
   std::vector<uint2> mm(m);
@@ -2159,12 +2092,12 @@ int b2m_ransac_model(b2m_ctx* ctx, int32_t kind, const double* points1, const do
   if (int rc = run_single(ctx, pts, mm, cams, t, kind, G, P)) return rc;
   int32_t i32[16];
   double models[27];
-  V_TRY(ctx, cudaMemcpyAsync(i32, G.d_i32, sizeof(i32), cudaMemcpyDeviceToHost, ctx->stream));
-  V_TRY(ctx, cudaMemcpyAsync(models, G.d_models, sizeof(models), cudaMemcpyDeviceToHost, ctx->stream));
+  B2M_CUDA_TRY(ctx, cudaMemcpyAsync(i32, G.d_i32, sizeof(i32), cudaMemcpyDeviceToHost, ctx->stream));
+  B2M_CUDA_TRY(ctx, cudaMemcpyAsync(models, G.d_models, sizeof(models), cudaMemcpyDeviceToHost, ctx->stream));
   if (m > 0 && inlier_mask)
-    V_TRY(ctx, cudaMemcpyAsync(inlier_mask, G.d_mask + static_cast<int64_t>(kind) * P.arena_cap, m,
+    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(inlier_mask, G.d_mask + static_cast<int64_t>(kind) * P.arena_cap, m,
                                cudaMemcpyDeviceToHost, ctx->stream));
-  V_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+  B2M_CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
   *num_inliers = i32[3 + kind];
   *success = i32[6 + kind];
   memcpy(out_model, models + 9 * kind, sizeof(double) * 9);
@@ -2178,19 +2111,15 @@ int b2m_estimate_two_view_geometry_pose(b2m_ctx* ctx, const b2m_camera* cam1, co
                                         const b2m_camera* cam2, const double* points2, int64_t n2,
                                         const uint32_t* inlier_matches, int64_t n_inliers, b2m_tvg_result* geometry) {
   if (!ctx) return B2M_EINVAL;
-  auto bad = [&](const char* msg) {
-    ctx->err = msg;
-    return B2M_EINVAL;
-  };
-  if (!cam1 || !cam2 || !geometry) return bad("[verify.cu] Check Failed: cameras and geometry != NULL");
-  if (const char* why = camera_problem(*cam1)) return bad(why);
-  if (const char* why = camera_problem(*cam2)) return bad(why);
-  if (n1 < 0 || n2 < 0 || (n1 > 0 && !points1) || (n2 > 0 && !points2)) return bad("[verify.cu] Check Failed: points");
+  if (!cam1 || !cam2 || !geometry) return fail(ctx, B2M_EINVAL, "[verify.cu] Check Failed: cameras and geometry != NULL");
+  if (const char* why = camera_problem(*cam1)) return fail(ctx, B2M_EINVAL, why);
+  if (const char* why = camera_problem(*cam2)) return fail(ctx, B2M_EINVAL, why);
+  if (n1 < 0 || n2 < 0 || (n1 > 0 && !points1) || (n2 > 0 && !points2)) return fail(ctx, B2M_EINVAL, "[verify.cu] Check Failed: points");
   if (n_inliers < 0 || n_inliers > INT32_MAX || (n_inliers > 0 && !inlier_matches))
-    return bad("[verify.cu] Check Failed: inlier_matches");
+    return fail(ctx, B2M_EINVAL, "[verify.cu] Check Failed: inlier_matches");
   for (int64_t i = 0; i < n_inliers; ++i)
     if (inlier_matches[2 * i] >= n1 || inlier_matches[2 * i + 1] >= n2)
-      return bad("[verify.cu] Check Failed: match index < number of points");
+      return fail(ctx, B2M_EINVAL, "[verify.cu] Check Failed: match index < number of points");
   cudaSetDevice(ctx->device);
   cudaStream_t st = ctx->stream;
   Single G;
@@ -2202,17 +2131,17 @@ int b2m_estimate_two_view_geometry_pose(b2m_ctx* ctx, const b2m_camera* cam1, co
   memset(models, 0, sizeof(models));
   memcpy(models, geometry->E, sizeof(double) * 9);
   memcpy(models + 18, geometry->H, sizeof(double) * 9);
-  V_TRY(ctx, cudaMalloc(&G.d_inliers, sizeof(uint2) * cap));
-  V_TRY(ctx, cudaMalloc(&G.d_cams, sizeof(DevCamera) * 2));
-  V_TRY(ctx, cudaMalloc(&G.d_i32, sizeof(i32)));
-  V_TRY(ctx, cudaMalloc(&G.d_off, sizeof(int64_t)));
-  V_TRY(ctx, cudaMalloc(&G.d_models, sizeof(models)));
+  B2M_CUDA_TRY(ctx, G.d_inliers.ensure(cap));
+  B2M_CUDA_TRY(ctx, G.d_cams.ensure(2));
+  B2M_CUDA_TRY(ctx, G.d_i32.ensure(4));
+  B2M_CUDA_TRY(ctx, G.d_off.ensure(1));
+  B2M_CUDA_TRY(ctx, G.d_models.ensure(27));
   if (n_inliers > 0)
-    V_TRY(ctx, cudaMemcpy(G.d_inliers, inlier_matches, sizeof(uint2) * n_inliers, cudaMemcpyHostToDevice));
-  V_TRY(ctx, cudaMemcpy(G.d_cams, cams, sizeof(cams), cudaMemcpyHostToDevice));
-  V_TRY(ctx, cudaMemcpy(G.d_i32, i32, sizeof(i32), cudaMemcpyHostToDevice));
-  V_TRY(ctx, cudaMemcpy(G.d_off, &off0, sizeof(int64_t), cudaMemcpyHostToDevice));
-  V_TRY(ctx, cudaMemcpy(G.d_models, models, sizeof(models), cudaMemcpyHostToDevice));
+    B2M_CUDA_TRY(ctx, cudaMemcpy(G.d_inliers, inlier_matches, sizeof(uint2) * n_inliers, cudaMemcpyHostToDevice));
+  B2M_CUDA_TRY(ctx, cudaMemcpy(G.d_cams, cams, sizeof(cams), cudaMemcpyHostToDevice));
+  B2M_CUDA_TRY(ctx, cudaMemcpy(G.d_i32, i32, sizeof(i32), cudaMemcpyHostToDevice));
+  B2M_CUDA_TRY(ctx, cudaMemcpy(G.d_off, &off0, sizeof(int64_t), cudaMemcpyHostToDevice));
+  B2M_CUDA_TRY(ctx, cudaMemcpy(G.d_models, models, sizeof(models), cudaMemcpyHostToDevice));
   VerifyParams P = VerifyParams{};
   P.pairs = G.d_i32;
   P.inl_cnt = G.d_i32 + 2;
@@ -2227,10 +2156,10 @@ int b2m_estimate_two_view_geometry_pose(b2m_ctx* ctx, const b2m_camera* cam1, co
   if (int rc = launch_pose_standalone(ctx, G, P, 1, cap, p1, p2, zero, zero, full_cams, 2, st)) return rc;
   double h_pose[8];
   int32_t h_valid = 0, h_i32[4];
-  V_TRY(ctx, cudaMemcpyAsync(h_pose, G.d_pose, sizeof(h_pose), cudaMemcpyDeviceToHost, st));
-  V_TRY(ctx, cudaMemcpyAsync(&h_valid, G.d_pose_valid, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-  V_TRY(ctx, cudaMemcpyAsync(h_i32, G.d_i32, sizeof(h_i32), cudaMemcpyDeviceToHost, st));
-  V_TRY(ctx, cudaStreamSynchronize(st));
+  B2M_CUDA_TRY(ctx, cudaMemcpyAsync(h_pose, G.d_pose, sizeof(h_pose), cudaMemcpyDeviceToHost, st));
+  B2M_CUDA_TRY(ctx, cudaMemcpyAsync(&h_valid, G.d_pose_valid, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  B2M_CUDA_TRY(ctx, cudaMemcpyAsync(h_i32, G.d_i32, sizeof(h_i32), cudaMemcpyDeviceToHost, st));
+  B2M_CUDA_TRY(ctx, cudaStreamSynchronize(st));
   geometry->qvec[0] = 1.0;
   geometry->qvec[1] = geometry->qvec[2] = geometry->qvec[3] = 0.0;
   geometry->tvec[0] = geometry->tvec[1] = geometry->tvec[2] = 0.0;
@@ -2248,106 +2177,67 @@ int b2m_estimate_two_view_geometry_pose(b2m_ctx* ctx, const b2m_camera* cam1, co
 
 int b2m_debug_five_point(b2m_ctx* ctx, const double* nullspaces, int64_t n, double* models, int32_t* n_models) {
   if (!ctx) return B2M_EINVAL;
-  if (n < 0 || (n > 0 && (!nullspaces || !models || !n_models))) {
-    ctx->err = "[verify.cu] Check Failed: nullspaces, models, n_models != NULL";
-    return B2M_EINVAL;
-  }
+  if (n < 0 || (n > 0 && (!nullspaces || !models || !n_models)))
+    return fail(ctx, B2M_EINVAL, "[verify.cu] Check Failed: nullspaces, models, n_models != NULL");
   if (n == 0) return B2M_OK;
   cudaSetDevice(ctx->device);
-  double *d_n = nullptr, *d_m = nullptr;
-  int32_t* d_c = nullptr;
-  auto cleanup = [&]() {
-    cudaFree(d_n); cudaFree(d_m); cudaFree(d_c);
-  };
-  if (cudaMalloc(&d_n, sizeof(double) * 36 * n) != cudaSuccess || cudaMalloc(&d_m, sizeof(double) * 90 * n) != cudaSuccess ||
-      cudaMalloc(&d_c, sizeof(int32_t) * n) != cudaSuccess) {
-    cleanup();
-    ctx->err = "[verify.cu] cudaMalloc failed";
-    return B2M_ENOMEM;
-  }
+  DeviceArray<double> d_n, d_m;
+  DeviceArray<int32_t> d_c;
+  B2M_CUDA_TRY(ctx, d_n.ensure(36 * n));
+  B2M_CUDA_TRY(ctx, d_m.ensure(90 * n));
+  B2M_CUDA_TRY(ctx, d_c.ensure(n));
   cudaMemcpyAsync(d_n, nullspaces, sizeof(double) * 36 * n, cudaMemcpyHostToDevice, ctx->stream);
   cudaMemsetAsync(d_m, 0, sizeof(double) * 90 * n, ctx->stream);
   b2m_five_point_kernel<<<static_cast<unsigned>((n + 3) / 4), 128, 0, ctx->stream>>>(d_n, n, d_m, d_c);
   ctx->stats.kernel_launches += 1;
   cudaMemcpyAsync(models, d_m, sizeof(double) * 90 * n, cudaMemcpyDeviceToHost, ctx->stream);
   cudaMemcpyAsync(n_models, d_c, sizeof(int32_t) * n, cudaMemcpyDeviceToHost, ctx->stream);
-  int rc = B2M_OK;
-  if (cudaStreamSynchronize(ctx->stream) != cudaSuccess) {
-    ctx->err = std::string("[verify.cu] CUDA error: ") + cudaGetErrorString(cudaGetLastError());
-    rc = B2M_ECUDA;
-  }
-  cleanup();
-  return rc;
+  B2M_CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+  return B2M_OK;
 }
 
 int b2m_cam_from_img(b2m_ctx* ctx, const b2m_camera* camera, const double* points, int64_t n, double* out) {
   if (!ctx) return B2M_EINVAL;
-  auto bad = [&](const char* msg) {
-    ctx->err = msg;
-    return B2M_EINVAL;
-  };
-  if (!camera || n < 0 || (n > 0 && (!points || !out))) return bad("[verify.cu] Check Failed: camera, points, out != NULL");
-  if (const char* why = camera_problem(*camera)) return bad(why);
+  if (!camera || n < 0 || (n > 0 && (!points || !out)))
+    return fail(ctx, B2M_EINVAL, "[verify.cu] Check Failed: camera, points, out != NULL");
+  if (const char* why = camera_problem(*camera)) return fail(ctx, B2M_EINVAL, why);
   if (n == 0) return B2M_OK;
   cudaSetDevice(ctx->device);
   const DevDistortion hd = to_dist(*camera);
-  DevDistortion* dc = nullptr;
-  double *dp = nullptr, *dout = nullptr;
-  auto cleanup = [&]() {
-    cudaFree(dc); cudaFree(dp); cudaFree(dout);
-  };
-  if (cudaMalloc(&dc, sizeof(DevDistortion)) != cudaSuccess || cudaMalloc(&dp, sizeof(double) * 2 * n) != cudaSuccess ||
-      cudaMalloc(&dout, sizeof(double) * 2 * n) != cudaSuccess) {
-    cleanup();
-    ctx->err = "[verify.cu] cudaMalloc failed";
-    return B2M_ENOMEM;
-  }
+  DeviceArray<DevDistortion> dc;
+  DeviceArray<double> dp, dout;
+  B2M_CUDA_TRY(ctx, dc.ensure(1));
+  B2M_CUDA_TRY(ctx, dp.ensure(2 * n));
+  B2M_CUDA_TRY(ctx, dout.ensure(2 * n));
   cudaMemcpyAsync(dc, &hd, sizeof(hd), cudaMemcpyHostToDevice, ctx->stream);
   cudaMemcpyAsync(dp, points, sizeof(double) * 2 * n, cudaMemcpyHostToDevice, ctx->stream);
   b2m_cam_from_img_kernel<<<static_cast<unsigned>((n + 127) / 128), 128, 0, ctx->stream>>>(dc, dp, n, dout);
   ctx->stats.kernel_launches += 1;
   cudaMemcpyAsync(out, dout, sizeof(double) * 2 * n, cudaMemcpyDeviceToHost, ctx->stream);
-  int rc = B2M_OK;
-  if (cudaStreamSynchronize(ctx->stream) != cudaSuccess) {
-    ctx->err = std::string("[verify.cu] CUDA error: ") + cudaGetErrorString(cudaGetLastError());
-    rc = B2M_ECUDA;
-  }
-  cleanup();
-  return rc;
+  B2M_CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+  return B2M_OK;
 }
 
 int b2m_squared_sampson_error(b2m_ctx* ctx, const double* points1, const double* points2, int64_t m, const double* E,
                               double* out_residuals) {
   if (!ctx) return B2M_EINVAL;
-  if (m < 0 || (m > 0 && (!points1 || !points2 || !out_residuals)) || !E) {
-    ctx->err = "[verify.cu] Check Failed: points, E, out != NULL";
-    return B2M_EINVAL;
-  }
+  if (m < 0 || (m > 0 && (!points1 || !points2 || !out_residuals)) || !E)
+    return fail(ctx, B2M_EINVAL, "[verify.cu] Check Failed: points, E, out != NULL");
   if (m == 0) return B2M_OK;
   cudaSetDevice(ctx->device);
-  double *d1 = nullptr, *d2 = nullptr, *dE = nullptr, *dout = nullptr;
-  int rc = B2M_OK;
-  auto cleanup = [&]() {
-    cudaFree(d1); cudaFree(d2); cudaFree(dE); cudaFree(dout);
-  };
-  if (cudaMalloc(&d1, sizeof(double) * 2 * m) != cudaSuccess || cudaMalloc(&d2, sizeof(double) * 2 * m) != cudaSuccess ||
-      cudaMalloc(&dE, sizeof(double) * 9) != cudaSuccess || cudaMalloc(&dout, sizeof(double) * m) != cudaSuccess) {
-    cleanup();
-    ctx->err = "[verify.cu] cudaMalloc failed";
-    return B2M_ENOMEM;
-  }
+  DeviceArray<double> d1, d2, dE, dout;
+  B2M_CUDA_TRY(ctx, d1.ensure(2 * m));
+  B2M_CUDA_TRY(ctx, d2.ensure(2 * m));
+  B2M_CUDA_TRY(ctx, dE.ensure(9));
+  B2M_CUDA_TRY(ctx, dout.ensure(m));
   cudaMemcpyAsync(d1, points1, sizeof(double) * 2 * m, cudaMemcpyHostToDevice, ctx->stream);
   cudaMemcpyAsync(d2, points2, sizeof(double) * 2 * m, cudaMemcpyHostToDevice, ctx->stream);
   cudaMemcpyAsync(dE, E, sizeof(double) * 9, cudaMemcpyHostToDevice, ctx->stream);
   b2m_sampson_kernel<<<static_cast<unsigned>((m + 255) / 256), 256, 0, ctx->stream>>>(d1, d2, m, dE, dout);
   ctx->stats.kernel_launches += 1;
   cudaMemcpyAsync(out_residuals, dout, sizeof(double) * m, cudaMemcpyDeviceToHost, ctx->stream);
-  if (cudaStreamSynchronize(ctx->stream) != cudaSuccess) {
-    ctx->err = std::string("[verify.cu] CUDA error: ") + cudaGetErrorString(cudaGetLastError());
-    rc = B2M_ECUDA;
-  }
-  cleanup();
-  return rc;
+  B2M_CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+  return B2M_OK;
 }
 
 }  // extern "C"
