@@ -11,8 +11,9 @@
 //                          with the scaled camera, then runs LO-RANSAC: a round is up to 128 P3P hypotheses (thread =
 //                          hypothesis, <= 4 models each), scored by the whole CTA with the division-free fp32 test
 //                          (u Z - X)^2 + (v Z - Y)^2 <= thr Z^2, Z > 0, borderline points re-decided in fp64, and the
-//                          exact pruning of verify.cu; a new best goes through EPnP refits on its inliers (moments
-//                          reduced by the CTA, the 12 x 12 eigenproblem on one warp, the beta solve on one thread).
+//                          exact pruning (the round of ransac_common.cuh); a new best goes through EPnP refits on its
+//                          inliers (moments reduced by the CTA, the 12 x 12 eigenproblem on one warp, the beta solve on
+//                          one thread).
 //   b2m_abs_select_kernel  one warp per problem: the focal sample with strictly the most inliers (earliest on ties),
 //                          its inlier mask, the pose in world coordinates and the camera parameters.
 //   b2m_abs_refine_kernel  one warp per problem: LM on 6 + k unknowns (k <= 10 camera parameters), exact Jacobians from
@@ -104,8 +105,6 @@ namespace {
 
 using namespace geom;
 
-constexpr int kThreads = 128;
-constexpr int kChunkModels = 256;
 constexpr int kMaxLocalTrials = 10;
 constexpr int kMaxRefine = 16;   // 6 pose + up to 10 camera parameters
 constexpr double kDblEps = 2.220446049250313e-16;
@@ -140,12 +139,7 @@ struct RansacParams {
 };
 
 struct Shared {
-  double chunk_d[kChunkModels][12];
-  float chunk_f[kChunkModels][12];
-  int chunk_cnt[kChunkModels];
-  int scan[kThreads];
-  int cnt_arr[kThreads];
-  double sum_arr[kThreads];
+  RoundShared<12> round;
   double best_model[12];
   double cand[3][12];
   double red[4][40];
@@ -158,9 +152,6 @@ struct Shared {
   double cand_err[3];
   double best_sum;
   int best_cnt;
-  int winner;
-  int improved;
-  int round_max;
   int n_cand;
   int first;
   int lo_ok;
@@ -198,6 +189,32 @@ __device__ __forceinline__ int inlier_f32(const float* M, float u, float v, floa
   const float ex = fmaf(u, zc, -xc), ey = fmaf(v, zc, -yc);
   return classify_f32(fmaf(ex, ex, ey * ey), thr * zc * zc);
 }
+
+// A problem's correspondences and poses in the shared LO-RANSAC round (ransac_common.cuh).
+struct ReprojModel {
+  static constexpr int kD = 12;
+  struct Pt {
+    float u, v, X, Y, Z;
+  };
+  const RansacParams& P;
+  const double2* xn;
+  int64_t off;
+  const double* c;
+  // a slot past the end is a point behind the camera (Z = -1)
+  __device__ __forceinline__ Pt load_f32(int i, bool live) const {
+    double u = 0, v = 0, X = 0, Y = 0, Z = -1;
+    if (live) load_point(P, xn, off, i, c, u, v, X, Y, Z);
+    return {static_cast<float>(u), static_cast<float>(v), static_cast<float>(X), static_cast<float>(Y), static_cast<float>(Z)};
+  }
+  __device__ __forceinline__ int test(const float* M, const Pt& p, float thr) const {
+    return inlier_f32(M, p.u, p.v, p.X, p.Y, p.Z, thr);
+  }
+  __device__ __forceinline__ double residual(const double* M, int i) const {
+    double u, v, X, Y, Z;
+    load_point(P, xn, off, i, c, u, v, X, Y, Z);
+    return reproj_sq(M, u, v, X, Y, Z);
+  }
+};
 
 __device__ void frame3(const double* a, const double* b, const double* c, double* F /* columns e1 e2 e3 */) {
   double e1[3] = {b[0] - a[0], b[1] - a[1], b[2] - a[2]}, d2[3] = {c[0] - a[0], c[1] - a[1], c[2] - a[2]}, e3[3], e2[3];
@@ -409,80 +426,6 @@ __device__ void epnp_candidates(const double (*V)[12], const double (*cw)[3], do
   }
 }
 
-// Scores a chunk of models over one block of points held in registers (fp32, fp64 for borderline points).
-template <int PPT>
-__device__ __forceinline__ void score_block(Shared& sh, const RansacParams& P, const double2* xn, int64_t off,
-                                            const double* c, int n, int pb, int n_chunk, double thr, float thr_f, int tid,
-                                            int need) {
-  float pu[PPT], pv[PPT], pX[PPT], pY[PPT], pZ[PPT];
-  int live[PPT];
-#pragma unroll
-  for (int q = 0; q < PPT; ++q) {
-    const int i = pb + q * kThreads + tid;
-    double u = 0, v = 0, X = 0, Y = 0, Z = -1;
-    live[q] = i < n ? 1 : 0;
-    if (i < n) load_point(P, xn, off, i, c, u, v, X, Y, Z);
-    pu[q] = static_cast<float>(u); pv[q] = static_cast<float>(v);
-    pX[q] = static_cast<float>(X); pY[q] = static_cast<float>(Y); pZ[q] = static_cast<float>(Z);
-  }
-  for (int m = 0; m < n_chunk; ++m) {
-    if (sh.chunk_cnt[m] < need) continue;  // exact pruning (uniform across the CTA), see verify.cu score_block
-    float Mf[12];
-    const float4* mp = reinterpret_cast<const float4*>(sh.chunk_f[m]);
-    const float4 m0 = mp[0], m1 = mp[1], m2 = mp[2];
-    Mf[0] = m0.x; Mf[1] = m0.y; Mf[2] = m0.z; Mf[3] = m0.w;
-    Mf[4] = m1.x; Mf[5] = m1.y; Mf[6] = m1.z; Mf[7] = m1.w;
-    Mf[8] = m2.x; Mf[9] = m2.y; Mf[10] = m2.z; Mf[11] = m2.w;
-    int cnt = 0, flags = 0;
-#pragma unroll
-    for (int q = 0; q < PPT; ++q) {
-      const int f = inlier_f32(Mf, pu[q], pv[q], pX[q], pY[q], pZ[q], thr_f);
-      cnt += f & live[q];
-      flags |= f & (live[q] << 1);
-    }
-    if (flags & 2) {
-      cnt = 0;
-      for (int q = 0; q < PPT; ++q) {
-        const int i = pb + q * kThreads + tid;
-        if (i < n) {
-          double u, v, X, Y, Z;
-          load_point(P, xn, off, i, c, u, v, X, Y, Z);
-          cnt += reproj_sq(sh.chunk_d[m], u, v, X, Y, Z) <= thr ? 1 : 0;
-        }
-      }
-    }
-    if (cnt) atomicAdd(&sh.chunk_cnt[m], cnt);
-  }
-}
-
-// exact fp64 support (count, residual sum) of `M` over all points, CTA-wide; every thread gets the totals
-__device__ void support(Shared& sh, const RansacParams& P, const double2* xn, int64_t off, const double* c, int n,
-                        const double* M, double thr, int& cnt, double& sum) {
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  int cl = 0;
-  double sl = 0.0;
-  for (int i = tid; i < n; i += kThreads) {
-    double u, v, X, Y, Z;
-    load_point(P, xn, off, i, c, u, v, X, Y, Z);
-    const double r = reproj_sq(M, u, v, X, Y, Z);
-    if (r <= thr) {
-      ++cl;
-      sl += r;
-    }
-  }
-  cl = __reduce_add_sync(0xffffffffu, cl);
-  sl = warp_sum_d(sl);
-  __syncthreads();
-  if (lane == 0) {
-    sh.scan[warp] = cl;
-    sh.sum_arr[warp] = sl;
-  }
-  __syncthreads();
-  cnt = sh.scan[0] + sh.scan[1] + sh.scan[2] + sh.scan[3];
-  sum = sh.sum_arr[0] + sh.sum_arr[1] + sh.sum_arr[2] + sh.sum_arr[3];
-  __syncthreads();
-}
-
 // One EPnP refit on the inliers of sh.best_model (EPNPEstimator as the local estimator of LORANSAC).  Returns the
 // candidate (the one of the three beta approximations with the least total reprojection error on the inliers) in
 // sh.cand[0] and 1, or 0 when EPnP returns no model.
@@ -493,7 +436,7 @@ __device__ int epnp_refit(Shared& sh, const RansacParams& P, const double2* xn, 
   // pass 1: moments of the inlier world points, first inlier
   double mo[10] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
   int first = INT32_MAX;
-  for (int i = tid; i < n; i += kThreads) {
+  for (int i = tid; i < n; i += kRansacThreads) {
     double u, v, X, Y, Z;
     load_point(P, xn, off, i, c, u, v, X, Y, Z);
     if (reproj_sq(M, u, v, X, Y, Z) <= thr) {
@@ -507,11 +450,11 @@ __device__ int epnp_refit(Shared& sh, const RansacParams& P, const double2* xn, 
     const double s = warp_sum_d(mo[k]);
     if (lane == 0) sh.red[warp][k] = s;
   }
-  if (lane == 0) sh.scan[warp] = first;
+  if (lane == 0) sh.round.scan[warp] = first;
   __syncthreads();
   if (tid == 0) {
     for (int k = 0; k < 10; ++k) sh.mom[k] = sh.red[0][k] + sh.red[1][k] + sh.red[2][k] + sh.red[3][k];
-    sh.first = min(min(sh.scan[0], sh.scan[1]), min(sh.scan[2], sh.scan[3]));
+    sh.first = min(min(sh.round.scan[0], sh.round.scan[1]), min(sh.round.scan[2], sh.round.scan[3]));
     const double nn = sh.mom[0];
     const double c0[3] = {sh.mom[1] / nn, sh.mom[2] / nn, sh.mom[3] / nn};
     double A[9] = {sh.mom[4] - nn * c0[0] * c0[0], sh.mom[5] - nn * c0[0] * c0[1], sh.mom[6] - nn * c0[0] * c0[2], 0, 0, 0, 0, 0, 0};
@@ -560,7 +503,7 @@ __device__ int epnp_refit(Shared& sh, const RansacParams& P, const double2* xn, 
   double Ci[9], c0[3];
   for (int k = 0; k < 9; ++k) Ci[k] = sh.ccinv[k];
   for (int k = 0; k < 3; ++k) c0[k] = sh.cw[0][k];
-  for (int i = tid; i < n; i += kThreads) {
+  for (int i = tid; i < n; i += kRansacThreads) {
     double u, v, X, Y, Z;
     load_point(P, xn, off, i, c, u, v, X, Y, Z);
     if (reproj_sq(M, u, v, X, Y, Z) <= thr) {
@@ -645,7 +588,7 @@ __device__ int epnp_refit(Shared& sh, const RansacParams& P, const double2* xn, 
   __syncthreads();
   // pass 3: total reprojection error (sum of sqrt) of the three candidates on the inlier set
   double e3[3] = {0, 0, 0};
-  for (int i = tid; i < n; i += kThreads) {
+  for (int i = tid; i < n; i += kRansacThreads) {
     double u, v, X, Y, Z;
     load_point(P, xn, off, i, c, u, v, X, Y, Z);
     if (reproj_sq(M, u, v, X, Y, Z) <= thr)
@@ -676,7 +619,7 @@ __device__ int epnp_refit(Shared& sh, const RansacParams& P, const double2* xn, 
   return sh.n_cand;
 }
 
-__global__ void __launch_bounds__(kThreads, 3) b2m_abs_ransac_kernel(const RansacParams P) {
+__global__ void __launch_bounds__(kRansacThreads, 3) b2m_abs_ransac_kernel(const RansacParams P) {
   __shared__ Shared sh;
   const int tid = threadIdx.x;
   const int cta = blockIdx.x;
@@ -689,18 +632,17 @@ __global__ void __launch_bounds__(kThreads, 3) b2m_abs_ransac_kernel(const Ransa
   const double fac = P.factors[fs];
   cm.p[0] *= fac;
   if (!cam::single_focal(cm.model)) cm.p[1] *= fac;
-  for (int i = tid; i < n; i += kThreads) {
+  for (int i = tid; i < n; i += kRansacThreads) {
     double u, v;
     cam::cam_from_img(cm.model, cm.p, P.px[2 * (off + i)], P.px[2 * (off + i) + 1], &u, &v);
     xn[i] = make_double2(u, v);
   }
   const double e = P.ro.max_error / cam::mean_focal_length(cm.model, cm.p);  // CamFromImgThreshold
   const double thr = e * e;
-  const float thr_f = static_cast<float>(thr);
   const double c[3] = {P.centroid[3 * prob], P.centroid[3 * prob + 1], P.centroid[3 * prob + 2]};
   __syncthreads();
   if (n < 3) {
-    for (int i = tid; i < n; i += kThreads) mask[i] = 0;
+    for (int i = tid; i < n; i += kRansacThreads) mask[i] = 0;
     if (tid == 0) {
       P.sup[cta] = 0;
       P.success[cta] = 0;
@@ -711,9 +653,8 @@ __global__ void __launch_bounds__(kThreads, 3) b2m_abs_ransac_kernel(const Ransa
   const b2m_ransac_opts& ro = P.ro;
   const uint64_t key = splitmix64(P.seed ^ splitmix64((static_cast<uint64_t>(P.problem_base + prob) << 8) ^
                                                       static_cast<uint64_t>(fs) ^ 0x5A00000000000000ull));
-  const double max_trials_d = compute_num_trials(floor(ro.min_inlier_ratio * 100000.0), 100000.0, ro.confidence,
-                                                 ro.dyn_num_trials_multiplier, 3);
-  const int max_trials = static_cast<int>(fmin(static_cast<double>(ro.max_num_trials), max_trials_d));
+  const int max_trials = static_cast<int>(ransac_trial_cap(ro, 3));
+  const ReprojModel model{P, xn, off, c};
   double dyn_max = max_trials;
   if (tid == 0) {
     sh.best_cnt = 0;
@@ -725,99 +666,26 @@ __global__ void __launch_bounds__(kThreads, 3) b2m_abs_ransac_kernel(const Ransa
   unsigned long long n_scored = 0;
   double mdl[4 * 12];
   while (trials < max_trials) {
-    int nb = min(kThreads, max_trials - trials);
-    if (trials < ro.min_num_trials) nb = min(nb, ro.min_num_trials - trials);
-    else if (dyn_max - trials < nb) nb = max(1, static_cast<int>(ceil(dyn_max - trials)));
+    const int nb = round_size(trials, max_trials, ro.min_num_trials, dyn_max);
     // ---- one P3P hypothesis per thread
     int nm = 0;
     if (tid < nb) {
-      const uint64_t tkey = splitmix64(key + static_cast<uint64_t>(trials + tid) * 0x100000001B3ull);
       int idx[3];
-      for (int j = 0; j < 3; ++j) {
-        int cand = 0;
-        for (int attempt = 0; attempt < 64; ++attempt) {
-          const uint64_t r = splitmix64(tkey + static_cast<uint64_t>(j * 64 + attempt));
-          cand = static_cast<int>(__umul64hi(r, static_cast<uint64_t>(n)));
-          bool dup = false;
-          for (int q = 0; q < j; ++q) dup |= (idx[q] == cand);
-          if (!dup) break;
-        }
-        idx[j] = cand;
-      }
+      draw_sample<3>(key, trials + tid, n, idx);
       double x[3], y[3], W[9];
       for (int j = 0; j < 3; ++j) load_point(P, xn, off, idx[j], c, x[j], y[j], W[3 * j], W[3 * j + 1], W[3 * j + 2]);
       nm = p3p(x, y, W, mdl);
     }
     // ---- score every model of the round: chunks in shared memory, fp32 with fp64 rechecks, exact pruning
-    int my_cnt = -1, my_m = 0;
-    sh.scan[tid] = nm;
-    if (tid == 0) sh.round_max = 0;
-    __syncthreads();
-    int my_base = 0, total_models = 0;
-    for (int t = 0; t < kThreads; ++t) {
-      const int v = sh.scan[t];
-      if (t < tid) my_base += v;
-      total_models += v;
-    }
-    n_scored += total_models;
-    for (int chunk0 = 0; chunk0 < total_models; chunk0 += kChunkModels) {
-      const int n_chunk = min(kChunkModels, total_models - chunk0);
-      for (int m = 0; m < nm; ++m) {
-        const int g = my_base + m - chunk0;
-        if (g >= 0 && g < kChunkModels)
-#pragma unroll
-          for (int k = 0; k < 12; ++k) {
-            sh.chunk_d[g][k] = mdl[m * 12 + k];
-            sh.chunk_f[g][k] = static_cast<float>(mdl[m * 12 + k]);
-          }
-      }
-      for (int m = tid; m < kChunkModels; m += kThreads) sh.chunk_cnt[m] = 0;
-      __syncthreads();
-      constexpr int kBlock = 4 * kThreads;
-      for (int pb = 0; pb < n; pb += kBlock) {
-        const int rem = n - pb;
-        int need = 0;
-        if (pb > 0) {
-          __syncthreads();
-          for (int m = tid; m < n_chunk; m += kThreads) atomicMax(&sh.round_max, sh.chunk_cnt[m]);
-          __syncthreads();
-          need = max(sh.best_cnt + 1, sh.round_max) - rem;
-        }
-        if (rem > 3 * kThreads) score_block<4>(sh, P, xn, off, c, n, pb, n_chunk, thr, thr_f, tid, need);
-        else if (rem > 2 * kThreads) score_block<3>(sh, P, xn, off, c, n, pb, n_chunk, thr, thr_f, tid, need);
-        else if (rem > kThreads) score_block<2>(sh, P, xn, off, c, n, pb, n_chunk, thr, thr_f, tid, need);
-        else score_block<1>(sh, P, xn, off, c, n, pb, n_chunk, thr, thr_f, tid, need);
-      }
-      __syncthreads();
-      for (int m = 0; m < nm; ++m) {
-        const int g = my_base + m - chunk0;
-        if (g >= 0 && g < kChunkModels && sh.chunk_cnt[g] > my_cnt) {
-          my_cnt = sh.chunk_cnt[g];
-          my_m = m;
-        }
-      }
-      __syncthreads();
-    }
-    sh.cnt_arr[tid] = my_cnt;
-    __syncthreads();
-    if (tid == 0) {  // among equal counts the earlier trial wins
-      int w = -1, bc = sh.best_cnt;
-      for (int t = 0; t < nb; ++t)
-        if (sh.cnt_arr[t] > bc) {
-          bc = sh.cnt_arr[t];
-          w = t;
-        }
-      sh.winner = w;
-      sh.improved = w >= 0;
-    }
-    __syncthreads();
-    if (sh.improved) {
-      if (tid == sh.winner)
-        for (int k = 0; k < 12; ++k) sh.best_model[k] = mdl[my_m * 12 + k];
+    const RoundResult round = score_round(sh.round, model, mdl, nm, nb, n, thr, sh.best_cnt);
+    n_scored += round.n_models;
+    if (round.winner >= 0) {
+      if (tid == round.winner)
+        for (int k = 0; k < 12; ++k) sh.best_model[k] = mdl[round.model * 12 + k];
       __syncthreads();
       int bc;
       double bs;
-      support(sh, P, xn, off, c, n, sh.best_model, thr, bc, bs);
+      exact_support(sh.round, model, sh.best_model, n, thr, bc, bs);
       if (tid == 0) {
         sh.best_cnt = bc;
         sh.best_sum = bs;
@@ -833,7 +701,7 @@ __global__ void __launch_bounds__(kThreads, 3) b2m_abs_ransac_kernel(const Ransa
           if (!nc) break;
           int cc;
           double cs;
-          support(sh, P, xn, off, c, n, sh.cand[0], thr, cc, cs);
+          exact_support(sh.round, model, sh.cand[0], n, thr, cc, cs);
           n_scored += 1;
           if (tid == 0 && (cc > sh.best_cnt || (cc == sh.best_cnt && cs < sh.best_sum))) {
             sh.best_cnt = cc;
@@ -853,7 +721,7 @@ __global__ void __launch_bounds__(kThreads, 3) b2m_abs_ransac_kernel(const Ransa
   double M[12];
   for (int k = 0; k < 12; ++k) M[k] = sh.best_model[k];
   const bool ok = sh.best_cnt >= 3;
-  for (int i = tid; i < n; i += kThreads) {
+  for (int i = tid; i < n; i += kRansacThreads) {
     double u, v, X, Y, Z;
     load_point(P, xn, off, i, c, u, v, X, Y, Z);
     mask[i] = (ok && reproj_sq(M, u, v, X, Y, Z) <= thr) ? 1 : 0;
@@ -1493,7 +1361,7 @@ int b2m_estimate_absolute_pose_batch(b2m_ctx* ctx, const b2m_abs_pose_problem* p
     P.xn = d_xn; P.mask = d_cmask; P.models = d_models; P.sup = d_sup; P.success = d_succ;
     P.factors = d_fac; P.n_factors = nf; P.ro = opts->ransac; P.seed = ctx->seed; P.problem_base = k0;
     P.counters = ctx->d_counters + kAbsPoseCounters;
-    b2m_abs_ransac_kernel<<<static_cast<unsigned>(nc), kThreads, 0, st>>>(P);
+    b2m_abs_ransac_kernel<<<static_cast<unsigned>(nc), kRansacThreads, 0, st>>>(P);
     B2M_CUDA_TRY(ctx, cudaGetLastError());
     SelectParams S{};
     S.off = d_off; S.cnt = d_cnt; S.xoff = d_xoff; S.cta_mask = d_cmask; S.models = d_models; S.sup = d_sup;

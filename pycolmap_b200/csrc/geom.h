@@ -15,6 +15,8 @@
 #include <math.h>
 #include <stdint.h>
 
+#include "../../include/b200match.h"
+
 #ifdef __CUDACC__
 #define B2M_HD __host__ __device__
 #else
@@ -855,6 +857,13 @@ B2M_HD inline double compute_num_trials(double num_inliers, double num_samples, 
   if (denom <= 0.0) return 1.0;
   if (denom == 1.0) return 1e18;
   return ceil(log(nom) / log(denom) * multiplier);
+}
+
+// The RANSAC constructor's clip (U:optim/ransac.h): max_num_trials, at most the bound at min_inlier_ratio.
+B2M_HD inline double ransac_trial_cap(const b2m_ransac_opts& ro, int min_samples) {
+  return fmin(static_cast<double>(ro.max_num_trials),
+              compute_num_trials(floor(ro.min_inlier_ratio * 100000.0), 100000.0, ro.confidence,
+                                 ro.dyn_num_trials_multiplier, min_samples));
 }
 
 }  // namespace geom

@@ -572,10 +572,7 @@ int b2m_estimate_triangulation_batch(b2m_ctx* ctx, int64_t n_tracks, const int64
     for (int a = 0; a < 3; ++a)
       centers[3 * i + a] = -(P[0 * 4 + a] * P[3] + P[1 * 4 + a] * P[7] + P[2 * 4 + a] * P[11]);
   }
-  // the RANSAC constructor's clip of max_num_trials at min_inlier_ratio (U:optim/ransac.h), kMinNumSamples = 2
-  const double at_ratio = geom::compute_num_trials(static_cast<double>(static_cast<int64_t>(ro.min_inlier_ratio * 100000)),
-                                                   100000.0, ro.confidence, ro.dyn_num_trials_multiplier, 2);
-  const double max_trials = std::min(static_cast<double>(ro.max_num_trials), at_ratio);
+  const double max_trials = geom::ransac_trial_cap(ro, 2);  // kMinNumSamples = 2
 
   // chunks: at most kChunkTracks tracks and kChunkObs observations (a longer single track is its own chunk)
   std::vector<int64_t> starts{0};

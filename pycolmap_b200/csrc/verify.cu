@@ -33,7 +33,6 @@ namespace {
 
 using namespace geom;
 
-constexpr int kRansacThreads = 128;
 constexpr int kMaxLocalTrials = 10;
 
 struct DevCamera {
@@ -131,44 +130,64 @@ __device__ __forceinline__ int inlier_f32(const float* M, float x1, float y1, fl
   return classify_f32(lhs, rhs);
 }
 
+// The verifier's matches and models in the shared LO-RANSAC round (ransac_common.cuh).
+template <int KIND>
+struct EpipolarModel {
+  static constexpr int kD = 9;
+  struct Pt {
+    float x1, y1, x2, y2;
+  };
+  const double4* pts;
+  int64_t off;
+  PointXform X;
+  // a slot past the end is a far-away point (x2 = y2 = 1e15)
+  __device__ __forceinline__ Pt load_f32(int i, bool live) const {
+    double x1 = 0, y1 = 0, x2 = 1e15, y2 = 1e15;
+    if (live) load_pt(pts, off + i, X, x1, y1, x2, y2);
+    return {static_cast<float>(x1), static_cast<float>(y1), static_cast<float>(x2), static_cast<float>(y2)};
+  }
+  __device__ __forceinline__ int test(const float* M, const Pt& p, float thr) const {
+    return inlier_f32<KIND>(M, p.x1, p.y1, p.x2, p.y2, thr);
+  }
+  __device__ __forceinline__ double residual(const double* M, int i) const {
+    double x1, y1, x2, y2;
+    load_pt(pts, off + i, X, x1, y1, x2, y2);
+    return b2m::residual<KIND>(M, x1, y1, x2, y2);
+  }
+};
+
 template <int KIND>
 struct Traits;
 template <>
 struct Traits<0> {  // E: 5-point for minimal and local
-  static constexpr int kMin = 5, kLocalMin = 5, kMaxModels = 10, kMaxLocalModels = 10;
+  static constexpr int kMin = 5, kLocalMin = 5, kMaxModels = 10;
 };
 template <>
 struct Traits<1> {  // F: 7-point minimal, 8-point local
-  static constexpr int kMin = 7, kLocalMin = 8, kMaxModels = 3, kMaxLocalModels = 1;
+  static constexpr int kMin = 7, kLocalMin = 8, kMaxModels = 3;
 };
 template <>
 struct Traits<2> {  // H: 4-point DLT for both
-  static constexpr int kMin = 4, kLocalMin = 4, kMaxModels = 1, kMaxLocalModels = 1;
+  static constexpr int kMin = 4, kLocalMin = 4, kMaxModels = 1;
 };
 
-constexpr int kChunkModels = 256;  // models scored per pass of the fp32 scoring loop
-constexpr int kPtsPerThread = 8;    // points held in registers per thread and pass
-
 struct Shared {
-  double chunk_d[kChunkModels][9];  // models of the current chunk (fp64, for borderline rechecks)
-  float chunk_f[kChunkModels][12];  // same, fp32, padded to three 16-byte loads
-  int chunk_cnt[kChunkModels];      // inlier counts of the chunk's models
-  int scan[kRansacThreads];
+  RoundShared<9> round;  // round.chunk_d doubles as the scratch of the warp 5-point and eigen solvers (fpw::Scratch,
+                         // eigw::Scratch) outside the scoring round
   double best_model[9];
   double cand_models[10 * 9];
   double red[4][64];     // per-warp partial sums (45 normal-equation entries + 8 moments)
-  double sum_arr[kRansacThreads];
-  int cnt_arr[kRansacThreads];
+  double sum_arr[kRansacThreads];  // eigenvectors of the LO eigen-solve
   int cand_cnt[10];
   double cand_sum[10];
   int n_cand;
   int best_cnt;
   double best_sum;
-  int winner;
-  int improved;
-  int round_max;         // largest (partial) inlier count among the models of the current round, for the exact pruning
   double norm[6];        // s1, cx1, cy1, s2, cx2, cy2
 };
+static_assert(sizeof(RoundShared<9>::chunk_d) >= (kRansacThreads / 32) * sizeof(fpw::Scratch) &&
+                  sizeof(RoundShared<9>::chunk_d) >= sizeof(fpw::Scratch) + sizeof(eigw::Scratch),
+              "the solver scratch does not fit in round.chunk_d");
 
 // Score `model` (registers of every lane hold the same 9 values) over all points; warp-cooperative.
 template <int KIND>
@@ -187,55 +206,6 @@ __device__ __forceinline__ void warp_score(const double* M, const double4* pts, 
   }
   cnt = __reduce_add_sync(0xffffffffu, c);
   sum = warp_sum_d(s);
-}
-
-// Hypothesis scoring of one block of points: every thread keeps PPT matches (fp32) in registers and sweeps the
-// chunk's models: division-free fp32 test, fp64 only for the borderline points of a (thread, model).  Inlier counts
-// go to sh.chunk_cnt.
-template <int KIND, int PPT>
-__device__ __forceinline__ void score_block(Shared& sh, const double4* pts, int64_t off, const PointXform& X, int n, int pb,
-                                            int n_chunk, double thr, float thr_f, int tid, int need) {
-  float px1[PPT], py1[PPT], px2[PPT], py2[PPT];
-  int live[PPT];   // 1 for a real match, 0 for a slot past the end: such a slot never counts, whatever the model
-                   // (its far-away point is an outlier for every sane model, but lhs and rhs can both overflow)
-#pragma unroll
-  for (int q = 0; q < PPT; ++q) {
-    const int i = pb + q * kRansacThreads + tid;
-    double x1 = 0, y1 = 0, x2 = 1e15, y2 = 1e15;
-    live[q] = i < n ? 1 : 0;
-    if (i < n) load_pt(pts, off + i, X, x1, y1, x2, y2);
-    px1[q] = static_cast<float>(x1); py1[q] = static_cast<float>(y1);
-    px2[q] = static_cast<float>(x2); py2[q] = static_cast<float>(y2);
-  }
-  for (int m = 0; m < n_chunk; ++m) {
-    // exact pruning: a model that cannot reach `need + (matches not yet scored)` even if every remaining match were
-    // an inlier can neither beat the best model so far nor the leader of this round (uniform across the CTA)
-    if (sh.chunk_cnt[m] < need) continue;
-    float Mf[12];
-    const float4* mp = reinterpret_cast<const float4*>(sh.chunk_f[m]);
-    const float4 m0 = mp[0], m1 = mp[1], m2 = mp[2];
-    Mf[0] = m0.x; Mf[1] = m0.y; Mf[2] = m0.z; Mf[3] = m0.w;
-    Mf[4] = m1.x; Mf[5] = m1.y; Mf[6] = m1.z; Mf[7] = m1.w; Mf[8] = m2.x;
-    int c = 0, flags = 0;
-#pragma unroll
-    for (int q = 0; q < PPT; ++q) {
-      const int f = inlier_f32<KIND>(Mf, px1[q], py1[q], px2[q], py2[q], thr_f);
-      c += f & live[q];
-      flags |= f;
-    }
-    if (flags & 2) {  // rare: a borderline point -> redo this thread's points of this model in fp64
-      c = 0;
-      for (int q = 0; q < PPT; ++q) {
-        const int i = pb + q * kRansacThreads + tid;
-        if (i < n) {
-          double x1, y1, x2, y2;
-          load_pt(pts, off + i, X, x1, y1, x2, y2);
-          c += (residual<KIND>(sh.chunk_d[m], x1, y1, x2, y2) <= thr) ? 1 : 0;
-        }
-      }
-    }
-    if (c) atomicAdd(&sh.chunk_cnt[m], c);  // most hypotheses have (almost) no inliers: cheaper than a warp reduce
-  }
 }
 
 #define B2M_TICK(slot)                                   \
@@ -271,10 +241,8 @@ __device__ void ransac_problem(const VerifyParams& P, Shared& sh, int pair, int6
     }
     return;
   }
-  // RANSAC ctor: clip max_num_trials by the bound at min_inlier_ratio
-  double max_trials_d = compute_num_trials(floor(ro.min_inlier_ratio * 100000.0), 100000.0, ro.confidence,
-                                           ro.dyn_num_trials_multiplier, T::kMin);
-  const int max_trials = static_cast<int>(fmin(static_cast<double>(ro.max_num_trials), max_trials_d));
+  const int max_trials = static_cast<int>(ransac_trial_cap(ro, T::kMin));
+  const EpipolarModel<KIND> model{pts, off, X};
   double dyn_max = max_trials;
   if (tid == 0) {
     sh.best_cnt = 0;
@@ -295,27 +263,12 @@ __device__ void ransac_problem(const VerifyParams& P, Shared& sh, int pair, int6
   long long prof_acc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
   long long prof_t = clock64();
   while (trials < max_trials) {
-    int nb = min(kRansacThreads, max_trials - trials);
-    if (trials < ro.min_num_trials) nb = min(nb, ro.min_num_trials - trials);
-    // past min_num_trials the sequential reference stops at the FIRST trial >= dyn_max: a round never needs more
-    // hypotheses than are missing to that bound (a better model found among them only lowers it)
-    else if (dyn_max - trials < nb) nb = max(1, static_cast<int>(ceil(dyn_max - trials)));
+    const int nb = round_size(trials, max_trials, ro.min_num_trials, dyn_max);
     // ---- phase 1: one minimal-sample hypothesis per thread
     int nm = 0;
     if (tid < nb) {
-      const uint64_t tkey = splitmix64(key + static_cast<uint64_t>(trials + tid) * 0x100000001B3ull);
       int idx[T::kMin];
-      for (int j = 0; j < T::kMin; ++j) {
-        int cand = 0;
-        for (int attempt = 0; attempt < 64; ++attempt) {
-          const uint64_t r = splitmix64(tkey + static_cast<uint64_t>(j * 64 + attempt));
-          cand = static_cast<int>(__umul64hi(r, static_cast<uint64_t>(n)));
-          bool dup = false;
-          for (int q = 0; q < j; ++q) dup |= (idx[q] == cand);
-          if (!dup) break;
-        }
-        idx[j] = cand;
-      }
+      draw_sample<T::kMin>(key, trials + tid, n, idx);
       double x1[T::kMin], y1[T::kMin], x2[T::kMin], y2[T::kMin];
       for (int j = 0; j < T::kMin; ++j) load_pt(pts, off + idx[j], X, x1[j], y1[j], x2[j], y2[j]);
       if (KIND == 0 && !kWarpMin) nm = minimal_E5(x1, y1, x2, y2, mdl);
@@ -332,12 +285,12 @@ __device__ void ransac_problem(const VerifyParams& P, Shared& sh, int pair, int6
       if (KIND == 2) nm = minimal_H4_closed(x1, y1, x2, y2, mdl);
     }
     if (kWarpMin) {
-      sh.scan[tid] = nm;
+      sh.round.scan[tid] = nm;
       __syncthreads();
-      fpw::Scratch& WS = reinterpret_cast<fpw::Scratch*>(sh.chunk_d)[warp];   // chunk_d is idle outside the scoring loop
+      fpw::Scratch& WS = reinterpret_cast<fpw::Scratch*>(sh.round.chunk_d)[warp];
       for (int h = warp; h < nb; h += kRansacThreads / 32) {
         int cnt = 0;
-        if (sh.scan[h]) {   // uniform in the warp
+        if (sh.round.scan[h]) {   // uniform in the warp
           double* hm = P.e_scratch + (static_cast<size_t>(pair) * kRansacThreads + h) * kEStride;
           for (int k = lane; k < 36; k += 32) WS.N[k] = hm[kEN + k];
           __syncwarp();
@@ -352,135 +305,30 @@ __device__ void ransac_problem(const VerifyParams& P, Shared& sh, int pair, int6
           }
         }
         __syncwarp();
-        if (lane == 0) sh.scan[h] = cnt;
+        if (lane == 0) sh.round.scan[h] = cnt;
       }
       __syncthreads();
-      nm = tid < nb ? sh.scan[tid] : 0;
+      nm = tid < nb ? sh.round.scan[tid] : 0;
       if (kHybrid && nm) nm = fpw::finish_thread(e_models + kEN, e_models + kEPoly, e_models + kEMr, e_models);
       __syncthreads();
     }
-    // ---- phase 2: score every model of every hypothesis of this warp (warp = one model at a time)
+    // ---- phase 2: score every model of the round
     B2M_TICK(0);
-    //      Models go to shared memory in chunks; every thread keeps kPtsPerThread points in registers
-    //      (fp32) and sweeps the chunk's models: division-free fp32 test, fp64 only for borderline
-    //      points.  Only inlier COUNTS are formed here; among equal counts the earlier trial wins
-    //      (the residual-sum tie-break of U:optim/support_measurement.h applies from the LO stage on).
-    int my_cnt = -1, my_m = 0;
-    double my_sum = 1e300;
-    sh.scan[tid] = nm;
-    if (tid == 0) sh.round_max = 0;
-    __syncthreads();
-    int my_base = 0, total_models = 0;
-    for (int t = 0; t < kRansacThreads; ++t) {
-      const int v = sh.scan[t];
-      if (t < tid) my_base += v;
-      total_models += v;
-    }
-    const float thr_f = static_cast<float>(thr);
-    n_scored += total_models;
-    for (int chunk0 = 0; chunk0 < total_models; chunk0 += kChunkModels) {
-      const int n_chunk = min(kChunkModels, total_models - chunk0);
-      for (int m = 0; m < nm; ++m) {
-        const int g = my_base + m - chunk0;
-        if (g >= 0 && g < kChunkModels) {
-#pragma unroll
-          for (int k = 0; k < 9; ++k) {
-            sh.chunk_d[g][k] = mdl[m * 9 + k];
-            sh.chunk_f[g][k] = static_cast<float>(mdl[m * 9 + k]);
-          }
-        }
-      }
-      for (int m = tid; m < kChunkModels; m += kRansacThreads) sh.chunk_cnt[m] = 0;
-      __syncthreads();
-      // Blocks of 512 matches.  Between blocks the inlier counts so far are complete (barrier), so a model whose count
-      // plus ALL remaining matches stays below the best of the earlier rounds or below what the leader of this round
-      // already has is dropped for the rest of the sweep -- exact: it could not have won, nor tied.
-      constexpr int kBlock = 4 * kRansacThreads;
-      for (int pb = 0; pb < n; pb += kBlock) {
-        const int rem = n - pb;
-        int need = 0;
-        if (pb > 0) {
-          __syncthreads();   // chunk_cnt of the previous blocks is complete
-          for (int m = tid; m < n_chunk; m += kRansacThreads) atomicMax(&sh.round_max, sh.chunk_cnt[m]);
-          __syncthreads();
-          need = max(sh.best_cnt + 1, sh.round_max) - rem;
-        }
-        // the last block takes as few point slots per thread as cover it (a slot past the end costs a full test)
-        if (rem > 3 * kRansacThreads) score_block<KIND, 4>(sh, pts, off, X, n, pb, n_chunk, thr, thr_f, tid, need);
-        else if (rem > 2 * kRansacThreads) score_block<KIND, 3>(sh, pts, off, X, n, pb, n_chunk, thr, thr_f, tid, need);
-        else if (rem > kRansacThreads) score_block<KIND, 2>(sh, pts, off, X, n, pb, n_chunk, thr, thr_f, tid, need);
-        else score_block<KIND, 1>(sh, pts, off, X, n, pb, n_chunk, thr, thr_f, tid, need);
-      }
-      __syncthreads();
-      for (int m = 0; m < nm; ++m) {
-        const int g = my_base + m - chunk0;
-        if (g >= 0 && g < kChunkModels) {
-          const int c = sh.chunk_cnt[g];
-          if (c > my_cnt) {
-            my_cnt = c;
-            my_m = m;
-          }
-        }
-      }
-      __syncthreads();
-    }
-    sh.cnt_arr[tid] = my_cnt;
-    sh.sum_arr[tid] = my_sum;
-    __syncthreads();
+    const RoundResult round = score_round(sh.round, model, mdl, nm, nb, n, thr, sh.best_cnt);
+    n_scored += round.n_models;
     B2M_TICK(1);
-    if (tid == 0) {
-      int w = -1, bc = sh.best_cnt;
-      double bs = sh.best_sum;
-      for (int t = 0; t < nb; ++t) {
-        const int c = sh.cnt_arr[t];
-        const double s = sh.sum_arr[t];
-        if (c > bc || (c == bc && s < bs)) {
-          bc = c;
-          bs = s;
-          w = t;
-        }
-      }
-      sh.winner = w;
-      sh.improved = (w >= 0);
-      if (w >= 0) {
+    if (round.winner >= 0) {
+      if (tid == round.winner)
+        for (int k = 0; k < 9; ++k) sh.best_model[k] = mdl[round.model * 9 + k];
+      __syncthreads();
+      int bc;
+      double bs;
+      exact_support(sh.round, model, sh.best_model, n, thr, bc, bs);
+      if (tid == 0) {
         sh.best_cnt = bc;
         sh.best_sum = bs;
       }
-    }
-    __syncthreads();
-    if (sh.improved) {
-      if (tid == sh.winner)
-        for (int k = 0; k < 9; ++k) sh.best_model[k] = mdl[my_m * 9 + k];
       __syncthreads();
-      {  // exact fp64 support (count, residual sum) of the new best model
-        double M[9];
-        for (int k = 0; k < 9; ++k) M[k] = sh.best_model[k];
-        int c;
-        double s;
-        int cl = 0;
-        double sl = 0.0;
-        for (int i = tid; i < n; i += kRansacThreads) {
-          double x1, y1, x2, y2;
-          load_pt(pts, off + i, X, x1, y1, x2, y2);
-          const double r = residual<KIND>(M, x1, y1, x2, y2);
-          if (r <= thr) {
-            ++cl;
-            sl += r;
-          }
-        }
-        c = __reduce_add_sync(0xffffffffu, cl);
-        s = warp_sum_d(sl);
-        if (lane == 0) {
-          sh.cand_cnt[warp] = c;
-          sh.cand_sum[warp] = s;
-        }
-        __syncthreads();
-        if (tid == 0) {
-          sh.best_cnt = sh.cand_cnt[0] + sh.cand_cnt[1] + sh.cand_cnt[2] + sh.cand_cnt[3];
-          sh.best_sum = sh.cand_sum[0] + sh.cand_sum[1] + sh.cand_sum[2] + sh.cand_sum[3];
-        }
-        __syncthreads();
-      }
       B2M_TICK(2);
       n_scored += 1;  // exact fp64 support of the new best
       // ---- phase 3: recursive local optimisation on the inliers of the current best
@@ -552,7 +400,7 @@ __device__ void ransac_problem(const VerifyParams& P, Shared& sh, int pair, int6
                 // IS the essential matrix).  The solver itself runs on warp 0 below.
                 double Nr[36];
                 smallest_eigvecs_invit<4>(St, Nr);
-                fpw::Scratch& WS = reinterpret_cast<fpw::Scratch*>(sh.chunk_d)[0];
+                fpw::Scratch& WS = reinterpret_cast<fpw::Scratch*>(sh.round.chunk_d)[0];
                 for (int k = 0; k < 4; ++k)
                   for (int e = 0; e < 9; ++e) WS.N[k * 9 + e] = Nr[(3 - k) * 9 + e];
               } else if (KIND == 1) {
@@ -570,9 +418,9 @@ __device__ void ransac_problem(const VerifyParams& P, Shared& sh, int pair, int6
               double* St = sh.red[0];   // summed in place: red[0][k] += red[1..3][k]
               for (int k = lane; k < 45; k += 32) St[k] = sh.red[0][k] + sh.red[1][k] + sh.red[2][k] + sh.red[3][k];
               __syncwarp();
-              // scratch: the second warp slot of the 5-point scratch area (chunk_d is idle outside the scoring loop)
-              eigw::Scratch& ES = *reinterpret_cast<eigw::Scratch*>(reinterpret_cast<fpw::Scratch*>(sh.chunk_d) + 1);
-              double* vec = sh.sum_arr;   // [K][9], free between rounds
+              // scratch: the second warp slot of the 5-point scratch area
+              eigw::Scratch& ES = *reinterpret_cast<eigw::Scratch*>(reinterpret_cast<fpw::Scratch*>(sh.round.chunk_d) + 1);
+              double* vec = sh.sum_arr;   // [K][9]
               eigw::smallest_eigvecs_warp<KIND == 0 ? 4 : 1>(St, vec, ES, lane);
               if (lane == 0) {
                 int nc = 0;
@@ -580,7 +428,7 @@ __device__ void ransac_problem(const VerifyParams& P, Shared& sh, int pair, int6
                   // least-squares 4-D null space of the N x 9 system.  The 5-point solver fixes the coefficient of
                   // its LAST basis vector to 1, so that one must be the smallest singular vector (for noise-free
                   // inliers it IS the essential matrix).
-                  fpw::Scratch& WS = reinterpret_cast<fpw::Scratch*>(sh.chunk_d)[0];
+                  fpw::Scratch& WS = reinterpret_cast<fpw::Scratch*>(sh.round.chunk_d)[0];
                   for (int k = 0; k < 4; ++k)
                     for (int e = 0; e < 9; ++e) WS.N[k * 9 + e] = vec[(3 - k) * 9 + e];
                 } else if (KIND == 1) {
@@ -602,7 +450,7 @@ __device__ void ransac_problem(const VerifyParams& P, Shared& sh, int pair, int6
           }
           if (KIND == 0) {
             if (warp == 0) {
-              const int nc = fpw::five_point_warp(reinterpret_cast<fpw::Scratch*>(sh.chunk_d)[0], sh.cand_models, lane);
+              const int nc = fpw::five_point_warp(reinterpret_cast<fpw::Scratch*>(sh.round.chunk_d)[0], sh.cand_models, lane);
               if (lane == 0) sh.n_cand = nc;
             }
             __syncthreads();

@@ -2,11 +2,14 @@
 each 1000-4000 2D-3D correspondences with 50 % outliers, SIMPLE_RADIAL camera, focal + extra-parameter refinement
 (what hloc-style localization runs once per query image).  Prints one JSON line.
 
-  python tools/bench_abs_pose.py [--queries 4096] [--reps 3] [--fail-queries 132] [--cpu-sample 4]
+  python tools/bench_abs_pose.py [--queries 4096] [--reps 3] [--fail-queries 132] [--cpu-sample 4] [--dump-outputs DIR]
 
 Reports: problems/s end to end (host clock around the blocking call) and from the kernel durations of a
 torch.profiler trace; the cost of all-outlier queries that run to max_num_trials; a CPU arm (the numpy oracle) on a
-sample with its agreement; the card name and power limit, read in the same run."""
+sample with its agreement; the card name and power limit, read in the same run.
+
+--dump-outputs DIR writes the results of the last timed call and of the all-outlier queries as DIR/<name>.npy, so that
+two builds can be compared output for output on identical, seeded inputs."""
 import argparse
 import json
 import os
@@ -54,12 +57,34 @@ def kernel_ms(fn):
     return tot
 
 
+def dump_outputs(out_dir, prefix, res):
+    """success, inlier count, pose (quaternion x, y, z, w and translation; NaN on failure), camera parameters (NaN on
+    failure) and the concatenated inlier masks of one estimate_absolute_poses call."""
+    ok = [r is not None for r in res]
+    nan = np.full(7, np.nan)
+    arrays = {
+        "success": np.array(ok, np.uint8),
+        "num_inliers": np.array([r["num_inliers"] if r is not None else 0 for r in res], np.int64),
+        "pose": np.array([np.r_[r["cam_from_world"].rotation.quat, r["cam_from_world"].translation] if r is not None
+                          else nan for r in res], np.float64),
+        "camera_params": np.array([r["camera_params"] if r is not None else np.full(len(CAM["params"]), np.nan)
+                                   for r in res], np.float64),
+        "inliers": np.concatenate([np.asarray(r["inliers"], np.uint8) for r in res if r is not None] +
+                                  [np.zeros(0, np.uint8)]),
+    }
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, f"{prefix}_{name}.npy"), a)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--queries", type=int, default=4096)
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--fail-queries", type=int, default=132)
     ap.add_argument("--cpu-sample", type=int, default=4)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the results of the last timed call and of the failing queries as DIR/<name>.npy")
     a = ap.parse_args()
     import torch
     if not torch.cuda.is_available():
@@ -95,6 +120,9 @@ def main():
     out["fail_queries"] = a.fail_queries
     out["fail_end_to_end_s"] = round(tf, 3)
     out["fail_success"] = int(sum(r is not None for r in fres))
+    if a.dump_outputs:
+        dump_outputs(a.dump_outputs, "queries", res)
+        dump_outputs(a.dump_outputs, "fail_queries", fres)
     # CPU arm: the numpy oracle on a sample, agreement of inlier counts with the GPU
     t0 = time.perf_counter()
     agree = []
