@@ -26,9 +26,10 @@
 extern "C" {
 #endif
 
-#define B2M_ABI_VERSION 6   /* 2: b2m_camera carries 12 parameters, batch estimator; 3: multi-GPU entry points (NCCL);
+#define B2M_ABI_VERSION 7   /* 2: b2m_camera carries 12 parameters, batch estimator; 3: multi-GPU entry points (NCCL);
                              * 4: absolute pose estimation / refinement, b2m_stats.abs_pose_*;
-                             * 5: triangulation, b2m_stats.tri_*; 6: SIFT feature extraction, b2m_stats.sift_* */
+                             * 5: triangulation, b2m_stats.tri_*; 6: SIFT feature extraction, b2m_stats.sift_*;
+                             * 7: extraction from encoded / RGB sources, b2m_stats.sift_decode* */
 
 /* error codes */
 #define B2M_OK 0
@@ -471,6 +472,48 @@ int b2m_extract_features_batch(b2m_ctx* ctx, const b2m_image* images, int32_t n,
 int b2m_features_get(const b2m_features* f, int32_t image, b2m_feature_view* out);
 void b2m_features_free(b2m_features* f);
 
+/* ---- feature extraction from image sources (ABI 7) ----------------------------------------------------------------
+ * What COLMAP's feature extraction does to one image between reading the file and writing the database (U:controllers/
+ * feature_extraction.cc, U:controllers/image_reader.cc; SURVEY.md rows U1-U6): decode, convert to grey (FreeImage's
+ * ConvertToGreyscale, Rec709 weights), downscale when max(w, h) > max_image_size (FreeImage's bilinear Rescale), SIFT,
+ * keypoints back to original-image coordinates as FeatureKeypoint's 6 columns, and the mask test.  Decoding uses
+ * nvJPEG's hardware backend where the GPU has JPEG engines and the file is baseline, the hybrid backend otherwise; a
+ * decoder thread and a side stream decode, convert and downscale the next images while SIFT runs the current one. */
+#define B2M_SOURCE_JPEG 0    /* data / size: a whole JPEG file, decoded on the device (nvJPEG) */
+#define B2M_SOURCE_PIXELS 1  /* data: width x height pixels of `channels` bytes (1 grey, 3 RGB, 4 RGBA: alpha ignored),
+                              * `stride` bytes per row, in host memory */
+typedef struct b2m_image_source {
+  int32_t kind;                  /* B2M_SOURCE_* */
+  int32_t channels;              /* B2M_SOURCE_PIXELS: 1, 3 or 4 */
+  int32_t width, height;         /* B2M_SOURCE_PIXELS: the size; JPEG: ignored, read from the stream */
+  int64_t stride;                /* B2M_SOURCE_PIXELS: bytes between rows (>= width x channels) */
+  const uint8_t* data;
+  int64_t size;                  /* B2M_SOURCE_JPEG: bytes */
+  const uint8_t* mask;           /* NULL, or a grey mask in original-image coordinates: a keypoint is dropped when its
+                                  * integer pixel (int)x, (int)y lies outside the mask or the mask is 0 there
+                                  * (MaskKeypoints) */
+  int32_t mask_width, mask_height;
+  int64_t mask_stride;
+} b2m_image_source;
+
+typedef struct b2m_source_view {
+  uint32_t struct_size;
+  int32_t status;                /* B2M_OK, or B2M_EINVAL when the source could not be decoded (nothing else is set) */
+  const char* error;             /* why, when status != B2M_OK */
+  int32_t width, height;         /* decoded (original) size */
+  int64_t n;                     /* features kept */
+  const float* keypoints;        /* [n x 6] (x, y, a11, a12, a21, a22) in original-image coordinates */
+  const uint8_t* descriptors;    /* [n x 128] */
+} b2m_source_view;
+
+/* Extracts `n` sources in order.  An image whose larger side exceeds opts->max_image_size is downscaled to
+ * (int)(w * s) x (int)(h * s), s = max_image_size / max(w, h), before SIFT, and its keypoints scaled back per axis
+ * (ScaleKeypoints).  A source that does not decode gets status B2M_EINVAL and the others go on; a bad argument fails
+ * the call.  *out is read with b2m_source_features_get and released with b2m_features_free. */
+int b2m_extract_features_sources(b2m_ctx* ctx, const b2m_image_source* sources, int32_t n, const b2m_extract_opts* opts,
+                                 b2m_features** out);
+int b2m_source_features_get(const b2m_features* f, int32_t image, b2m_source_view* out);
+
 /* ---- instrumentation ---------------------------------------------------------------- */
 
 /* The cross-check consults m21 only at the columns some row matched (m21[m12[i]]): the column-direction GEMM is run
@@ -496,6 +539,12 @@ enum b2m_k1_dir1_mode {
  * csrc/geom.h compiled for the host (U:estimators/essential_matrix.cc EssentialMatrixFivePointEstimator). */
 int b2m_debug_five_point(b2m_ctx* ctx, const double* nullspaces, int64_t n, double* models, int32_t* n_models);
 
+/* The grey image b2m_extract_features_sources feeds to SIFT for `source` (decoded, grey, downscaled when it exceeds
+ * max_image_size).  With grey == NULL only *width / *height are set; otherwise grey holds width x height bytes.
+ * Exists so that tests can hold the device decoder and the rescale against a host decoder / the numpy oracle. */
+int b2m_debug_decode_grey(b2m_ctx* ctx, const b2m_image_source* source, int32_t max_image_size, uint8_t* grey,
+                          int32_t* width, int32_t* height);
+
 typedef struct b2m_stats {
   uint32_t struct_size;
   uint32_t reserved;
@@ -520,6 +569,9 @@ typedef struct b2m_stats {
   uint64_t sift_images;               /* SIFT extraction: images processed since reset */
   uint64_t sift_keypoints;            /* SIFT extraction: keypoints kept after the max_num_features cut */
   uint64_t sift_descriptors;          /* SIFT extraction: descriptors computed (keypoints x orientations) */
+  uint64_t sift_decoded_bytes;        /* extraction from sources: encoded JPEG bytes decoded on the device */
+  uint64_t sift_decode_images;        /* extraction from sources: images decoded (JPEG) or uploaded (pixels) */
+  uint64_t sift_decode_hardware;      /* of those, JPEG files decoded by nvJPEG's hardware backend (the JPEG engines) */
 } b2m_stats;
 int b2m_get_stats(b2m_ctx* ctx, b2m_stats* out);
 int b2m_reset_stats(b2m_ctx* ctx);

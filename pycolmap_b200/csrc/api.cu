@@ -744,6 +744,7 @@ void b2m_destroy(b2m_ctx* ctx) {
   comm_release(ctx);
   tri_release(ctx);
   sift_release(ctx);
+  image_io_release(ctx);
   verify_release(ctx);
   delete ctx;
 }

@@ -131,6 +131,7 @@ struct b2m_ctx {
   int comm_size = 1, comm_rank = 0;
   void* tri_state = nullptr;     // b2m::TriState (triangulation.cu): pinned staging and device buffers
   void* sift_state = nullptr;    // b2m::SiftState (sift.cu): pyramid, gradient and keypoint buffers
+  void* image_io_state = nullptr;  // b2m::ImageIoState (image_io.cu): nvJPEG handles, decode and rescale buffers
 };
 
 namespace b2m {
@@ -143,7 +144,31 @@ inline int fail(b2m_ctx* ctx, int code, const std::string& msg) {
 void tri_release(b2m_ctx* ctx);
 // sift.cu
 void sift_release(b2m_ctx* ctx);
+// One extraction call: the options, checked, and the Gaussian filters sift_begin uploaded for them.
+struct SiftPlan {
+  b2m_extract_opts opts;
+  std::vector<int> tap_off, tap_r;
+};
+// SiftExtractionOptions::Check and the size checks of n images (widths / heights), then the buffers sized for the
+// largest of them and the filter taps uploaded.
+int sift_begin(b2m_ctx* ctx, const b2m_extract_opts* opts, const int32_t* widths, const int32_t* heights, int32_t n,
+               SiftPlan* plan);
+// K6 on one W x H grey image (`stride` bytes per row) in host memory, or in device memory when `on_device`; appends
+// its features to F.  *d_kout (when not NULL) = the device copy of its [n x 4] keypoints, valid until the next call.
+int sift_extract(b2m_ctx* ctx, const SiftPlan& plan, const uint8_t* img, int64_t stride, int W, int H, bool on_device,
+                 b2m_features* F, const float** d_kout);
+// image_io.cu
+void image_io_release(b2m_ctx* ctx);
 }  // namespace b2m
+
+struct b2m_features {
+  std::vector<int64_t> off;   // [n_images + 1] feature offsets
+  std::vector<float> kpts;    // [total x 4] (b2m_extract_features_batch) or [total x 6] (b2m_extract_features_sources)
+  std::vector<uint8_t> desc;  // [total x 128]
+  // b2m_extract_features_sources only, per image: decoded width / height, status and the reason of a failed decode
+  std::vector<int32_t> width, height, status;
+  std::vector<std::string> error;
+};
 
 namespace b2m {
 // Allocator of the two big result arrays (hundreds of MB per exhaustive call): resize() leaves new elements

@@ -19,12 +19,6 @@
 
 #include "internal.h"
 
-struct b2m_features {
-  std::vector<int64_t> off;   // [n_images + 1] feature offsets
-  std::vector<float> kpts;    // [total x 4]
-  std::vector<uint8_t> desc;  // [total x 128]
-};
-
 namespace b2m {
 namespace {
 
@@ -597,17 +591,17 @@ int num_octaves_built(int W, int H, const b2m_extract_opts& op) {
 
 inline unsigned blocks_for(int64_t n, int t) { return static_cast<unsigned>((n + t - 1) / t); }
 
-int extract_one(b2m_ctx* ctx, SiftState* S, const b2m_image& im, const b2m_extract_opts& op, const std::vector<int>& tap_off,
-                const std::vector<int>& tap_r, b2m_features* F) {
+int extract_one(b2m_ctx* ctx, SiftState* S, const uint8_t* src, int64_t stride, int W, int H, cudaMemcpyKind kind,
+                const b2m_extract_opts& op, const std::vector<int>& tap_off, const std::vector<int>& tap_r, b2m_features* F) {
   cudaStream_t st = ctx->stream;
-  const int Sr = op.octave_resolution, o_min = op.first_octave, W = im.width, H = im.height;
+  const int Sr = op.octave_resolution, o_min = op.first_octave;
   const double sigmak = std::pow(2.0, 1.0 / Sr), sigma0 = 1.6 * sigmak;
   auto dims = [&](int o, int* w, int* h) { octave_dims(W, H, o, w, h); };
   int w0, h0;
   dims(o_min, &w0, &h0);
   const int64_t A0 = static_cast<int64_t>(w0) * h0;
   // base level
-  B2M_CUDA_TRY(ctx, cudaMemcpy2DAsync(S->px.d_img, W, im.data, im.stride, W, H, cudaMemcpyHostToDevice, st));
+  B2M_CUDA_TRY(ctx, cudaMemcpy2DAsync(S->px.d_img, W, src, stride, W, H, kind, st));
   float* G = S->px.d_G;
   float* base = G;  // level s = -1
   {
@@ -758,33 +752,8 @@ void sift_release(b2m_ctx* ctx) {
   ctx->sift_state = nullptr;
 }
 
-}  // namespace b2m
-
-using namespace b2m;
-
-extern "C" {
-
-void b2m_extract_opts_default(b2m_extract_opts* o) {
-  if (!o) return;
-  memset(o, 0, sizeof(*o));
-  o->struct_size = sizeof(*o);
-  o->max_image_size = 3200;
-  o->max_num_features = 8192;
-  o->first_octave = -1;
-  o->num_octaves = 4;
-  o->octave_resolution = 3;
-  o->peak_threshold = 0.02 / 3;
-  o->edge_threshold = 10.0;
-  o->max_num_orientations = 2;
-  o->upright = 0;
-  o->normalization = B2M_NORMALIZATION_L1_ROOT;
-}
-
-int b2m_extract_features_batch(b2m_ctx* ctx, const b2m_image* images, int32_t n, const b2m_extract_opts* opts,
-                               b2m_features** out) {
-  if (!ctx) return B2M_EINVAL;
-  if (!out || !opts || n < 0 || (n > 0 && !images)) return fail(ctx, B2M_EINVAL, "[sift.cu] Check Failed: images, options and out != NULL");
-  *out = nullptr;
+int sift_begin(b2m_ctx* ctx, const b2m_extract_opts* opts, const int32_t* widths, const int32_t* heights, int32_t n,
+               SiftPlan* plan) {
   if (opts->struct_size != sizeof(b2m_extract_opts))
     return fail(ctx, B2M_EINVAL, "[sift.cu] Check Failed: b2m_extract_opts.struct_size == sizeof(b2m_extract_opts)");
   const b2m_extract_opts& o = *opts;
@@ -802,12 +771,11 @@ int b2m_extract_features_batch(b2m_ctx* ctx, const b2m_image* images, int32_t n,
   if (o.estimate_affine_shape || o.domain_size_pooling)
     return fail(ctx, B2M_EINVAL, "[sift.cu] Check Failed: estimate_affine_shape and domain_size_pooling (the covariant path) are not supported");
   if (o.darkness_adaptivity) return fail(ctx, B2M_EINVAL, "[sift.cu] Check Failed: darkness_adaptivity (SiftGPU only) is not supported");
+  plan->opts = o;
   int64_t max_a0 = 0, need_grad = 1;
   int max_w = 0, max_h = 0;
   for (int32_t i = 0; i < n; ++i) {
-    const b2m_image& im = images[i];
-    if (!im.data || im.width <= 0 || im.height <= 0 || im.stride < im.width)
-      return fail(ctx, B2M_EINVAL, "[sift.cu] Check Failed: image " + std::to_string(i) + " is non-empty with stride >= width");
+    const b2m_image im{widths[i], heights[i], widths[i], nullptr};
     if (im.width > o.max_image_size || im.height > o.max_image_size)
       return fail(ctx, B2M_EINVAL, "[sift.h] Check Failed: image " + std::to_string(i) + " within max_image_size");
     const int f = o.first_octave;
@@ -871,7 +839,10 @@ int b2m_extract_features_batch(b2m_ctx* ctx, const b2m_image* images, int32_t n,
   const double sigmak = std::pow(2.0, 1.0 / Sr), sigma0 = 1.6 * sigmak;
   const double dsigma0 = sigma0 * std::sqrt(1.0 - 1.0 / (sigmak * sigmak));
   std::vector<float> taps;
-  std::vector<int> tap_off(nlev), tap_r(nlev);
+  std::vector<int>& tap_off = plan->tap_off;
+  std::vector<int>& tap_r = plan->tap_r;
+  tap_off.assign(nlev, 0);
+  tap_r.assign(nlev, 0);
   {
     const double sa = sigma0 * std::pow(sigmak, -1), sb = 0.5 * std::pow(2.0, -o.first_octave);
     tap_off[0] = 0;
@@ -894,6 +865,58 @@ int b2m_extract_features_batch(b2m_ctx* ctx, const b2m_image* images, int32_t n,
     return fail(ctx, B2M_EINVAL, "[sift.cu] Check Failed: Gaussian half-width <= " + std::to_string(kMaxBlurR) +
                " (octave_resolution and first_octave give a smoothing this wide)");
   B2M_CUDA_TRY(ctx, cudaMemcpy(S->tab.d_taps, taps.data(), sizeof(float) * std::max<size_t>(taps.size(), 1), cudaMemcpyHostToDevice));
+  return B2M_OK;
+}
+
+int sift_extract(b2m_ctx* ctx, const SiftPlan& plan, const uint8_t* img, int64_t stride, int W, int H, bool on_device,
+                 b2m_features* F, const float** d_kout) {
+  SiftState* S = static_cast<SiftState*>(ctx->sift_state);
+  if (int rc = extract_one(ctx, S, img, stride, W, H, on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice,
+                           plan.opts, plan.tap_off, plan.tap_r, F))
+    return rc;
+  if (d_kout) *d_kout = S->d_kout;
+  return B2M_OK;
+}
+
+}  // namespace b2m
+
+using namespace b2m;
+
+extern "C" {
+
+void b2m_extract_opts_default(b2m_extract_opts* o) {
+  if (!o) return;
+  memset(o, 0, sizeof(*o));
+  o->struct_size = sizeof(*o);
+  o->max_image_size = 3200;
+  o->max_num_features = 8192;
+  o->first_octave = -1;
+  o->num_octaves = 4;
+  o->octave_resolution = 3;
+  o->peak_threshold = 0.02 / 3;
+  o->edge_threshold = 10.0;
+  o->max_num_orientations = 2;
+  o->upright = 0;
+  o->normalization = B2M_NORMALIZATION_L1_ROOT;
+}
+
+int b2m_extract_features_batch(b2m_ctx* ctx, const b2m_image* images, int32_t n, const b2m_extract_opts* opts,
+                               b2m_features** out) {
+  if (!ctx) return B2M_EINVAL;
+  if (!out || !opts || n < 0 || (n > 0 && !images)) return fail(ctx, B2M_EINVAL, "[sift.cu] Check Failed: images, options and out != NULL");
+  *out = nullptr;
+  if (opts->struct_size != sizeof(b2m_extract_opts))
+    return fail(ctx, B2M_EINVAL, "[sift.cu] Check Failed: b2m_extract_opts.struct_size == sizeof(b2m_extract_opts)");
+  std::vector<int32_t> widths(n), heights(n);
+  for (int32_t i = 0; i < n; ++i) {
+    const b2m_image& im = images[i];
+    if (!im.data || im.width <= 0 || im.height <= 0 || im.stride < im.width)
+      return fail(ctx, B2M_EINVAL, "[sift.cu] Check Failed: image " + std::to_string(i) + " is non-empty with stride >= width");
+    widths[i] = im.width;
+    heights[i] = im.height;
+  }
+  SiftPlan plan;
+  if (int rc = sift_begin(ctx, opts, widths.data(), heights.data(), n, &plan)) return rc;
   b2m_features* F = new b2m_features();
   F->off.push_back(0);
   for (int32_t i = 0; i < n; ++i) {
@@ -901,7 +924,7 @@ int b2m_extract_features_batch(b2m_ctx* ctx, const b2m_image* images, int32_t n,
       delete F;
       return B2M_ESTOPPED;
     }
-    if (int rc = extract_one(ctx, S, images[i], o, tap_off, tap_r, F)) {
+    if (int rc = sift_extract(ctx, plan, images[i].data, images[i].stride, images[i].width, images[i].height, false, F, nullptr)) {
       delete F;
       return rc;
     }

@@ -24,13 +24,17 @@
 #include <atomic>
 #include <chrono>
 #include <cstring>
+#include <filesystem>
+#include <fstream>
 #include <functional>
+#include <future>
 #include <thread>
 
 #include "../csrc/camera_models.h"
 #include "controllers.h"
 #include "dataclass.h"
 #include "database.h"
+#include "image_reader.h"
 
 namespace py = pybind11;
 using namespace b2mh;
@@ -695,6 +699,253 @@ py::list ExtractBatch(const Sift& s, const py::sequence& images) {
   return out;
 }
 
+
+// b2m_debug_decode_grey on a JPEG / PNG file's bytes (PNG decoded by the host reader first).
+py::array_t<uint8_t> DebugDecodeGrey(b2m_ctx* ctx, const py::bytes& file, int max_image_size) {
+  const std::string buf = file;
+  const std::vector<uint8_t> bytes(buf.begin(), buf.end());
+  ImageHeader h;
+  std::string why;
+  if (!ReadImageHeader(bytes, &h, &why)) throw std::invalid_argument("[bindings.cc] " + why);
+  b2m_image_source s;
+  std::memset(&s, 0, sizeof(s));
+  Pixels px;
+  if (h.format == ImageFormat::PNG) {
+    if (!DecodePng(bytes, &px, &why)) throw std::invalid_argument("[bindings.cc] " + why);
+    s.kind = B2M_SOURCE_PIXELS;
+    s.channels = px.channels;
+    s.width = px.width;
+    s.height = px.height;
+    s.stride = static_cast<int64_t>(px.width) * px.channels;
+    s.data = px.data.data();
+  } else {
+    s.kind = B2M_SOURCE_JPEG;
+    s.data = bytes.data();
+    s.size = static_cast<int64_t>(bytes.size());
+  }
+  const auto decode = SiftSymbol<decltype(&b2m_debug_decode_grey)>("b2m_debug_decode_grey");
+  int32_t w = 0, hh = 0;
+  ThrowOnError(ctx, decode(ctx, &s, max_image_size, nullptr, &w, &hh));
+  py::array_t<uint8_t> out(std::vector<py::ssize_t>{hh, w});
+  ThrowOnError(ctx, decode(ctx, &s, max_image_size, out.mutable_data(), &w, &hh));
+  return out;
+}
+
+// ---- feature extraction from image files (R:pycolmap/pipeline/extract_features.h:23-61, images.h:24-94) ------------
+// THROW_CHECK_MSG's message (R:log_exceptions.h): "[file:line] Check Failed: <expression> : <message>"
+[[noreturn]] void CheckFailed(const char* where, const std::string& expr, const std::string& msg) {
+  throw std::invalid_argument(std::string("[") + where + "] Check Failed: " + expr + (msg.empty() ? "" : " : " + msg));
+}
+
+bool IsDir(const std::string& p) {
+  std::error_code ec;
+  return std::filesystem::is_directory(p, ec);
+}
+
+bool IsFile(const std::string& p) {
+  std::error_code ec;
+  return std::filesystem::is_regular_file(p, ec);
+}
+
+// Bitmap::Read(path, false) of a mask: grey pixels, or false when the file is not a PNG this reader decodes.
+bool ReadMask(const std::string& path, Pixels* grey, std::string* why) {
+  Pixels px;
+  if (!DecodePng(ReadFileBytes(path), &px, why)) return false;
+  grey->width = px.width;
+  grey->height = px.height;
+  grey->channels = 1;
+  grey->data = ToGrey(px);
+  return true;
+}
+
+// A keypoint passes both masks iff it lies inside both and both are nonzero there: the mask over the common extent.
+Pixels MaskAnd(const Pixels& a, const Pixels& b) {
+  Pixels m;
+  m.width = std::min(a.width, b.width);
+  m.height = std::min(a.height, b.height);
+  m.channels = 1;
+  m.data.resize(static_cast<size_t>(m.width) * m.height);
+  for (int y = 0; y < m.height; ++y)
+    for (int x = 0; x < m.width; ++x)
+      m.data[static_cast<size_t>(y) * m.width + x] =
+          a.data[static_cast<size_t>(y) * a.width + x] && b.data[static_cast<size_t>(y) * b.width + x] ? 255 : 0;
+  return m;
+}
+
+// One image between the reader thread and the device: the file, its decoded PNG pixels, its mask.
+struct Loaded {
+  ImageReader::Item item;
+  Pixels pixels;  // PNG only
+  Pixels mask;    // mask_path/<name>.png when it exists
+  bool has_mask = false;
+};
+
+// Images per device call, and the host bytes (files, PNG pixels, masks) one call may hold: the reader runs one call
+// ahead and the writer one call behind, so at most three calls' worth is in memory.
+constexpr size_t kExtractBatch = 32;
+constexpr size_t kExtractBatchBytes = size_t(256) << 20;
+
+// File reading, PNG decoding and mask reading of images [begin, end) up to the byte budget; touches no database.
+std::vector<Loaded> LoadBatch(const ImageReader& reader, const ImageReaderOptions& ro, size_t begin, size_t* end) {
+  std::vector<Loaded> out;
+  size_t bytes = 0;
+  size_t i = begin;
+  for (; i < reader.NumImages() && out.size() < kExtractBatch && (out.empty() || bytes < kExtractBatchBytes); ++i) {
+    Loaded l;
+    reader.Load(i, &l.item);
+    try {
+      if (l.item.error.empty() && l.item.header.format == ImageFormat::PNG && !DecodePng(l.item.bytes, &l.pixels, &l.item.error))
+        l.item.bytes.clear();
+      if (l.item.error.empty() && !ro.mask_path.empty()) {
+        const std::string mp = (std::filesystem::path(ro.mask_path) / (l.item.name + ".png")).string();
+        std::string why;
+        if (IsFile(mp)) {
+          if (ReadMask(mp, &l.mask, &why)) l.has_mask = true;
+          else l.item.error = "mask " + mp + ": " + why;
+        }
+      }
+    } catch (const std::exception& e) {  // out of host memory for one file's pixels: that file is skipped
+      l.item.error = std::string("cannot decode it: ") + e.what();
+      l.pixels = Pixels();
+      l.mask = Pixels();
+      l.has_mask = false;
+    }
+    bytes += l.item.bytes.size() + l.pixels.data.size() + l.mask.data.size();
+    out.push_back(std::move(l));
+  }
+  *end = i;
+  return out;
+}
+
+// One device call's worth: the loaded images, the sources handed to the device (index into `batch` in `which`) and,
+// once the call returned, its features.
+struct Call {
+  std::vector<Loaded> batch;
+  std::vector<b2m_image_source> src;
+  std::vector<size_t> which;
+  std::vector<Pixels> masks;
+  std::shared_ptr<b2m_features> features;
+};
+
+// ImageReader::Assign over a loaded batch (cameras go to the database here), and the device sources of the images
+// that pass.
+void AssignBatch(ImageReader& reader, const Pixels& camera_mask, Call* c) {
+  c->masks.resize(c->batch.size());
+  for (size_t k = 0; k < c->batch.size(); ++k) {
+    Loaded& l = c->batch[k];
+    if (reader.Assign(&l.item) != ImageReader::Status::SUCCESS) continue;
+    b2m_image_source s;
+    std::memset(&s, 0, sizeof(s));
+    if (l.item.header.format == ImageFormat::JPEG) {
+      s.kind = B2M_SOURCE_JPEG;
+      s.data = l.item.bytes.data();
+      s.size = static_cast<int64_t>(l.item.bytes.size());
+    } else {
+      s.kind = B2M_SOURCE_PIXELS;
+      s.channels = l.pixels.channels;
+      s.width = l.pixels.width;
+      s.height = l.pixels.height;
+      s.stride = static_cast<int64_t>(l.pixels.width) * l.pixels.channels;
+      s.data = l.pixels.data.data();
+    }
+    const Pixels* m = nullptr;
+    if (l.has_mask && !camera_mask.data.empty()) m = &(c->masks[k] = MaskAnd(l.mask, camera_mask));
+    else if (l.has_mask) m = &l.mask;
+    else if (!camera_mask.data.empty()) m = &camera_mask;
+    if (m) {
+      s.mask = m->data.data();
+      s.mask_width = m->width;
+      s.mask_height = m->height;
+      s.mask_stride = m->width;
+    }
+    c->src.push_back(s);
+    c->which.push_back(k);
+  }
+}
+
+// The images, keypoints and descriptors of one call, in one transaction; a source the device could not decode is
+// skipped with a warning.
+void WriteCall(Database& db, const Call& c, decltype(&b2m_source_features_get) get) {
+  DatabaseTransaction txn(&db);
+  for (size_t j = 0; j < c.src.size(); ++j) {
+    const ImageReader::Item& it = c.batch[c.which[j]].item;
+    b2m_source_view v;
+    std::memset(&v, 0, sizeof(v));
+    if (get(c.features.get(), static_cast<int32_t>(j), &v) != B2M_OK)
+      throw std::runtime_error("[bindings.cc] b2m_source_features_get failed for " + it.name);
+    if (v.status != B2M_OK) {
+      ImageReader::Warn(it.name, v.error && *v.error ? v.error : "does not decode");
+      continue;
+    }
+    if (v.width != it.camera.width || v.height != it.camera.height) {
+      ImageReader::Warn(it.name, "decodes to a size other than its header's");
+      continue;
+    }
+    const int64_t id = db.AddImage(it.name, it.camera.camera_id);
+    db.WriteKeypoints(id, v.keypoints, v.n, 6);
+    db.WriteDescriptors(id, v.descriptors, v.n, 128);
+  }
+}
+
+// Three stages, as MatchPairsIntoDb has: a reader thread loads call k + 1 (files, PNG, masks), the device runs call k
+// (decode, grey, rescale and SIFT; inside it the decoder runs ahead of SIFT), and a writer thread commits call k - 1.
+// The database sees one thread at a time: cameras of call k + 1 are assigned after the writer of call k - 1 is done
+// and before the writer of call k starts.
+void ExtractFeaturesRun(const std::string& database_path, const std::string& image_path,
+                        const std::vector<std::string>& image_list, CameraMode mode, const ImageReaderOptions& ro,
+                        const SiftExtractionOptions& so, int dev) {
+  const auto extract = SiftSymbol<decltype(&b2m_extract_features_sources)>("b2m_extract_features_sources");
+  const auto get = SiftSymbol<decltype(&b2m_source_features_get)>("b2m_source_features_get");
+  const auto release = SiftSymbol<decltype(&b2m_features_free)>("b2m_features_free");
+  Pixels camera_mask;
+  if (!ro.camera_mask_path.empty()) {
+    std::string why;
+    if (!ReadMask(ro.camera_mask_path, &camera_mask, &why)) {  // FeatureExtractorController: go on without the mask
+      fprintf(stderr, "E [bindings.cc] Cannot read camera mask file: %s (%s). No mask is going to be used.\n",
+              ro.camera_mask_path.c_str(), why.c_str());
+      camera_mask = Pixels();
+    }
+  }
+  b2m_ctx* ctx = Engine::Get(dev);
+  const b2m_extract_opts opts = ToAbi(so);
+  Database db(database_path);
+  ImageReader reader(ro, mode, image_path, image_list, &db);
+  size_t next = 0;
+  auto cur = std::make_unique<Call>();
+  cur->batch = LoadBatch(reader, ro, 0, &next);
+  AssignBatch(reader, camera_mask, cur.get());
+  std::future<void> writer;
+  std::future<std::vector<Loaded>> ahead;
+  auto drain = [&] {  // leaves no thread behind when an exception unwinds
+    if (ahead.valid()) ahead.wait();
+    if (writer.valid()) writer.wait();
+  };
+  try {
+    while (!cur->batch.empty()) {
+      ahead = std::async(std::launch::async, [&, begin = next] { return LoadBatch(reader, ro, begin, &next); });
+      b2m_features* f = nullptr;
+      if (!cur->src.empty()) ThrowOnError(ctx, extract(ctx, cur->src.data(), static_cast<int32_t>(cur->src.size()), &opts, &f));
+      cur->features.reset(f, release);
+      auto following = std::make_unique<Call>();
+      following->batch = ahead.get();
+      if (writer.valid()) writer.get();
+      AssignBatch(reader, camera_mask, following.get());
+      writer = std::async(std::launch::async, [&db, get, c = std::shared_ptr<Call>(std::move(cur))] {
+        if (c->features) WriteCall(db, *c, get);
+      });
+      cur = std::move(following);
+    }
+    if (writer.valid()) writer.get();
+  } catch (...) {
+    drain();
+    throw;
+  }
+}
+
+void CheckCameraMode(const ImageReaderOptions& o, const char* where) {
+  if (CameraModelId(o.camera_model) < 0)
+    throw std::invalid_argument(std::string("[") + where + "] Invalid camera model: " + o.camera_model);
+}
 }  // namespace
 
 PYBIND11_MODULE(_core, m) {
@@ -1272,6 +1523,119 @@ PYBIND11_MODULE(_core, m) {
             "The device the extractor runs on, resolved like upstream's Sift::GetDevice (use_gpu ? CUDA : CPU): always "
             "Device.cuda, since Device.auto resolves to the GPU and Device.cpu is refused.");
   }
+  // ---- feature extraction from image files ----
+  auto camera_mode = py::enum_<CameraMode>(m, "CameraMode")
+                         .value("AUTO", CameraMode::AUTO)
+                         .value("SINGLE", CameraMode::SINGLE)
+                         .value("PER_FOLDER", CameraMode::PER_FOLDER)
+                         .value("PER_IMAGE", CameraMode::PER_IMAGE);
+  AddStringConstructor(camera_mode);
+  OptionsClass<ImageReaderOptions>(m, "ImageReaderOptions")
+      .field("camera_model", &ImageReaderOptions::camera_model, "Name of the camera model.")
+      .field("mask_path", &ImageReaderOptions::mask_path,
+             "Optional root path to folder which contains image masks: the mask of image_path/abc/012.jpg is "
+             "mask_path/abc/012.jpg.png.  No features are kept where the mask is black (grey value 0).")
+      .field("existing_camera_id", &ImageReaderOptions::existing_camera_id,
+             "Use this existing camera for all images (the camera model and parameters are then ignored).")
+      .field("camera_params", &ImageReaderOptions::camera_params,
+             "Manual specification of camera parameters.  If empty, they come from EXIF (focal length) and the "
+             "image size (principal point).")
+      .field("default_focal_length_factor", &ImageReaderOptions::default_focal_length_factor,
+             "Without manual parameters or an EXIF focal length, the focal length is "
+             "default_focal_length_factor * max(width, height).")
+      .field("camera_mask_path", &ImageReaderOptions::camera_mask_path,
+             "Optional mask for all images: no features are kept where it is black (grey value 0).")
+      .Finish();
+  {
+    SiftExtractionOptions cxx_defaults;  // the C++ constructor's (R:pipeline/extract_features.h:140), not Sift()'s
+    m.def("extract_features",
+          [](const py::object& database_path, const py::object& image_path, const std::vector<std::string>& image_list,
+             CameraMode camera_mode, const std::string& camera_model, ImageReaderOptions reader_options,
+             const SiftExtractionOptions& sift_options, Device device) {
+            const std::string db = FsPath(database_path), images = FsPath(image_path);
+            if (std::filesystem::exists(db)) CheckFailed("extract_features.h:31", "!ExistsFile(database_path)", db + " already exists.");
+            if (!(db.size() >= 3 && db.compare(db.size() - 3, 3, ".db") == 0))
+              CheckFailed("extract_features.h:33", "HasFileExtension(database_path, \".db\")",
+                          "Path " + db + " does not match file extension .db.");
+            if (!std::ofstream(db, std::ios::trunc).is_open())
+              CheckFailed("extract_features.h:34", "std::ofstream(database_path, std::ios::trunc).is_open()",
+                          ": Could not open " + db + ". Is the path a directory or does the parent dir not exist?");
+            if (!IsDir(images)) CheckFailed("extract_features.h:35", "ExistsDir(image_path)", "Directory " + images + " does not exist.");
+            const int dev = SiftDevice(device, sift_options);
+            reader_options.camera_model = camera_model;
+            if (CameraModelId(camera_model) < 0)
+              CheckFailed("extract_features.h:49", "ExistsCameraModelWithName(reader_options.camera_model)", "");
+            if (!VerifyCameraParams(camera_model, reader_options.camera_params))
+              throw std::invalid_argument("[extract_features.h:51] Invalid camera parameters.");
+            CheckSiftOptions(sift_options);
+            RunInterruptible([&] { ExtractFeaturesRun(db, images, image_list, camera_mode, reader_options, sift_options, dev); });
+          },
+          "database_path"_a, "image_path"_a, "image_list"_a = std::vector<std::string>(), "camera_mode"_a = CameraMode::AUTO,
+          "camera_model"_a = "SIMPLE_RADIAL", "reader_options"_a = ImageReaderOptions(), "sift_options"_a = cxx_defaults,
+          "device"_a = Device::AUTO,
+          "Extract SIFT features of the JPEG / PNG files under image_path and write cameras, images, keypoints and "
+          "descriptors to a new database");
+  }
+  m.def("debug_decode_grey",
+        [](const py::bytes& file, int max_image_size, int device) { return DebugDecodeGrey(Engine::Get(device), file, max_image_size); },
+        "file"_a, "max_image_size"_a = 3200, "device"_a = 0,
+        "Instrumentation: the grey image extract_features feeds to SIFT for this JPEG / PNG file's bytes (decoded on "
+        "the device, downscaled when larger than max_image_size)");
+  m.def("debug_decode_png",
+        [](const py::bytes& file) {
+          const std::string buf = file;
+          Pixels px;
+          std::string why;
+          if (!DecodePng(std::vector<uint8_t>(buf.begin(), buf.end()), &px, &why)) throw std::invalid_argument("[bindings.cc] " + why);
+          py::array_t<uint8_t> out(std::vector<py::ssize_t>{px.height, px.width, px.channels});
+          std::memcpy(out.mutable_data(), px.data.data(), px.data.size());
+          return out;
+        },
+        "file"_a,
+        "Instrumentation: the pixels extract_features' host PNG decoder gives for a PNG file's bytes, (H, W, C) with C = 1 "
+        "(grey, grey + alpha), 3 (RGB, palette) or 4 (RGBA)");
+  m.def("import_images",
+        [](const py::object& database_path, const py::object& image_path, CameraMode camera_mode,
+           const std::vector<std::string>& image_list, const ImageReaderOptions& options) {
+          const std::string db_path = FsPath(database_path), images = FsPath(image_path);
+          if (!IsFile(db_path)) CheckFailed("images.h:29", "ExistsFile(database_path)", "File " + db_path + " does not exist.");
+          if (!IsDir(images)) CheckFailed("images.h:30", "ExistsDir(image_path)", "Directory " + images + " does not exist.");
+          CheckCameraMode(options, "images.h:37");
+          Database db(db_path);
+          ImageReader reader(options, camera_mode, images, image_list, &db);
+          for (size_t i = 0; i < reader.NumImages(); ++i) {
+            if (PyErr_CheckSignals() != 0) throw py::error_already_set();
+            ImageReader::Item item;
+            reader.Load(i, &item);
+            DatabaseTransaction txn(&db);
+            if (reader.Assign(&item) == ImageReader::Status::SUCCESS) db.AddImage(item.name, item.camera.camera_id);
+          }
+        },
+        "database_path"_a, "image_path"_a, "camera_mode"_a = CameraMode::AUTO, "image_list"_a = std::vector<std::string>(),
+        "options"_a = ImageReaderOptions(),
+        "Write a camera and an image row for every JPEG / PNG file under image_path (images already in the database "
+        "are skipped)");
+  m.def("infer_camera_from_image",
+        [](const py::object& image_path, const ImageReaderOptions& options) {
+          const std::string path = FsPath(image_path);
+          if (!IsFile(path)) CheckFailed("images.h:67", "ExistsFile(image_path)", "File " + path + " does not exist.");
+          ImageHeader h;
+          std::string why;
+          if (!ReadImageHeader(ReadFileBytes(path), &h, &why))
+            throw std::invalid_argument("[images.h:70] Cannot read image file: " + path);
+          CheckCameraMode(options, "images.h:76");
+          CameraRow c;
+          c.model = CameraModelId(options.camera_model);
+          c.width = h.width;
+          c.height = h.height;
+          c.has_prior_focal_length = h.has_focal;
+          const double f = h.has_focal ? h.focal : options.default_focal_length_factor * std::max(h.width, h.height);
+          c.params = InitialCameraParams(c.model, f, h.width, h.height);
+          return CameraToDict(c);
+        },
+        "image_path"_a, "options"_a = ImageReaderOptions(),
+        "The camera ImageReader would create for this image: a dict {model, width, height, params, "
+        "has_prior_focal_length}");
   m.def("fundamental_matrix_estimation",
         [](const ArrD& points1, const ArrD& points2, const RANSACOptions& estimation_options) {
           CheckSameLength(points1, points2, "fundamental_matrix.h:22");
@@ -1787,6 +2151,9 @@ PYBIND11_MODULE(_core, m) {
              return py::make_tuple(models, counts);
            },
            "nullspaces"_a, "The device 5-point solver (one warp per 4-D null space): (models [n, 10, 9], counts [n])")
+      .def("debug_decode_grey",
+           [](CoreContext& c, const py::bytes& file, int max_image_size) { return DebugDecodeGrey(c.Handle(), file, max_image_size); },
+           "file"_a, "max_image_size"_a = 3200, "pycolmap_b200.debug_decode_grey on this context")
       .def("stats", [](CoreContext& c) {
         b2m_stats s;
         memset(&s, 0, sizeof(s));
@@ -1805,7 +2172,9 @@ PYBIND11_MODULE(_core, m) {
                         "comm_size"_a = s.comm_size, "comm_rank"_a = s.comm_rank,
                         "tri_models_scored"_a = s.tri_models_scored, "tri_residuals"_a = s.tri_residuals,
                         "sift_images"_a = s.sift_images, "sift_keypoints"_a = s.sift_keypoints,
-                        "sift_descriptors"_a = s.sift_descriptors);
+                        "sift_descriptors"_a = s.sift_descriptors, "sift_decoded_bytes"_a = s.sift_decoded_bytes,
+                        "sift_decode_images"_a = s.sift_decode_images,
+                        "sift_decode_hardware"_a = s.sift_decode_hardware);
       })
       .def("reset_stats", [](CoreContext& c) { ThrowOnError(c.Handle(), b2m_reset_stats(c.Handle()));
       });
