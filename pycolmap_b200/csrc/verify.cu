@@ -1429,51 +1429,81 @@ void verify_release(b2m_ctx* ctx) {
 }
 
 // ---- stand-alone estimators ------------------------------------------------------------------
+// A single problem is a batch of one: staged as images (0, 1), it is keyed like problem 0 of a batch and draws the
+// same RANSAC samples.
 
 namespace {
 
-struct Single {
+// The device arrays of one stand-alone call over `nb` problems.
+struct StandaloneBatch {
+  // Offsets of the per-problem scalars in d_i32: pairs[2nb] cnt[nb] sup[3nb] success[3nb] config[nb] inl_cnt[nb]
+  struct Scalars {
+    int64_t pairs, cnt, sup, success, config, inl_cnt, size;
+    explicit Scalars(int64_t nb)
+        : pairs(0), cnt(2 * nb), sup(cnt + nb), success(sup + 3 * nb), config(success + 3 * nb), inl_cnt(config + nb),
+          size(inl_cnt + nb) {}
+  };
+
   DeviceArray<double4> d_pts;
   DeviceArray<uint2> d_matches;
   DeviceArray<uint2> d_inliers;
   DeviceArray<uint8_t> d_mask;
   DeviceArray<DevCamera> d_cams;
-  DeviceArray<int32_t> d_i32;   // pairs[2], cnt[1], sup[3], success[3], config[1], inl_cnt[1]
+  DeviceArray<int32_t> d_i32;   // laid out by Scalars
   DeviceArray<int64_t> d_off;
   DeviceArray<double> d_models;
   DeviceArray<DevDistortion> d_dist;  // only when a camera has distortion
   DeviceArray<double4> d_pts_undist;
-  DeviceArray<double> d_e_scratch;    // E kernel scratch, [problems][128][90]
+  DeviceArray<double> d_e_scratch;    // E kernel scratch, [problems][kRansacThreads][kEStride]
   // compute_relative_pose
   DeviceArray<double> d_p1, d_p2, d_angles, d_pose;
   DeviceArray<int64_t> d_p1_off, d_p2_off;
   DeviceArray<int32_t> d_pose_valid;
+  int64_t n_matches = 0;  // staged, over all problems
+
+  // The kernels' view of these arrays for `nb` problems in arenas of `cap` matches
+  VerifyParams params(int nb, int64_t cap) const {
+    const Scalars L(nb);
+    VerifyParams P{};
+    P.pairs = d_i32 + L.pairs;
+    P.pair_cnt = d_i32 + L.cnt;
+    P.sup_cnt = d_i32 + L.sup;
+    P.success = d_i32 + L.success;
+    P.config = d_i32 + L.config;
+    P.inl_cnt = d_i32 + L.inl_cnt;
+    P.pair_off = d_off;
+    P.pts = d_pts;
+    P.matches = d_matches;
+    P.cams = d_cams;
+    P.mask = d_mask;
+    P.arena_cap = cap;
+    P.models = d_models;
+    P.inliers = d_inliers;
+    P.e_scratch = d_e_scratch;
+    return P;
+  }
 };
 
-// Stand-alone estimator calls with compute_relative_pose: upload the callers' point arrays (concatenated over the
-// `nb` problems, offsets in points) and run the pose kernel after the decision kernel.  `P` is the VerifyParams the
-// RANSAC / decision kernels ran with; G.d_dist may be null (no distortion).  Outputs stay in G.d_pose / d_pose_valid.
-int launch_pose_standalone(b2m_ctx* ctx, Single& G, const VerifyParams& P, int nb, int64_t cap, const std::vector<double>& p1,
-                           const std::vector<double>& p2, const std::vector<int64_t>& off1, const std::vector<int64_t>& off2,
-                           const b2m_camera* const* cams, int n_cams, cudaStream_t st) {
+// Stand-alone estimator calls with compute_relative_pose: upload the point arrays of problems[0, nb) and run the pose
+// kernel after the decision kernel.  `P` is the VerifyParams the RANSAC / decision kernels ran with; G.d_dist may be
+// null (no distortion).  Outputs stay in G.d_pose / d_pose_valid.
+int launch_pose_standalone(b2m_ctx* ctx, StandaloneBatch& G, const VerifyParams& P, const b2m_tvg_problem* problems, int nb) {
+  std::vector<double> p1, p2;  // the callers' point arrays, concatenated
+  std::vector<int64_t> off1(nb), off2(nb);
+  for (int k = 0; k < nb; ++k) {
+    const b2m_tvg_problem& q = problems[k];
+    off1[k] = static_cast<int64_t>(p1.size() / 2);
+    off2[k] = static_cast<int64_t>(p2.size() / 2);
+    p1.insert(p1.end(), q.points1, q.points1 + 2 * q.n1);
+    p2.insert(p2.end(), q.points2, q.points2 + 2 * q.n2);
+  }
   B2M_CUDA_TRY(ctx, G.d_p1.ensure(std::max<size_t>(p1.size(), 2)));
   B2M_CUDA_TRY(ctx, G.d_p2.ensure(std::max<size_t>(p2.size(), 2)));
   B2M_CUDA_TRY(ctx, G.d_p1_off.ensure(nb));
   B2M_CUDA_TRY(ctx, G.d_p2_off.ensure(nb));
-  B2M_CUDA_TRY(ctx, G.d_angles.ensure(cap));
+  B2M_CUDA_TRY(ctx, G.d_angles.ensure(P.arena_cap));
   B2M_CUDA_TRY(ctx, G.d_pose.ensure(8 * nb));
   B2M_CUDA_TRY(ctx, G.d_pose_valid.ensure(nb));
-  if (!G.d_dist) {  // undistort_for_E uploads the models only when it had to; the pose kernel needs them as well
-    bool any = false;
-    for (int i = 0; i < n_cams; ++i) any = any || cam::has_distortion(cams[i]->model);
-    if (any) {
-      std::vector<DevDistortion> dd(n_cams);
-      for (int i = 0; i < n_cams; ++i) dd[i] = to_dist(*cams[i]);
-      B2M_CUDA_TRY(ctx, G.d_dist.ensure(n_cams));
-      B2M_CUDA_TRY(ctx, cudaMemcpy(G.d_dist, dd.data(), sizeof(DevDistortion) * n_cams, cudaMemcpyHostToDevice));
-    }
-  }
-  // synchronous copies: the host vectors are the caller's locals
   if (!p1.empty()) B2M_CUDA_TRY(ctx, cudaMemcpy(G.d_p1, p1.data(), sizeof(double) * p1.size(), cudaMemcpyHostToDevice));
   if (!p2.empty()) B2M_CUDA_TRY(ctx, cudaMemcpy(G.d_p2, p2.data(), sizeof(double) * p2.size(), cudaMemcpyHostToDevice));
   B2M_CUDA_TRY(ctx, cudaMemcpy(G.d_p1_off, off1.data(), sizeof(int64_t) * nb, cudaMemcpyHostToDevice));
@@ -1494,112 +1524,152 @@ int launch_pose_standalone(b2m_ctx* ctx, Single& G, const VerifyParams& P, int n
   Q.angles = G.d_angles;
   Q.out = G.d_pose;
   Q.out_valid = G.d_pose_valid;
-  b2m_pose_kernel<<<nb, 256, 0, st>>>(Q);
+  b2m_pose_kernel<<<nb, 256, 0, ctx->stream>>>(Q);
   B2M_CUDA_TRY(ctx, cudaGetLastError());
   ctx->stats.kernel_launches += 1;
   return B2M_OK;
 }
 
-// copy the pose of problem k (device arrays already downloaded into h_pose / h_valid) into a result
-void fill_pose(b2m_tvg_result* r, const double* h_pose, const int32_t* h_valid, int k) {
-  r->qvec[0] = 1.0;
-  if (h_pose && h_valid && h_valid[k] && r->n_inliers > 0) {
-    memcpy(r->qvec, h_pose + 8 * k, sizeof(double) * 4);
-    memcpy(r->tvec, h_pose + 8 * k + 4, sizeof(double) * 3);
-    r->tri_angle = h_pose[8 * k + 7];
-    r->pose_valid = 1;
-  }
+// copy a pose downloaded from G.d_pose (qvec, tvec, tri_angle) into a result; an invalid one as identity and angle 0
+void fill_pose(b2m_tvg_result* r, const double* h_pose, bool valid) {
+  static const double kIdentity[8] = {1, 0, 0, 0, 0, 0, 0, 0};
+  const double* p = valid ? h_pose : kIdentity;
+  memcpy(r->qvec, p, sizeof(double) * 4);
+  memcpy(r->tvec, p + 4, sizeof(double) * 3);
+  r->tri_angle = p[7];
+  r->pose_valid = valid ? 1 : 0;
 }
 
-// Stand-alone estimator calls: upload the full camera models and undistort the E-kernel input when any
-// of the `n_cams` cameras has a distortion function.  Returns the E arena (nullptr: use P.pts) in *pts_E.
-int undistort_for_E(b2m_ctx* ctx, Single& G, const VerifyParams& P, const b2m_camera* const* cams, int n_cams, int nb,
-                    int64_t cap, cudaStream_t st, const double4** pts_E) {
-  *pts_E = nullptr;
+// Uploads the full models of the cameras of problems[0, nb) into G.d_dist when any of them has a distortion function,
+// for the undistortion of the E input and for the pose kernel.  G.d_dist stays null otherwise.
+int upload_distortion(b2m_ctx* ctx, StandaloneBatch& G, const b2m_tvg_problem* problems, int nb) {
   bool any = false;
-  for (int i = 0; i < n_cams; ++i) any = any || cam::has_distortion(cams[i]->model);
+  for (int k = 0; k < nb; ++k)
+    any = any || cam::has_distortion(problems[k].cam1.model) || cam::has_distortion(problems[k].cam2.model);
   if (!any) return B2M_OK;
-  std::vector<DevDistortion> dd(n_cams);
-  for (int i = 0; i < n_cams; ++i) dd[i] = to_dist(*cams[i]);
-  B2M_CUDA_TRY(ctx, G.d_dist.ensure(n_cams));
-  B2M_CUDA_TRY(ctx, G.d_pts_undist.ensure(cap));
-  // synchronous copy: `dd` is a local that must not be read after this function returns
-  B2M_CUDA_TRY(ctx, cudaMemcpy(G.d_dist, dd.data(), sizeof(DevDistortion) * n_cams, cudaMemcpyHostToDevice));
-  b2m_undistort_kernel<<<nb, 256, 0, st>>>(P, G.d_dist, G.d_pts_undist);
-  B2M_CUDA_TRY(ctx, cudaGetLastError());
-  ctx->stats.kernel_launches += 1;
-  *pts_E = G.d_pts_undist;
+  std::vector<DevDistortion> dd(2 * nb);
+  for (int k = 0; k < nb; ++k) {
+    dd[2 * k] = to_dist(problems[k].cam1);
+    dd[2 * k + 1] = to_dist(problems[k].cam2);
+  }
+  B2M_CUDA_TRY(ctx, G.d_dist.ensure(2 * nb));
+  B2M_CUDA_TRY(ctx, cudaMemcpy(G.d_dist, dd.data(), sizeof(DevDistortion) * 2 * nb, cudaMemcpyHostToDevice));
   return B2M_OK;
 }
 
-// `full_cams`: the two cameras with their distortion parameters, or nullptr (single-model API: the
-// caller's points are already in the frame the model is estimated in).
-int run_single(b2m_ctx* ctx, const std::vector<double4>& pts, const std::vector<uint2>& matches, const DevCamera cams[2],
-               const b2m_tvg_opts& opt, int single_kind, Single& G, VerifyParams& P,
-               const b2m_camera* const* full_cams = nullptr, const double* raw1 = nullptr, int64_t n1 = 0,
-               const double* raw2 = nullptr, int64_t n2 = 0) {
-  const int64_t m = static_cast<int64_t>(pts.size());
-  const int64_t cap = std::max<int64_t>(m, 1);
+// Stages problems[0, nb) (at most one chunk, arguments checked) into G as images (2k, 2k + 1) and returns in *P the
+// VerifyParams the kernels run with.  single_kind >= 0: only that model kind is estimated.
+int stage(b2m_ctx* ctx, const b2m_tvg_problem* problems, int nb, const b2m_tvg_opts& opt, int single_kind,
+          StandaloneBatch& G, VerifyParams* P) {
+  const StandaloneBatch::Scalars L(nb);
+  std::vector<double4> pts;
+  std::vector<uint2> mm;
+  std::vector<int64_t> off(nb);
+  std::vector<int32_t> i32(L.size, 0);
+  std::vector<DevCamera> cams(2 * nb);
+  for (int k = 0; k < nb; ++k) {
+    const b2m_tvg_problem& q = problems[k];
+    const int64_t m = q.matches ? q.m : q.n1;
+    off[k] = static_cast<int64_t>(pts.size());
+    i32[L.pairs + 2 * k] = 2 * k;
+    i32[L.pairs + 2 * k + 1] = 2 * k + 1;
+    i32[L.cnt + k] = static_cast<int32_t>(m);
+    cams[2 * k] = to_dev(q.cam1);
+    cams[2 * k + 1] = to_dev(q.cam2);
+    for (int64_t i = 0; i < m; ++i) {
+      const uint32_t a = q.matches ? q.matches[2 * i] : static_cast<uint32_t>(i);
+      const uint32_t b = q.matches ? q.matches[2 * i + 1] : static_cast<uint32_t>(i);
+      if (a >= q.n1 || b >= q.n2) return fail(ctx, B2M_EINVAL, "[verify.cu] Check Failed: match index < number of points");
+      pts.push_back(make_double4(q.points1[2 * a], q.points1[2 * a + 1], q.points2[2 * b], q.points2[2 * b + 1]));
+      mm.push_back(make_uint2(a, b));
+    }
+  }
+  const int64_t total = static_cast<int64_t>(pts.size());
+  const int64_t cap = std::max<int64_t>(total, 1);
   B2M_CUDA_TRY(ctx, G.d_pts.ensure(cap));
   B2M_CUDA_TRY(ctx, G.d_matches.ensure(cap));
   B2M_CUDA_TRY(ctx, G.d_inliers.ensure(cap));
   B2M_CUDA_TRY(ctx, G.d_mask.ensure(3 * cap));
-  B2M_CUDA_TRY(ctx, G.d_cams.ensure(2));
-  B2M_CUDA_TRY(ctx, G.d_i32.ensure(16));
-  B2M_CUDA_TRY(ctx, G.d_off.ensure(1));
-  B2M_CUDA_TRY(ctx, G.d_models.ensure(27));
-  B2M_CUDA_TRY(ctx, G.d_e_scratch.ensure(static_cast<size_t>(kEStride) * kRansacThreads));
-  const int32_t i32[16] = {0, 1, static_cast<int32_t>(m), 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
-  const int64_t off0 = 0;
+  B2M_CUDA_TRY(ctx, G.d_cams.ensure(2 * nb));
+  B2M_CUDA_TRY(ctx, G.d_i32.ensure(L.size));
+  B2M_CUDA_TRY(ctx, G.d_off.ensure(nb));
+  B2M_CUDA_TRY(ctx, G.d_models.ensure(27 * nb));
+  B2M_CUDA_TRY(ctx, G.d_e_scratch.ensure(static_cast<size_t>(kEStride) * kRansacThreads * nb));
+  // an asynchronous copy from pageable memory returns once its source is staged: the host vectors may go out of scope
   cudaStream_t st = ctx->stream;
-  if (m > 0) {
-    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(G.d_pts, pts.data(), sizeof(double4) * m, cudaMemcpyHostToDevice, st));
-    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(G.d_matches, matches.data(), sizeof(uint2) * m, cudaMemcpyHostToDevice, st));
+  if (total > 0) {
+    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(G.d_pts, pts.data(), sizeof(double4) * total, cudaMemcpyHostToDevice, st));
+    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(G.d_matches, mm.data(), sizeof(uint2) * total, cudaMemcpyHostToDevice, st));
   }
-  B2M_CUDA_TRY(ctx, cudaMemcpyAsync(G.d_cams, cams, sizeof(DevCamera) * 2, cudaMemcpyHostToDevice, st));
-  B2M_CUDA_TRY(ctx, cudaMemcpyAsync(G.d_i32, i32, sizeof(i32), cudaMemcpyHostToDevice, st));
-  B2M_CUDA_TRY(ctx, cudaMemcpyAsync(G.d_off, &off0, sizeof(int64_t), cudaMemcpyHostToDevice, st));
-  B2M_CUDA_TRY(ctx, cudaMemsetAsync(G.d_models, 0, sizeof(double) * 27, st));
-  P = VerifyParams{};
-  P.pairs = G.d_i32;
-  P.pair_cnt = G.d_i32 + 2;
-  P.sup_cnt = G.d_i32 + 3;
-  P.success = G.d_i32 + 6;
-  P.config = G.d_i32 + 9;
-  P.inl_cnt = G.d_i32 + 10;
-  P.pair_off = G.d_off;
-  P.pts = G.d_pts;
-  P.matches = G.d_matches;
-  P.cams = G.d_cams;
-  P.mask = G.d_mask;
-  P.arena_cap = cap;
-  P.models = G.d_models;
-  P.inliers = G.d_inliers;
-  P.opt = opt;
-  P.seed = ctx->seed;
-  P.single_kind = single_kind;
-  P.counters = ctx->d_counters + kVerifyCounters;
-  P.e_scratch = G.d_e_scratch;
-  P.lo_eig_thread = lo_eig_thread_mode();
-  if (single_kind >= 0) {
-    B2M_CUDA_TRY(ctx, launch_ransac(P, 1, st));
-  } else {
-    const double4* pts_E = nullptr;
-    if (full_cams)
-      if (int rc = undistort_for_E(ctx, G, P, full_cams, 2, 1, cap, st, &pts_E)) return rc;
-    B2M_CUDA_TRY(ctx, launch_ransac(P, 1, st, nullptr, pts_E));
-    ctx->stats.kernel_launches += 2;
-    b2m_decide_kernel<<<1, 256, 0, st>>>(P);
+  B2M_CUDA_TRY(ctx, cudaMemcpyAsync(G.d_cams, cams.data(), sizeof(DevCamera) * 2 * nb, cudaMemcpyHostToDevice, st));
+  B2M_CUDA_TRY(ctx, cudaMemcpyAsync(G.d_i32, i32.data(), sizeof(int32_t) * L.size, cudaMemcpyHostToDevice, st));
+  B2M_CUDA_TRY(ctx, cudaMemcpyAsync(G.d_off, off.data(), sizeof(int64_t) * nb, cudaMemcpyHostToDevice, st));
+  B2M_CUDA_TRY(ctx, cudaMemsetAsync(G.d_models, 0, sizeof(double) * 27 * nb, st));
+  G.n_matches = total;
+  *P = G.params(nb, cap);
+  P->opt = opt;
+  P->seed = ctx->seed;
+  P->single_kind = single_kind;
+  P->counters = ctx->d_counters + kVerifyCounters;
+  P->lo_eig_thread = lo_eig_thread_mode();
+  return B2M_OK;
+}
+
+// Estimates problems[0, nb) (at most one chunk, arguments checked): RANSAC for E / F / H, with E on undistorted
+// points when a camera has distortion, the decision kernel, the relative pose when asked for, and the results in
+// out[0, nb) and inlier_matches[0, nb).
+int run_chunk(b2m_ctx* ctx, const b2m_tvg_problem* problems, int nb, const b2m_tvg_opts& opt, b2m_tvg_result* out,
+              uint32_t* const* inlier_matches) {
+  cudaStream_t st = ctx->stream;
+  StandaloneBatch G;
+  VerifyParams P;
+  if (int rc = stage(ctx, problems, nb, opt, -1, G, &P)) return rc;
+  if (int rc = upload_distortion(ctx, G, problems, nb)) return rc;
+  if (G.d_dist) {  // the E kernel reads undistorted points
+    B2M_CUDA_TRY(ctx, G.d_pts_undist.ensure(P.arena_cap));
+    b2m_undistort_kernel<<<nb, 256, 0, st>>>(P, G.d_dist, G.d_pts_undist);
+    B2M_CUDA_TRY(ctx, cudaGetLastError());
     ctx->stats.kernel_launches += 1;
-    if (opt.compute_relative_pose && full_cams) {
-      B2M_CUDA_TRY(ctx, cudaGetLastError());
-      const std::vector<double> p1(raw1, raw1 + 2 * n1), p2(raw2, raw2 + 2 * n2);
-      const std::vector<int64_t> zero(1, 0);
-      if (int rc = launch_pose_standalone(ctx, G, P, 1, cap, p1, p2, zero, zero, full_cams, 2, st)) return rc;
-    }
   }
+  B2M_CUDA_TRY(ctx, launch_ransac(P, nb, st, nullptr, G.d_pts_undist));
+  b2m_decide_kernel<<<nb, 256, 0, st>>>(P);
   B2M_CUDA_TRY(ctx, cudaGetLastError());
-  ctx->stats.kernel_launches += 1;
+  ctx->stats.kernel_launches += 4;
+  if (opt.compute_relative_pose)
+    if (int rc = launch_pose_standalone(ctx, G, P, problems, nb)) return rc;
+  const StandaloneBatch::Scalars L(nb);
+  std::vector<double> h_pose(static_cast<size_t>(8) * nb, 0.0);
+  std::vector<int32_t> h_pose_valid(nb, 0);
+  if (G.d_pose) {
+    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(h_pose.data(), G.d_pose, sizeof(double) * 8 * nb, cudaMemcpyDeviceToHost, st));
+    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(h_pose_valid.data(), G.d_pose_valid, sizeof(int32_t) * nb, cudaMemcpyDeviceToHost, st));
+  }
+  std::vector<int32_t> h_i32(L.size);
+  std::vector<double> h_models(static_cast<size_t>(27) * nb);
+  std::vector<uint2> h_inl(G.n_matches);
+  B2M_CUDA_TRY(ctx, cudaMemcpyAsync(h_i32.data(), G.d_i32, sizeof(int32_t) * L.size, cudaMemcpyDeviceToHost, st));
+  B2M_CUDA_TRY(ctx, cudaMemcpyAsync(h_models.data(), G.d_models, sizeof(double) * 27 * nb, cudaMemcpyDeviceToHost, st));
+  if (G.n_matches > 0 && inlier_matches)
+    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(h_inl.data(), G.d_inliers, sizeof(uint2) * G.n_matches, cudaMemcpyDeviceToHost, st));
+  B2M_CUDA_TRY(ctx, cudaStreamSynchronize(st));
+  int64_t off = 0;  // of problem k in the arenas
+  for (int k = 0; k < nb; ++k) {
+    b2m_tvg_result& r = out[k];
+    memset(&r, 0, sizeof(r));
+    r.struct_size = sizeof(r);
+    r.config = h_i32[L.config + k];
+    r.n_inliers = h_i32[L.inl_cnt + k];
+    r.nE = h_i32[L.sup + 3 * k];
+    r.nF = h_i32[L.sup + 3 * k + 1];
+    r.nH = h_i32[L.sup + 3 * k + 2];
+    memcpy(r.E, h_models.data() + 27 * k, sizeof(double) * 9);
+    memcpy(r.F, h_models.data() + 27 * k + 9, sizeof(double) * 9);
+    memcpy(r.H, h_models.data() + 27 * k + 18, sizeof(double) * 9);
+    fill_pose(&r, h_pose.data() + 8 * k, h_pose_valid[k] && r.n_inliers > 0);
+    if (r.n_inliers > 0 && inlier_matches && inlier_matches[k])
+      memcpy(inlier_matches[k], h_inl.data() + off, sizeof(uint2) * r.n_inliers);
+    off += h_i32[L.cnt + k];
+  }
   return B2M_OK;
 }
 
@@ -1637,61 +1707,6 @@ using namespace b2m;
 
 extern "C" {
 
-// One EstimateTwoViewGeometry run (multiple_models ignored): the body of b2m_estimate_two_view_geometry.
-static int estimate_tvg_once(b2m_ctx* ctx, const b2m_camera* cam1, const double* points1, int64_t n1,
-                             const b2m_camera* cam2, const double* points2, int64_t n2, const uint32_t* matches,
-                             int64_t m, const b2m_tvg_opts* opts, b2m_tvg_result* out, uint32_t* inlier_matches) {
-  if (!ctx) return B2M_EINVAL;
-  if (!cam1 || !cam2 || !opts || !out) return fail(ctx, B2M_EINVAL, "[verify.cu] Check Failed: cameras, options and out != NULL");
-  if (const char* why = camera_problem(*cam1)) return fail(ctx, B2M_EINVAL, why);
-  if (const char* why = camera_problem(*cam2)) return fail(ctx, B2M_EINVAL, why);
-  if (n1 < 0 || n2 < 0 || (n1 > 0 && !points1) || (n2 > 0 && !points2)) return fail(ctx, B2M_EINVAL, "[verify.cu] Check Failed: points");
-  if (!matches) {  // identity matching (R:estimators/two_view_geometry.h:136-142)
-    if (n1 != n2) return fail(ctx, B2M_EINVAL, "[verify.cu] Check Failed: points1.size() == points2.size()");
-    m = n1;
-  }
-  if (m < 0) return fail(ctx, B2M_EINVAL, "[verify.cu] Check Failed: m >= 0");
-  cudaSetDevice(ctx->device);
-  std::vector<double4> pts(m);
-  std::vector<uint2> mm(m);
-  for (int64_t i = 0; i < m; ++i) {
-    const uint32_t a = matches ? matches[2 * i] : static_cast<uint32_t>(i);
-    const uint32_t b = matches ? matches[2 * i + 1] : static_cast<uint32_t>(i);
-    if (a >= n1 || b >= n2) return fail(ctx, B2M_EINVAL, "[verify.cu] Check Failed: match index < number of points");
-    pts[i] = make_double4(points1[2 * a], points1[2 * a + 1], points2[2 * b], points2[2 * b + 1]);
-    mm[i] = make_uint2(a, b);
-  }
-  const DevCamera cams[2] = {to_dev(*cam1), to_dev(*cam2)};
-  Single G;
-  VerifyParams P;
-  const b2m_camera* full_cams[2] = {cam1, cam2};
-  if (int rc = run_single(ctx, pts, mm, cams, *opts, -1, G, P, full_cams, points1, n1, points2, n2)) return rc;
-  int32_t i32[16];
-  double models[27];
-  double h_pose[8] = {1, 0, 0, 0, 0, 0, 0, 0};
-  int32_t h_pose_valid = 0;
-  B2M_CUDA_TRY(ctx, cudaMemcpyAsync(i32, G.d_i32, sizeof(i32), cudaMemcpyDeviceToHost, ctx->stream));
-  B2M_CUDA_TRY(ctx, cudaMemcpyAsync(models, G.d_models, sizeof(models), cudaMemcpyDeviceToHost, ctx->stream));
-  if (G.d_pose) {
-    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(h_pose, G.d_pose, sizeof(h_pose), cudaMemcpyDeviceToHost, ctx->stream));
-    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(&h_pose_valid, G.d_pose_valid, sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
-  }
-  B2M_CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
-  memset(out, 0, sizeof(*out));
-  out->struct_size = sizeof(*out);
-  out->config = i32[9];
-  out->n_inliers = i32[10];
-  fill_pose(out, h_pose, &h_pose_valid, 0);
-  out->nE = i32[3]; out->nF = i32[4]; out->nH = i32[5];
-  memcpy(out->E, models, sizeof(double) * 9);
-  memcpy(out->F, models + 9, sizeof(double) * 9);
-  memcpy(out->H, models + 18, sizeof(double) * 9);
-  if (out->n_inliers > 0 && inlier_matches) {
-    B2M_CUDA_TRY(ctx, cudaMemcpy(inlier_matches, G.d_inliers, sizeof(uint2) * out->n_inliers, cudaMemcpyDeviceToHost));
-  }
-  return B2M_OK;
-}
-
 // EstimateTwoViewGeometry; with opts->multiple_models the loop of EstimateMultipleTwoViewGeometries
 // (U:estimators/two_view_geometry.cc): estimate on the remaining matches, keep the geometry (a WATERMARK one
 // only if !multiple_ignore_watermark), remove its inliers from the remaining matches, repeat until the
@@ -1703,8 +1718,21 @@ int b2m_estimate_two_view_geometry(b2m_ctx* ctx, const b2m_camera* cam1, const d
                                    const uint32_t* matches, int64_t m, const b2m_tvg_opts* opts,
                                    b2m_tvg_result* out, uint32_t* inlier_matches) {
   if (!ctx) return B2M_EINVAL;
-  if (!opts || !opts->multiple_models)
-    return estimate_tvg_once(ctx, cam1, points1, n1, cam2, points2, n2, matches, m, opts, out, inlier_matches);
+  if (!opts || !opts->multiple_models) {
+    if (!cam1 || !cam2 || !opts || !out) return fail(ctx, B2M_EINVAL, "[verify.cu] Check Failed: cameras, options and out != NULL");
+    if (const char* why = camera_problem(*cam1)) return fail(ctx, B2M_EINVAL, why);
+    if (const char* why = camera_problem(*cam2)) return fail(ctx, B2M_EINVAL, why);
+    if (n1 < 0 || n2 < 0 || (n1 > 0 && !points1) || (n2 > 0 && !points2)) return fail(ctx, B2M_EINVAL, "[verify.cu] Check Failed: points");
+    if (!matches) {  // identity matching (R:estimators/two_view_geometry.h:136-142)
+      if (n1 != n2) return fail(ctx, B2M_EINVAL, "[verify.cu] Check Failed: points1.size() == points2.size()");
+      m = n1;
+    }
+    if (m < 0) return fail(ctx, B2M_EINVAL, "[verify.cu] Check Failed: m >= 0");
+    if (m > INT32_MAX) return fail(ctx, B2M_EINVAL, "[verify.cu] Check Failed: matches per problem < 2^31");
+    cudaSetDevice(ctx->device);
+    const b2m_tvg_problem q{sizeof(q), 0, *cam1, *cam2, points1, n1, points2, n2, matches, m};
+    return run_chunk(ctx, &q, 1, *opts, out, &inlier_matches);
+  }
   if (!out) return fail(ctx, B2M_EINVAL, "[verify.cu] Check Failed: out != NULL");
   if (!matches) {
     if (n1 != n2) return fail(ctx, B2M_EINVAL, "[verify.cu] Check Failed: points1.size() == points2.size()");
@@ -1724,7 +1752,9 @@ int b2m_estimate_two_view_geometry(b2m_ctx* ctx, const b2m_camera* cam1, const d
     b2m_tvg_result g;
     const int64_t rem = static_cast<int64_t>(remaining.size() / 2);
     std::vector<uint32_t> inl(static_cast<size_t>(std::max<int64_t>(rem, 1)) * 2);
-    if (int rc = estimate_tvg_once(ctx, cam1, points1, n1, cam2, points2, n2, remaining.data(), rem, &once, &g, inl.data()))
+    // one round: the plain estimate (multiple_models off) on the remaining matches
+    if (int rc = b2m_estimate_two_view_geometry(ctx, cam1, points1, n1, cam2, points2, n2, remaining.data(), rem, &once,
+                                                &g, inl.data()))
       return rc;
     if (g.config == B2M_DEGENERATE || g.n_inliers <= 0) break;
     inl.resize(static_cast<size_t>(g.n_inliers) * 2);
@@ -1789,127 +1819,10 @@ int b2m_estimate_two_view_geometry_batch(b2m_ctx* ctx, const b2m_tvg_problem* pr
     if (const char* why = camera_problem(q.cam2)) return fail(ctx, B2M_EINVAL, why);
   }
   cudaSetDevice(ctx->device);
-  cudaStream_t st = ctx->stream;
   constexpr int64_t kChunk = 4096;  // problems per launch: bounds the staging memory, plenty to fill 132 SMs
   for (int64_t k0 = 0; k0 < n_problems; k0 += kChunk) {
     const int nb = static_cast<int>(std::min(kChunk, n_problems - k0));
-    std::vector<double4> pts;
-    std::vector<uint2> mm;
-    std::vector<int64_t> off(nb);
-    std::vector<int32_t> cnt(nb), pairs(2 * nb);
-    std::vector<DevCamera> cams(2 * nb);
-    std::vector<const b2m_camera*> full_cams(2 * nb);
-    std::vector<double> raw1, raw2;            // compute_relative_pose: the callers' point arrays, concatenated
-    std::vector<int64_t> raw1_off(nb, 0), raw2_off(nb, 0);
-    for (int k = 0; k < nb; ++k) {
-      const b2m_tvg_problem& q = problems[k0 + k];
-      full_cams[2 * k] = &q.cam1;
-      full_cams[2 * k + 1] = &q.cam2;
-      if (opts->compute_relative_pose) {
-        raw1_off[k] = static_cast<int64_t>(raw1.size() / 2);
-        raw2_off[k] = static_cast<int64_t>(raw2.size() / 2);
-        raw1.insert(raw1.end(), q.points1, q.points1 + 2 * q.n1);
-        raw2.insert(raw2.end(), q.points2, q.points2 + 2 * q.n2);
-      }
-      const int64_t m = q.matches ? q.m : q.n1;
-      off[k] = static_cast<int64_t>(pts.size());
-      cnt[k] = static_cast<int32_t>(m);
-      pairs[2 * k] = 2 * k;
-      pairs[2 * k + 1] = 2 * k + 1;
-      cams[2 * k] = to_dev(q.cam1);
-      cams[2 * k + 1] = to_dev(q.cam2);
-      for (int64_t i = 0; i < m; ++i) {
-        const uint32_t a = q.matches ? q.matches[2 * i] : static_cast<uint32_t>(i);
-        const uint32_t b = q.matches ? q.matches[2 * i + 1] : static_cast<uint32_t>(i);
-        if (a >= q.n1 || b >= q.n2) return fail(ctx, B2M_EINVAL, "[verify.cu] Check Failed: match index < number of points");
-        pts.push_back(make_double4(q.points1[2 * a], q.points1[2 * a + 1], q.points2[2 * b], q.points2[2 * b + 1]));
-        mm.push_back(make_uint2(a, b));
-      }
-    }
-    const int64_t total = static_cast<int64_t>(pts.size());
-    const int64_t cap = std::max<int64_t>(total, 1);
-    Single G;  // owns the arenas; the per-problem scalars live in one int32 block (see the offsets below)
-    int32_t* d_i32 = nullptr;  // pairs[2nb] cnt[nb] sup[3nb] success[3nb] config[nb] inl_cnt[nb]
-    B2M_CUDA_TRY(ctx, G.d_pts.ensure(cap));
-    B2M_CUDA_TRY(ctx, G.d_matches.ensure(cap));
-    B2M_CUDA_TRY(ctx, G.d_inliers.ensure(cap));
-    B2M_CUDA_TRY(ctx, G.d_mask.ensure(3 * cap));
-    B2M_CUDA_TRY(ctx, G.d_cams.ensure(2 * nb));
-    B2M_CUDA_TRY(ctx, G.d_i32.ensure(11 * nb));
-    B2M_CUDA_TRY(ctx, G.d_off.ensure(nb));
-    B2M_CUDA_TRY(ctx, G.d_models.ensure(27 * nb));
-    B2M_CUDA_TRY(ctx, G.d_e_scratch.ensure(static_cast<size_t>(kEStride) * kRansacThreads * nb));
-    d_i32 = G.d_i32;
-    if (total > 0) {
-      B2M_CUDA_TRY(ctx, cudaMemcpyAsync(G.d_pts, pts.data(), sizeof(double4) * total, cudaMemcpyHostToDevice, st));
-      B2M_CUDA_TRY(ctx, cudaMemcpyAsync(G.d_matches, mm.data(), sizeof(uint2) * total, cudaMemcpyHostToDevice, st));
-    }
-    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(G.d_cams, cams.data(), sizeof(DevCamera) * 2 * nb, cudaMemcpyHostToDevice, st));
-    B2M_CUDA_TRY(ctx, cudaMemsetAsync(d_i32, 0, sizeof(int32_t) * 11 * nb, st));
-    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(d_i32, pairs.data(), sizeof(int32_t) * 2 * nb, cudaMemcpyHostToDevice, st));
-    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(d_i32 + 2 * nb, cnt.data(), sizeof(int32_t) * nb, cudaMemcpyHostToDevice, st));
-    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(G.d_off, off.data(), sizeof(int64_t) * nb, cudaMemcpyHostToDevice, st));
-    B2M_CUDA_TRY(ctx, cudaMemsetAsync(G.d_models, 0, sizeof(double) * 27 * nb, st));
-    VerifyParams P = VerifyParams{};
-    P.pairs = d_i32;
-    P.pair_cnt = d_i32 + 2 * nb;
-    P.sup_cnt = d_i32 + 3 * nb;
-    P.success = d_i32 + 6 * nb;
-    P.config = d_i32 + 9 * nb;
-    P.inl_cnt = d_i32 + 10 * nb;
-    P.pair_off = G.d_off;
-    P.pts = G.d_pts;
-    P.matches = G.d_matches;
-    P.cams = G.d_cams;
-    P.mask = G.d_mask;
-    P.arena_cap = cap;
-    P.models = G.d_models;
-    P.inliers = G.d_inliers;
-    P.opt = *opts;
-    P.seed = ctx->seed;
-    P.single_kind = -1;
-    P.counters = ctx->d_counters + kVerifyCounters;
-      P.e_scratch = G.d_e_scratch;
-    P.lo_eig_thread = lo_eig_thread_mode();
-    const double4* pts_E = nullptr;
-    if (int rc = undistort_for_E(ctx, G, P, full_cams.data(), 2 * nb, nb, cap, st, &pts_E)) return rc;
-    B2M_CUDA_TRY(ctx, launch_ransac(P, nb, st, nullptr, pts_E));
-    b2m_decide_kernel<<<nb, 256, 0, st>>>(P);
-    B2M_CUDA_TRY(ctx, cudaGetLastError());
-    ctx->stats.kernel_launches += 4;
-    if (opts->compute_relative_pose)
-      if (int rc = launch_pose_standalone(ctx, G, P, nb, cap, raw1, raw2, raw1_off, raw2_off, full_cams.data(), 2 * nb, st))
-        return rc;
-    std::vector<double> h_pose(static_cast<size_t>(8) * nb, 0.0);
-    std::vector<int32_t> h_pose_valid(nb, 0);
-    if (G.d_pose) {
-      B2M_CUDA_TRY(ctx, cudaMemcpyAsync(h_pose.data(), G.d_pose, sizeof(double) * 8 * nb, cudaMemcpyDeviceToHost, st));
-      B2M_CUDA_TRY(ctx, cudaMemcpyAsync(h_pose_valid.data(), G.d_pose_valid, sizeof(int32_t) * nb, cudaMemcpyDeviceToHost, st));
-    }
-    std::vector<int32_t> h_i32(static_cast<size_t>(11) * nb);
-    std::vector<double> h_models(static_cast<size_t>(27) * nb);
-    std::vector<uint2> h_inl(static_cast<size_t>(cap));
-    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(h_i32.data(), d_i32, sizeof(int32_t) * 11 * nb, cudaMemcpyDeviceToHost, st));
-    B2M_CUDA_TRY(ctx, cudaMemcpyAsync(h_models.data(), G.d_models, sizeof(double) * 27 * nb, cudaMemcpyDeviceToHost, st));
-    if (total > 0 && inlier_matches)
-      B2M_CUDA_TRY(ctx, cudaMemcpyAsync(h_inl.data(), G.d_inliers, sizeof(uint2) * total, cudaMemcpyDeviceToHost, st));
-    B2M_CUDA_TRY(ctx, cudaStreamSynchronize(st));
-    for (int k = 0; k < nb; ++k) {
-      b2m_tvg_result& r = out[k0 + k];
-      memset(&r, 0, sizeof(r));
-      r.struct_size = sizeof(r);
-      r.config = h_i32[9 * nb + k];
-      r.n_inliers = h_i32[10 * nb + k];
-      r.nE = h_i32[3 * nb + 3 * k];
-      r.nF = h_i32[3 * nb + 3 * k + 1];
-      r.nH = h_i32[3 * nb + 3 * k + 2];
-      memcpy(r.E, h_models.data() + 27 * k, sizeof(double) * 9);
-      memcpy(r.F, h_models.data() + 27 * k + 9, sizeof(double) * 9);
-      memcpy(r.H, h_models.data() + 27 * k + 18, sizeof(double) * 9);
-      fill_pose(&r, h_pose.data(), h_pose_valid.data(), k);
-      if (r.n_inliers > 0 && inlier_matches && inlier_matches[k0 + k])
-        memcpy(inlier_matches[k0 + k], h_inl.data() + off[k], sizeof(uint2) * r.n_inliers);
-    }
+    if (int rc = run_chunk(ctx, problems + k0, nb, *opts, out + k0, inlier_matches ? inlier_matches + k0 : nullptr)) return rc;
   }
   return B2M_OK;
 }
@@ -1922,32 +1835,28 @@ int b2m_ransac_model(b2m_ctx* ctx, int32_t kind, const double* points1, const do
   if (!opts || !out_model || !num_inliers || !success) return fail(ctx, B2M_EINVAL, "[verify.cu] Check Failed: outputs != NULL");
   if (m < 0 || (m > 0 && (!points1 || !points2))) return fail(ctx, B2M_EINVAL, "[verify.cu] Check Failed: points");
   cudaSetDevice(ctx->device);
-  std::vector<double4> pts(m);
-  std::vector<uint2> mm(m);
-  for (int64_t i = 0; i < m; ++i) {
-    pts[i] = make_double4(points1[2 * i], points1[2 * i + 1], points2[2 * i], points2[2 * i + 1]);
-    mm[i] = make_uint2(static_cast<uint32_t>(i), static_cast<uint32_t>(i));
-  }
   b2m_tvg_opts t;
   b2m_tvg_opts_default(&t);
   t.ransac = *opts;
-  DevCamera cams[2];
-  memset(cams, 0, sizeof(cams));
-  cams[0].fx = cams[0].fy = cams[0].mean_f = 1.0;
-  cams[1] = cams[0];
-  Single G;
+  // identity matches; a unit SIMPLE_PINHOLE camera (f, cx, cy) = (1, 0, 0), which a single-kind kernel does not read
+  const b2m_camera unit{sizeof(unit), 0, 0, 0, 0, 0, {1.0}};
+  const b2m_tvg_problem q{sizeof(q), 0, unit, unit, points1, m, points2, m, nullptr, 0};
+  StandaloneBatch G;
   VerifyParams P;
-  if (int rc = run_single(ctx, pts, mm, cams, t, kind, G, P)) return rc;
-  int32_t i32[16];
+  if (int rc = stage(ctx, &q, 1, t, kind, G, &P)) return rc;
+  B2M_CUDA_TRY(ctx, launch_ransac(P, 1, ctx->stream));
+  ctx->stats.kernel_launches += 1;
+  const StandaloneBatch::Scalars L(1);
+  std::vector<int32_t> i32(L.size);
   double models[27];
-  B2M_CUDA_TRY(ctx, cudaMemcpyAsync(i32, G.d_i32, sizeof(i32), cudaMemcpyDeviceToHost, ctx->stream));
+  B2M_CUDA_TRY(ctx, cudaMemcpyAsync(i32.data(), G.d_i32, sizeof(int32_t) * L.size, cudaMemcpyDeviceToHost, ctx->stream));
   B2M_CUDA_TRY(ctx, cudaMemcpyAsync(models, G.d_models, sizeof(models), cudaMemcpyDeviceToHost, ctx->stream));
   if (m > 0 && inlier_mask)
     B2M_CUDA_TRY(ctx, cudaMemcpyAsync(inlier_mask, G.d_mask + static_cast<int64_t>(kind) * P.arena_cap, m,
                                cudaMemcpyDeviceToHost, ctx->stream));
   B2M_CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
-  *num_inliers = i32[3 + kind];
-  *success = i32[6 + kind];
+  *num_inliers = i32[L.sup + kind];
+  *success = i32[L.success + kind];
   memcpy(out_model, models + 9 * kind, sizeof(double) * 9);
   return B2M_OK;
 }
@@ -1970,56 +1879,41 @@ int b2m_estimate_two_view_geometry_pose(b2m_ctx* ctx, const b2m_camera* cam1, co
       return fail(ctx, B2M_EINVAL, "[verify.cu] Check Failed: match index < number of points");
   cudaSetDevice(ctx->device);
   cudaStream_t st = ctx->stream;
-  Single G;
+  StandaloneBatch G;
+  const StandaloneBatch::Scalars L(1);
   const int64_t cap = std::max<int64_t>(n_inliers, 1);
   const DevCamera cams[2] = {to_dev(*cam1), to_dev(*cam2)};
-  const int32_t i32[4] = {0, 1, static_cast<int32_t>(n_inliers), geometry->config};  // pairs[2], inl_cnt, config
+  std::vector<int32_t> i32(L.size, 0);
+  i32[L.pairs + 1] = 1;
+  i32[L.inl_cnt] = static_cast<int32_t>(n_inliers);
+  i32[L.config] = geometry->config;
   const int64_t off0 = 0;
-  double models[27];
-  memset(models, 0, sizeof(models));
+  double models[27] = {};
   memcpy(models, geometry->E, sizeof(double) * 9);
   memcpy(models + 18, geometry->H, sizeof(double) * 9);
   B2M_CUDA_TRY(ctx, G.d_inliers.ensure(cap));
   B2M_CUDA_TRY(ctx, G.d_cams.ensure(2));
-  B2M_CUDA_TRY(ctx, G.d_i32.ensure(4));
+  B2M_CUDA_TRY(ctx, G.d_i32.ensure(L.size));
   B2M_CUDA_TRY(ctx, G.d_off.ensure(1));
   B2M_CUDA_TRY(ctx, G.d_models.ensure(27));
   if (n_inliers > 0)
     B2M_CUDA_TRY(ctx, cudaMemcpy(G.d_inliers, inlier_matches, sizeof(uint2) * n_inliers, cudaMemcpyHostToDevice));
   B2M_CUDA_TRY(ctx, cudaMemcpy(G.d_cams, cams, sizeof(cams), cudaMemcpyHostToDevice));
-  B2M_CUDA_TRY(ctx, cudaMemcpy(G.d_i32, i32, sizeof(i32), cudaMemcpyHostToDevice));
+  B2M_CUDA_TRY(ctx, cudaMemcpy(G.d_i32, i32.data(), sizeof(int32_t) * L.size, cudaMemcpyHostToDevice));
   B2M_CUDA_TRY(ctx, cudaMemcpy(G.d_off, &off0, sizeof(int64_t), cudaMemcpyHostToDevice));
   B2M_CUDA_TRY(ctx, cudaMemcpy(G.d_models, models, sizeof(models), cudaMemcpyHostToDevice));
-  VerifyParams P = VerifyParams{};
-  P.pairs = G.d_i32;
-  P.inl_cnt = G.d_i32 + 2;
-  P.config = G.d_i32 + 3;
-  P.pair_off = G.d_off;
-  P.inliers = G.d_inliers;
-  P.models = G.d_models;
-  P.cams = G.d_cams;
-  const std::vector<double> p1(points1, points1 + 2 * n1), p2(points2, points2 + 2 * n2);
-  const std::vector<int64_t> zero(1, 0);
-  const b2m_camera* full_cams[2] = {cam1, cam2};
-  if (int rc = launch_pose_standalone(ctx, G, P, 1, cap, p1, p2, zero, zero, full_cams, 2, st)) return rc;
+  const VerifyParams P = G.params(1, cap);
+  const b2m_tvg_problem q{sizeof(q), 0, *cam1, *cam2, points1, n1, points2, n2, inlier_matches, n_inliers};
+  if (int rc = upload_distortion(ctx, G, &q, 1)) return rc;
+  if (int rc = launch_pose_standalone(ctx, G, P, &q, 1)) return rc;
   double h_pose[8];
-  int32_t h_valid = 0, h_i32[4];
+  int32_t h_valid = 0;
   B2M_CUDA_TRY(ctx, cudaMemcpyAsync(h_pose, G.d_pose, sizeof(h_pose), cudaMemcpyDeviceToHost, st));
   B2M_CUDA_TRY(ctx, cudaMemcpyAsync(&h_valid, G.d_pose_valid, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-  B2M_CUDA_TRY(ctx, cudaMemcpyAsync(h_i32, G.d_i32, sizeof(h_i32), cudaMemcpyDeviceToHost, st));
+  B2M_CUDA_TRY(ctx, cudaMemcpyAsync(i32.data(), G.d_i32, sizeof(int32_t) * L.size, cudaMemcpyDeviceToHost, st));
   B2M_CUDA_TRY(ctx, cudaStreamSynchronize(st));
-  geometry->qvec[0] = 1.0;
-  geometry->qvec[1] = geometry->qvec[2] = geometry->qvec[3] = 0.0;
-  geometry->tvec[0] = geometry->tvec[1] = geometry->tvec[2] = 0.0;
-  geometry->tri_angle = 0.0;
-  geometry->pose_valid = 0;
-  if (h_valid) {
-    geometry->config = h_i32[3];
-    memcpy(geometry->qvec, h_pose, sizeof(double) * 4);
-    memcpy(geometry->tvec, h_pose + 4, sizeof(double) * 3);
-    geometry->tri_angle = h_pose[7];
-    geometry->pose_valid = 1;
-  }
+  fill_pose(geometry, h_pose, h_valid);
+  if (h_valid) geometry->config = i32[L.config];
   return B2M_OK;
 }
 
