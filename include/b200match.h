@@ -26,10 +26,11 @@
 extern "C" {
 #endif
 
-#define B2M_ABI_VERSION 7   /* 2: b2m_camera carries 12 parameters, batch estimator; 3: multi-GPU entry points (NCCL);
+#define B2M_ABI_VERSION 8   /* 2: b2m_camera carries 12 parameters, batch estimator; 3: multi-GPU entry points (NCCL);
                              * 4: absolute pose estimation / refinement, b2m_stats.abs_pose_*;
                              * 5: triangulation, b2m_stats.tri_*; 6: SIFT feature extraction, b2m_stats.sift_*;
-                             * 7: extraction from encoded / RGB sources, b2m_stats.sift_decode* */
+                             * 7: extraction from encoded / RGB sources, b2m_stats.sift_decode*;
+                             * 8: PatchMatch stereo, b2m_stats.pm_* */
 
 /* error codes */
 #define B2M_OK 0
@@ -514,6 +515,80 @@ int b2m_extract_features_sources(b2m_ctx* ctx, const b2m_image_source* sources, 
                                  b2m_features** out);
 int b2m_source_features_get(const b2m_features* f, int32_t image, b2m_source_view* out);
 
+/* ---- PatchMatch stereo (ABI 8) -------------------------------------------------------------------------------------
+ * What COLMAP's PatchMatch stereo (U:mvs/patch_match_cuda.cu; Schoenberger et al., ECCV 2016) computes for one reference
+ * image and its sources: a depth (camera z) and a normal (camera frame, facing the camera) per pixel, chosen by
+ * propagation and random search to minimise 1 - bilaterally weighted NCC through the plane-induced homography, averaged
+ * over Monte Carlo draws of the sources from their posterior visibility (forward / backward messages of a hidden Markov
+ * chain along each sweep) times the triangulation- and incident-angle priors.  K8 (csrc/patch_match.cu); the schedule is spelled out in DESIGN.md section 4
+ * and restated by oracle/patch_match.py. */
+#define B2M_PM_MAX_SOURCES 32
+typedef struct b2m_patch_match_opts {
+  uint32_t struct_size;
+  int32_t window_radius;                  /* 5 */
+  int32_t window_step;                    /* 1 */
+  int32_t num_samples;                    /* 15: Monte Carlo draws of sources per pixel and hypothesis */
+  int32_t num_iterations;                 /* 5: each of four sweeps (down, up, right, left) */
+  int32_t geom_consistency;               /* 0: photometric pass; 1: geometric term through the sources' depth maps */
+  int32_t filter;                         /* 1 */
+  int32_t filter_min_num_consistent;      /* 2 */
+  float sigma_spatial;                    /* -1 = window_radius */
+  float sigma_color;                      /* 0.2 (intensities in [0, 1]) */
+  float ncc_sigma;                        /* 0.6 */
+  float min_triangulation_angle;          /* 1, degrees */
+  float incident_angle_sigma;             /* 0.9 */
+  float geom_consistency_regularizer;     /* 0.3 */
+  float geom_consistency_max_cost;        /* 3, pixels */
+  float filter_min_ncc;                   /* 0.1 */
+  float filter_min_triangulation_angle;   /* 3, degrees */
+  float filter_geom_consistency_max_cost; /* 1, pixels */
+} b2m_patch_match_opts;
+void b2m_patch_match_opts_default(b2m_patch_match_opts* o);
+
+/* Uploads the images of a workspace once: grey uint8 images and pinhole cameras, cameras[i] = 16 doubles (fx, fy, cx,
+ * cy, then cam_from_world as R row-major (9) and t (3)).  They stay resident until the next call or b2m_destroy.
+ * depth_maps: NULL, or n entries of NULL / a width x height float32 depth map of that image (the photometric maps the
+ * geometric pass reads).  A set that does not fit in device memory is B2M_ENOMEM with its size in the message. */
+int b2m_patch_match_set_images(b2m_ctx* ctx, int32_t n, const b2m_image* images, const double* cameras,
+                               const float* const* depth_maps);
+
+typedef struct b2m_patch_match_problem {
+  uint32_t struct_size;
+  int32_t ref;                  /* index into the image set */
+  int32_t n_src;                /* 1 .. B2M_PM_MAX_SOURCES */
+  int32_t image_id;             /* a stable id of the reference (e.g. its workspace image_id): the key of its random
+                                 * numbers, so that its maps do not depend on which image set or batch it runs in */
+  const int32_t* src;           /* n_src image indices, distinct and != ref */
+  float depth_min, depth_max;   /* 0 < depth_min < depth_max */
+  const float* init_depth;      /* NULL, or the ref's width x height start depths (0 = start at random) */
+  const float* init_normal;     /* NULL, or width x height x 3 start normals (with init_depth) */
+} b2m_patch_match_problem;
+
+typedef struct b2m_depth_maps b2m_depth_maps;
+typedef struct b2m_depth_map_view {
+  uint32_t struct_size;
+  int32_t width, height;
+  int32_t reserved;
+  const float* depth;           /* [height x width]; 0 where filtered */
+  const float* normal;          /* [height x width x 3]; 0 where filtered */
+} b2m_depth_map_view;
+
+/* Runs the problems in one batch of launches; with opts->geom_consistency every source of every problem needs a depth
+ * map in the image set.  Problem k's maps depend only on (ctx seed, its image_id, its images, cameras and options),
+ * never on the index of its images in the set, its position in the batch or the batch's other problems.  Read with b2m_depth_maps_get, release with
+ * b2m_depth_maps_free. */
+int b2m_patch_match_batch(b2m_ctx* ctx, const b2m_patch_match_problem* problems, int32_t n,
+                          const b2m_patch_match_opts* opts, b2m_depth_maps** out);
+int b2m_depth_maps_get(const b2m_depth_maps* m, int32_t k, b2m_depth_map_view* out);
+void b2m_depth_maps_free(b2m_depth_maps* m);
+
+/* K8's cost arithmetic for given hypotheses of `problem`: queries [n x 7] = (x, y, depth, nx, ny, nz, source slot);
+ * out [n x 3] = (photometric cost 1 - NCC in [0, 2], geometric cost min(forward-backward reprojection error,
+ * geom_consistency_max_cost) or 0 without source depth maps, depth of the same plane at pixel (x, y + 1)).  Exists so
+ * that tests can hold the device arithmetic against oracle/patch_match.py. */
+int b2m_debug_patch_match_cost(b2m_ctx* ctx, const b2m_patch_match_problem* problem, const b2m_patch_match_opts* opts,
+                               const float* queries, int32_t n, float* out);
+
 /* ---- instrumentation ---------------------------------------------------------------- */
 
 /* The cross-check consults m21 only at the columns some row matched (m21[m12[i]]): the column-direction GEMM is run
@@ -572,6 +647,9 @@ typedef struct b2m_stats {
   uint64_t sift_decoded_bytes;        /* extraction from sources: encoded JPEG bytes decoded on the device */
   uint64_t sift_decode_images;        /* extraction from sources: images decoded (JPEG) or uploaded (pixels) */
   uint64_t sift_decode_hardware;      /* of those, JPEG files decoded by nvJPEG's hardware backend (the JPEG engines) */
+  uint64_t pm_problems;               /* PatchMatch: reference images processed since reset */
+  uint64_t pm_pixel_updates;          /* PatchMatch: pixel x sweep steps */
+  uint64_t pm_window_samples;         /* PatchMatch: window samples evaluated (one reference / source pixel pair each) */
 } b2m_stats;
 int b2m_get_stats(b2m_ctx* ctx, b2m_stats* out);
 int b2m_reset_stats(b2m_ctx* ctx);

@@ -19,6 +19,8 @@ try:
     from ._core import (EstimateTriangulationOptions, PointData, estimate_triangulation,  # noqa: F401
                         estimate_triangulations)
     from ._core import Normalization, Sift, SiftExtractionOptions  # noqa: F401
+    from ._core import PatchMatchOptions  # noqa: F401
+    from .mvs import patch_match_stereo  # noqa: F401
     from ._core import (Context, Database, DatabaseTransaction, Device, ExhaustiveMatchingOptions,  # noqa: F401
                         RANSACOptions, Results, Rigid3d, Rotation3d, SequentialMatchingOptions,
                         SiftMatchingOptions, SpatialMatchingOptions, TwoViewGeometry,

@@ -745,6 +745,7 @@ void b2m_destroy(b2m_ctx* ctx) {
   tri_release(ctx);
   sift_release(ctx);
   image_io_release(ctx);
+  pm_release(ctx);
   verify_release(ctx);
   delete ctx;
 }
@@ -1031,6 +1032,7 @@ int b2m_get_stats(b2m_ctx* ctx, b2m_stats* out) {
     out->abs_pose_residuals = h[kAbsPoseCounters + 1];
     out->tri_models_scored = h[kTriCounters];
     out->tri_residuals = h[kTriCounters + 1];
+    out->pm_window_samples = h[kPmCounters];
   }
   return B2M_OK;
 }

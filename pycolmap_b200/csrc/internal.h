@@ -85,7 +85,8 @@ extern thread_local std::string g_noctx_err;
 constexpr int kVerifyCounters = 0;    // [6]: per model kind E, F, H (verify.cu)
 constexpr int kAbsPoseCounters = 6;   // [2] (abs_pose.cu)
 constexpr int kTriCounters = 8;       // [2] (triangulation.cu)
-constexpr int kNumCounters = 10;
+constexpr int kPmCounters = 10;       // [1]: window samples evaluated (patch_match.cu)
+constexpr int kNumCounters = 11;
 
 }  // namespace b2m
 
@@ -132,6 +133,7 @@ struct b2m_ctx {
   void* tri_state = nullptr;     // b2m::TriState (triangulation.cu): pinned staging and device buffers
   void* sift_state = nullptr;    // b2m::SiftState (sift.cu): pyramid, gradient and keypoint buffers
   void* image_io_state = nullptr;  // b2m::ImageIoState (image_io.cu): nvJPEG handles, decode and rescale buffers
+  void* pm_state = nullptr;        // b2m::PmState (patch_match.cu): the resident images, depth maps and map buffers
 };
 
 namespace b2m {
@@ -159,6 +161,8 @@ int sift_extract(b2m_ctx* ctx, const SiftPlan& plan, const uint8_t* img, int64_t
                  b2m_features* F, const float** d_kout);
 // image_io.cu
 void image_io_release(b2m_ctx* ctx);
+// patch_match.cu
+void pm_release(b2m_ctx* ctx);
 }  // namespace b2m
 
 struct b2m_features {

@@ -942,6 +942,206 @@ void ExtractFeaturesRun(const std::string& database_path, const std::string& ima
   }
 }
 
+// ---- PatchMatch stereo (R:pipeline/mvs.h:92-190; U:mvs/patch_match.h PatchMatchOptions) -----------------------------
+// The workspace I/O and the pass controller live in pycolmap_b200/mvs.py; this is the option class and the device call.
+struct PatchMatchOptions {
+  int max_image_size = -1;
+  std::string gpu_index = "-1";
+  double depth_min = -1.0;
+  double depth_max = -1.0;
+  int window_radius = 5;
+  int window_step = 1;
+  double sigma_spatial = -1.0;
+  double sigma_color = 0.2;
+  int num_samples = 15;
+  double ncc_sigma = 0.6;
+  double min_triangulation_angle = 1.0;
+  double incident_angle_sigma = 0.9;
+  int num_iterations = 5;
+  bool geom_consistency = true;
+  double geom_consistency_regularizer = 0.3;
+  double geom_consistency_max_cost = 3.0;
+  bool filter = true;
+  double filter_min_ncc = 0.1;
+  double filter_min_triangulation_angle = 3.0;
+  int filter_min_num_consistent = 2;
+  double filter_geom_consistency_max_cost = 1.0;
+  double cache_size = 32.0;
+  bool allow_missing_files = false;
+  bool write_consistency_graph = false;
+};
+
+// PatchMatchOptions::Check (U:mvs/patch_match.h), in its order.
+void CheckPatchMatchOptions(const PatchMatchOptions& o) {
+  auto check = [](bool ok, const char* expr) {
+    if (!ok) throw std::invalid_argument(std::string("[patch_match.h] Check Failed: ") + expr);
+  };
+  if (o.depth_min != -1.0 || o.depth_max != -1.0) {
+    check(o.depth_min <= o.depth_max, "depth_min <= depth_max");
+    check(o.depth_min >= 0.0, "depth_min >= 0");
+  }
+  check(o.window_radius <= 32, "window_radius <= kMaxPatchMatchWindowRadius (32)");
+  check(o.sigma_color > 0.0, "sigma_color > 0");
+  check(o.window_radius > 0, "window_radius > 0");
+  check(o.window_step > 0, "window_step > 0");
+  check(o.window_step <= 2, "window_step <= 2");
+  check(o.num_samples > 0, "num_samples > 0");
+  check(o.ncc_sigma > 0.0, "ncc_sigma > 0");
+  check(o.min_triangulation_angle >= 0.0, "min_triangulation_angle >= 0");
+  check(o.min_triangulation_angle < 180.0, "min_triangulation_angle < 180");
+  check(o.incident_angle_sigma > 0.0, "incident_angle_sigma > 0");
+  check(o.num_iterations > 0, "num_iterations > 0");
+  check(o.geom_consistency_regularizer >= 0.0, "geom_consistency_regularizer >= 0");
+  check(o.geom_consistency_max_cost >= 0.0, "geom_consistency_max_cost >= 0");
+  check(o.filter_min_ncc >= -1.0, "filter_min_ncc >= -1");
+  check(o.filter_min_ncc <= 1.0, "filter_min_ncc <= 1");
+  check(o.filter_min_triangulation_angle >= 0.0, "filter_min_triangulation_angle >= 0");
+  check(o.filter_min_triangulation_angle <= 180.0, "filter_min_triangulation_angle <= 180");
+  check(o.filter_min_num_consistent >= 0, "filter_min_num_consistent >= 0");
+  check(o.filter_geom_consistency_max_cost >= 0.0, "filter_geom_consistency_max_cost >= 0");
+  check(o.cache_size > 0.0, "cache_size > 0");
+}
+
+// One device for PatchMatch, as for extraction: gpu_index is a single ordinal, -1 = device 0.
+int PatchMatchDevice(const PatchMatchOptions& o) {
+  if (o.gpu_index.find(',') != std::string::npos)
+    throw std::invalid_argument("[bindings.cc] Check Failed: patch_match_stereo runs on one GPU: gpu_index is a single "
+                                "index, got \"" + o.gpu_index + "\"");
+  int v;
+  try {
+    v = std::stoi(o.gpu_index);
+  } catch (const std::exception&) {
+    throw std::invalid_argument("[bindings.cc] Check Failed: gpu_index is an integer, got \"" + o.gpu_index + "\"");
+  }
+  if (v < -1) throw std::invalid_argument("[bindings.cc] Check Failed: gpu_index >= -1");
+  return v < 0 ? 0 : v;
+}
+
+// The pass a call runs: geometric (geom_consistency) or photometric, filtered or not.
+b2m_patch_match_opts ToAbi(const PatchMatchOptions& o, bool geom, bool filter) {
+  b2m_patch_match_opts a;  // every field set below: no link-time reference to an ABI 8 symbol
+  std::memset(&a, 0, sizeof(a));
+  a.struct_size = sizeof(a);
+  a.window_radius = o.window_radius;
+  a.window_step = o.window_step;
+  a.num_samples = o.num_samples;
+  a.num_iterations = o.num_iterations;
+  a.geom_consistency = geom ? 1 : 0;
+  a.filter = filter ? 1 : 0;
+  a.filter_min_num_consistent = o.filter_min_num_consistent;
+  a.sigma_spatial = static_cast<float>(o.sigma_spatial);
+  a.sigma_color = static_cast<float>(o.sigma_color);
+  a.ncc_sigma = static_cast<float>(o.ncc_sigma);
+  a.min_triangulation_angle = static_cast<float>(o.min_triangulation_angle);
+  a.incident_angle_sigma = static_cast<float>(o.incident_angle_sigma);
+  a.geom_consistency_regularizer = static_cast<float>(o.geom_consistency_regularizer);
+  a.geom_consistency_max_cost = static_cast<float>(o.geom_consistency_max_cost);
+  a.filter_min_ncc = static_cast<float>(o.filter_min_ncc);
+  a.filter_min_triangulation_angle = static_cast<float>(o.filter_min_triangulation_angle);
+  a.filter_geom_consistency_max_cost = static_cast<float>(o.filter_geom_consistency_max_cost);
+  return a;
+}
+
+// The host copies one device call reads: grey images, cameras [n x 16], optional depth maps, problems.
+struct PmInputs {
+  std::vector<ArrU8> images;
+  std::vector<b2m_image> ims;
+  ArrD cameras;
+  std::vector<ArrF32> dmaps;
+  std::vector<const float*> dmap_ptrs;
+  std::vector<std::vector<int32_t>> src;
+  std::vector<ArrF32> init;
+  std::vector<b2m_patch_match_problem> probs;
+};
+
+void LoadPmInputs(const py::list& images, const ArrD& cameras, const py::object& depth_maps, const py::list& problems,
+                  PmInputs* in) {
+  const size_t n = images.size();
+  if (cameras.ndim() != 2 || cameras.shape(0) != static_cast<py::ssize_t>(n) || cameras.shape(1) != 16)
+    throw std::invalid_argument("[bindings.cc] Check Failed: cameras is an n x 16 array (fx, fy, cx, cy, R, t)");
+  in->cameras = cameras;
+  for (size_t i = 0; i < n; ++i) {
+    ArrU8 a = ArrU8::ensure(images[i]);
+    if (!a || a.ndim() != 2) throw std::invalid_argument("[bindings.cc] Check Failed: images are 2-D uint8 arrays");
+    in->ims.push_back(b2m_image{static_cast<int32_t>(a.shape(1)), static_cast<int32_t>(a.shape(0)), a.shape(1), a.data()});
+    in->images.push_back(std::move(a));
+  }
+  if (!depth_maps.is_none()) {
+    const py::list dl = depth_maps;
+    if (dl.size() != n) throw std::invalid_argument("[bindings.cc] Check Failed: one depth map entry per image");
+    for (size_t i = 0; i < n; ++i) {
+      if (dl[i].is_none()) {
+        in->dmap_ptrs.push_back(nullptr);
+        continue;
+      }
+      ArrF32 d = ArrF32::ensure(dl[i]);
+      if (!d || d.ndim() != 2 || d.shape(0) != in->ims[i].height || d.shape(1) != in->ims[i].width)
+        throw std::invalid_argument("[bindings.cc] Check Failed: a depth map has its image's size");
+      in->dmap_ptrs.push_back(d.data());
+      in->dmaps.push_back(std::move(d));
+    }
+  }
+  in->src.resize(problems.size());
+  for (size_t k = 0; k < problems.size(); ++k) {
+    const py::dict d = problems[k];
+    b2m_patch_match_problem p;
+    std::memset(&p, 0, sizeof(p));
+    p.struct_size = sizeof(p);
+    p.ref = d["ref"].cast<int32_t>();
+    p.image_id = d.contains("image_id") ? d["image_id"].cast<int32_t>() : p.ref;
+    in->src[k] = d["src"].cast<std::vector<int32_t>>();
+    p.n_src = static_cast<int32_t>(in->src[k].size());
+    p.src = in->src[k].data();
+    p.depth_min = d["depth_min"].cast<float>();
+    p.depth_max = d["depth_max"].cast<float>();
+    if (d.contains("init_depth") && !d["init_depth"].is_none()) {
+      if (p.ref < 0 || p.ref >= static_cast<int32_t>(n)) throw std::invalid_argument("[bindings.cc] Check Failed: ref in range");
+      ArrF32 dep = ArrF32::ensure(d["init_depth"]), nor = ArrF32::ensure(d["init_normal"]);
+      const b2m_image& im = in->ims[p.ref];
+      if (!dep || !nor || dep.ndim() != 2 || dep.shape(0) != im.height || dep.shape(1) != im.width || nor.ndim() != 3 ||
+          nor.shape(0) != im.height || nor.shape(1) != im.width || nor.shape(2) != 3)
+        throw std::invalid_argument("[bindings.cc] Check Failed: init_depth (H, W) and init_normal (H, W, 3) of the reference");
+      p.init_depth = dep.data();
+      p.init_normal = nor.data();
+      in->init.push_back(std::move(dep));
+      in->init.push_back(std::move(nor));
+    }
+    in->probs.push_back(p);
+  }
+}
+
+// One device call: upload the image set, run the problems, return [(depth (H, W), normal (H, W, 3))].
+py::list PatchMatchRun(b2m_ctx* ctx, const py::list& images, const ArrD& cameras, const py::object& depth_maps,
+                       const py::list& problems, const PatchMatchOptions& options, bool geom, bool filter) {
+  CheckPatchMatchOptions(options);
+  PmInputs in;
+  LoadPmInputs(images, cameras, depth_maps, problems, &in);
+  const auto set = SiftSymbol<decltype(&b2m_patch_match_set_images)>("b2m_patch_match_set_images");
+  const auto batch = SiftSymbol<decltype(&b2m_patch_match_batch)>("b2m_patch_match_batch");
+  const auto get = SiftSymbol<decltype(&b2m_depth_maps_get)>("b2m_depth_maps_get");
+  const auto release = SiftSymbol<decltype(&b2m_depth_maps_free)>("b2m_depth_maps_free");
+  const b2m_patch_match_opts o = ToAbi(options, geom, filter);
+  b2m_depth_maps* maps = nullptr;
+  RunInterruptible([&] {
+    ThrowOnError(ctx, set(ctx, static_cast<int32_t>(in.ims.size()), in.ims.data(), in.cameras.data(),
+                          in.dmap_ptrs.empty() ? nullptr : in.dmap_ptrs.data()));
+    ThrowOnError(ctx, batch(ctx, in.probs.data(), static_cast<int32_t>(in.probs.size()), &o, &maps));
+  });
+  std::unique_ptr<b2m_depth_maps, decltype(release)> guard(maps, release);
+  py::list out;
+  for (size_t k = 0; k < in.probs.size(); ++k) {
+    b2m_depth_map_view v;
+    std::memset(&v, 0, sizeof(v));
+    ThrowOnError(ctx, get(maps, static_cast<int32_t>(k), &v));
+    py::array_t<float> dep(std::vector<py::ssize_t>{v.height, v.width});
+    py::array_t<float> nor(std::vector<py::ssize_t>{v.height, v.width, 3});
+    std::memcpy(dep.mutable_data(), v.depth, sizeof(float) * v.width * v.height);
+    std::memcpy(nor.mutable_data(), v.normal, sizeof(float) * 3 * v.width * v.height);
+    out.append(py::make_tuple(dep, nor));
+  }
+  return out;
+}
+
 void CheckCameraMode(const ImageReaderOptions& o, const char* where) {
   if (CameraModelId(o.camera_model) < 0)
     throw std::invalid_argument(std::string("[") + where + "] Invalid camera model: " + o.camera_model);
@@ -1576,6 +1776,93 @@ PYBIND11_MODULE(_core, m) {
           "Extract SIFT features of the JPEG / PNG files under image_path and write cameras, images, keypoints and "
           "descriptors to a new database");
   }
+  OptionsClass<PatchMatchOptions>(m, "PatchMatchOptions")
+      .field("max_image_size", &PatchMatchOptions::max_image_size,
+             "Maximum image size in either dimension; larger images are downscaled (-1: no limit).")
+      .field("gpu_index", &PatchMatchOptions::gpu_index, "Index of the GPU used for patch match (one index; -1: device 0).")
+      .field("depth_min", &PatchMatchOptions::depth_min, "Minimum depth (-1: from the sparse points of each image).")
+      .field("depth_max", &PatchMatchOptions::depth_max, "Maximum depth (-1: from the sparse points of each image).")
+      .field("window_radius", &PatchMatchOptions::window_radius, "Half window size to compute NCC photo-consistency cost.")
+      .field("window_step", &PatchMatchOptions::window_step, "Number of pixels to skip when computing NCC (1 or 2).")
+      .field("sigma_spatial", &PatchMatchOptions::sigma_spatial,
+             "Spatial sigma for bilaterally weighted NCC (-1: window_radius).")
+      .field("sigma_color", &PatchMatchOptions::sigma_color, "Color sigma for bilaterally weighted NCC.")
+      .field("num_samples", &PatchMatchOptions::num_samples, "Number of random samples to draw in Monte Carlo sampling.")
+      .field("ncc_sigma", &PatchMatchOptions::ncc_sigma, "Spread of the NCC likelihood function.")
+      .field("min_triangulation_angle", &PatchMatchOptions::min_triangulation_angle,
+             "Minimum triangulation angle in degrees.")
+      .field("incident_angle_sigma", &PatchMatchOptions::incident_angle_sigma,
+             "Spread of the incident angle likelihood function.")
+      .field("num_iterations", &PatchMatchOptions::num_iterations, "Number of coordinate descent iterations.")
+      .field("geom_consistency", &PatchMatchOptions::geom_consistency,
+             "Whether to add a regularized geometric consistency term to the cost function.")
+      .field("geom_consistency_regularizer", &PatchMatchOptions::geom_consistency_regularizer,
+             "The relative weight of the geometric consistency term w.r.t. the photo-consistency term.")
+      .field("geom_consistency_max_cost", &PatchMatchOptions::geom_consistency_max_cost,
+             "Maximum geometric consistency cost in terms of the forward-backward reprojection error in pixels.")
+      .field("filter", &PatchMatchOptions::filter, "Whether to enable filtering.")
+      .field("filter_min_ncc", &PatchMatchOptions::filter_min_ncc, "Minimum NCC coefficient for pixel to be photo-consistent.")
+      .field("filter_min_triangulation_angle", &PatchMatchOptions::filter_min_triangulation_angle,
+             "Minimum triangulation angle to be stable.")
+      .field("filter_min_num_consistent", &PatchMatchOptions::filter_min_num_consistent,
+             "Minimum number of source images have to be consistent for pixel not to be filtered.")
+      .field("filter_geom_consistency_max_cost", &PatchMatchOptions::filter_geom_consistency_max_cost,
+             "Maximum forward-backward reprojection error for pixel to be geometrically consistent.")
+      .field("cache_size", &PatchMatchOptions::cache_size,
+             "Cache size in gigabytes for patch match.  Checked and otherwise without effect: every image of the "
+             "workspace is decoded once per call and held on the GPU.")
+      .field("allow_missing_files", &PatchMatchOptions::allow_missing_files,
+             "Whether to tolerate missing images/maps in the problem setup (skipped with a warning).")
+      .field("write_consistency_graph", &PatchMatchOptions::write_consistency_graph,
+             "Whether to write the consistency graph (not supported: True is refused).")
+      .Finish();
+  m.def("_check_patch_match_options", [](const PatchMatchOptions& o) {
+    CheckPatchMatchOptions(o);
+    return PatchMatchDevice(o);
+  });
+  m.def("_patch_match_run",
+        [](const py::list& images, const ArrD& cameras, const py::object& depth_maps, const py::list& problems,
+           const PatchMatchOptions& options, bool geom, bool filter) {
+          return PatchMatchRun(Engine::Get(PatchMatchDevice(options)), images, cameras, depth_maps, problems, options, geom,
+                               filter);
+        },
+        "images"_a, "cameras"_a, "depth_maps"_a, "problems"_a, "options"_a, "geom"_a, "filter"_a,
+        "One PatchMatch device call (pycolmap_b200.mvs): [(depth (H, W), normal (H, W, 3))] per problem");
+  m.def("_patch_match_stats",
+        [](int device) {
+          b2m_ctx* ctx = Engine::Get(device);
+          b2m_stats st;
+          std::memset(&st, 0, sizeof(st));
+          st.struct_size = sizeof(st);
+          ThrowOnError(ctx, b2m_get_stats(ctx, &st));
+          return py::dict("pm_problems"_a = st.pm_problems, "pm_pixel_updates"_a = st.pm_pixel_updates,
+                          "pm_window_samples"_a = st.pm_window_samples, "kernel_launches"_a = st.kernel_launches);
+        },
+        "device"_a = 0, "The PatchMatch counters of the context patch_match_stereo uses on this device (since it was created)");
+  m.def("debug_patch_match_cost",
+        [](const py::list& images, const ArrD& cameras, const py::object& depth_maps, const py::dict& problem,
+           const ArrF32& queries, const PatchMatchOptions& options) {
+          CheckPatchMatchOptions(options);
+          PmInputs in;
+          py::list one;
+          one.append(problem);
+          LoadPmInputs(images, cameras, depth_maps, one, &in);
+          if (queries.ndim() != 2 || queries.shape(1) != 7)
+            throw std::invalid_argument("[bindings.cc] Check Failed: queries is an n x 7 float32 array");
+          b2m_ctx* ctx = Engine::Get(PatchMatchDevice(options));
+          const auto set = SiftSymbol<decltype(&b2m_patch_match_set_images)>("b2m_patch_match_set_images");
+          const auto cost = SiftSymbol<decltype(&b2m_debug_patch_match_cost)>("b2m_debug_patch_match_cost");
+          ThrowOnError(ctx, set(ctx, static_cast<int32_t>(in.ims.size()), in.ims.data(), in.cameras.data(),
+                                in.dmap_ptrs.empty() ? nullptr : in.dmap_ptrs.data()));
+          const b2m_patch_match_opts o = ToAbi(options, false, false);
+          py::array_t<float> out(std::vector<py::ssize_t>{queries.shape(0), 3});
+          ThrowOnError(ctx, cost(ctx, &in.probs[0], &o, queries.data(), static_cast<int32_t>(queries.shape(0)),
+                                 out.mutable_data()));
+          return out;
+        },
+        "images"_a, "cameras"_a, "depth_maps"_a, "problem"_a, "queries"_a, "options"_a,
+        "Instrumentation: K8's cost arithmetic, [n x 3] = (photometric cost, geometric cost, depth of the plane at "
+        "(x, y + 1)) for queries [n x 7] = (x, y, depth, nx, ny, nz, source slot)");
   m.def("debug_decode_grey",
         [](const py::bytes& file, int max_image_size, int device) { return DebugDecodeGrey(Engine::Get(device), file, max_image_size); },
         "file"_a, "max_image_size"_a = 3200, "device"_a = 0,
@@ -2174,7 +2461,8 @@ PYBIND11_MODULE(_core, m) {
                         "sift_images"_a = s.sift_images, "sift_keypoints"_a = s.sift_keypoints,
                         "sift_descriptors"_a = s.sift_descriptors, "sift_decoded_bytes"_a = s.sift_decoded_bytes,
                         "sift_decode_images"_a = s.sift_decode_images,
-                        "sift_decode_hardware"_a = s.sift_decode_hardware);
+                        "sift_decode_hardware"_a = s.sift_decode_hardware, "pm_problems"_a = s.pm_problems,
+                        "pm_pixel_updates"_a = s.pm_pixel_updates, "pm_window_samples"_a = s.pm_window_samples);
       })
       .def("reset_stats", [](CoreContext& c) { ThrowOnError(c.Handle(), b2m_reset_stats(c.Handle()));
       });

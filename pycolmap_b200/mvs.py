@@ -1,0 +1,358 @@
+"""PatchMatch stereo over a COLMAP dense workspace: `patch_match_stereo` (R:pipeline/mvs.h:5-90).
+
+A workspace is what upstream's `undistort_images` writes: `images/`, `sparse/` (cameras, images, points3D as .bin or
+.txt) and `stereo/patch-match.cfg`.  This module reads the part of the sparse model PatchMatch needs (pinhole K,
+cam_from_world, image names, each point's xyz and track image ids), the problem list of the configuration file, and
+writes `stereo/depth_maps/<name>.<type>.bin` and `stereo/normal_maps/<name>.<type>.bin` in COLMAP's `Mat<float>`
+layout, which upstream's `stereo_fusion` and `read_array` read.  The maps come from K8 (csrc/patch_match.cu) through
+`_core._patch_match_run`; there is no CPU path.
+"""
+import math
+import os
+import struct
+import sys
+
+import numpy as np
+
+from . import _core
+
+# COLMAP camera model ids and parameter counts (U:sensor/models.h); PatchMatch takes the two pinhole models only.
+_NUM_PARAMS = {0: 3, 1: 4, 2: 4, 3: 5, 4: 8, 5: 8, 6: 12, 7: 5, 8: 4, 9: 5, 10: 12}
+_MODEL_NAMES = ["SIMPLE_PINHOLE", "PINHOLE", "SIMPLE_RADIAL", "RADIAL", "OPENCV", "OPENCV_FISHEYE", "FULL_OPENCV", "FOV",
+                "SIMPLE_RADIAL_FISHEYE", "RADIAL_FISHEYE", "THIN_PRISM_FISHEYE"]
+
+
+def _warn(msg):
+    print(f"W [mvs.py] {msg}", file=sys.stderr, flush=True)
+
+
+# ---- sparse model ----------------------------------------------------------------------------------------------------
+
+def _quat_to_R(q):
+    w, x, y, z = q / np.linalg.norm(q)
+    return np.array([[1 - 2 * (y * y + z * z), 2 * (x * y - w * z), 2 * (x * z + w * y)],
+                     [2 * (x * y + w * z), 1 - 2 * (x * x + z * z), 2 * (y * z - w * x)],
+                     [2 * (x * z - w * y), 2 * (y * z + w * x), 1 - 2 * (x * x + y * y)]])
+
+
+class SparseModel:
+    """cameras {id: (model_id, width, height, params)}, images {id: (name, camera_id, R, t)}, points {id: (xyz,
+    [image ids of the track])}."""
+
+    def __init__(self):
+        self.cameras, self.images, self.points = {}, {}, {}
+
+
+def _read_bin(path):
+    m = SparseModel()
+    with open(os.path.join(path, "cameras.bin"), "rb") as f:
+        for _ in range(struct.unpack("<Q", f.read(8))[0]):
+            cid, model, w, h = struct.unpack("<iiQQ", f.read(24))
+            n = _NUM_PARAMS[model]
+            m.cameras[cid] = (model, w, h, np.array(struct.unpack(f"<{n}d", f.read(8 * n))))
+    with open(os.path.join(path, "images.bin"), "rb") as f:
+        for _ in range(struct.unpack("<Q", f.read(8))[0]):
+            iid = struct.unpack("<i", f.read(4))[0]
+            q = np.array(struct.unpack("<4d", f.read(32)))
+            t = np.array(struct.unpack("<3d", f.read(24)))
+            cid = struct.unpack("<i", f.read(4))[0]
+            name = b""
+            while (c := f.read(1)) != b"\0":
+                name += c
+            n2d = struct.unpack("<Q", f.read(8))[0]
+            f.seek(24 * n2d, 1)
+            m.images[iid] = (name.decode(), cid, _quat_to_R(q), t)
+    with open(os.path.join(path, "points3D.bin"), "rb") as f:
+        for _ in range(struct.unpack("<Q", f.read(8))[0]):
+            pid = struct.unpack("<Q", f.read(8))[0]
+            xyz = np.array(struct.unpack("<3d", f.read(24)))
+            f.seek(3 + 8, 1)
+            n = struct.unpack("<Q", f.read(8))[0]
+            track = np.frombuffer(f.read(8 * n), np.int32).reshape(n, 2)[:, 0]
+            m.points[pid] = (xyz, [int(i) for i in track])
+    return m
+
+
+def _lines(path):
+    with open(path) as f:
+        return [ln.strip() for ln in f if ln.strip() and not ln.lstrip().startswith("#")]
+
+
+def _read_txt(path):
+    m = SparseModel()
+    for ln in _lines(os.path.join(path, "cameras.txt")):
+        e = ln.split()
+        m.cameras[int(e[0])] = (_MODEL_NAMES.index(e[1]), int(e[2]), int(e[3]), np.array([float(v) for v in e[4:]]))
+    # images.txt: two lines per image; the second (the 2-D points) may be empty, so empty lines are kept here
+    with open(os.path.join(path, "images.txt")) as f:
+        rows = [ln.rstrip("\n") for ln in f if not ln.startswith("#")]
+    for k in range(0, len(rows) - 1, 2):
+        e = rows[k].split()
+        if not e:
+            continue
+        q = np.array([float(v) for v in e[1:5]])
+        t = np.array([float(v) for v in e[5:8]])
+        m.images[int(e[0])] = (" ".join(e[9:]), int(e[8]), _quat_to_R(q), t)
+    for ln in _lines(os.path.join(path, "points3D.txt")):
+        e = ln.split()
+        track = [int(v) for v in e[8::2]]
+        m.points[int(e[0])] = (np.array([float(v) for v in e[1:4]]), track)
+    return m
+
+
+def read_sparse(path):
+    """The sparse model under `path`: the .bin files, or the .txt files when the binaries are absent
+    (Reconstruction::Read)."""
+    if all(os.path.isfile(os.path.join(path, f + ".bin")) for f in ("cameras", "images", "points3D")):
+        return _read_bin(path)
+    if all(os.path.isfile(os.path.join(path, f + ".txt")) for f in ("cameras", "images", "points3D")):
+        return _read_txt(path)
+    raise ValueError(f"[mvs.py] Check Failed: {path} holds cameras, images and points3D as .bin or .txt")
+
+
+def pinhole_K(camera):
+    """(fx, fy, cx, cy) of a SIMPLE_PINHOLE or PINHOLE camera; other models are refused (the workspace must be
+    undistorted)."""
+    model, _, _, p = camera
+    if model == 0:
+        return p[0], p[0], p[1], p[2]
+    if model == 1:
+        return p[0], p[1], p[2], p[3]
+    raise ValueError(f"[mvs.py] Check Failed: camera model {_MODEL_NAMES[model]} is PINHOLE or SIMPLE_PINHOLE "
+                     "(patch_match_stereo needs an undistorted workspace)")
+
+
+# ---- problems, source selection, depth ranges --------------------------------------------------------------------------
+
+def _tri_angles(model, ref_id, src_id, point_ids):
+    c1 = -model.images[ref_id][2].T @ model.images[ref_id][3]
+    c2 = -model.images[src_id][2].T @ model.images[src_id][3]
+    X = np.array([model.points[p][0] for p in point_ids])
+    r1, r2 = X - c1, X - c2
+    cos = np.sum(r1 * r2, 1) / (np.linalg.norm(r1, axis=1) * np.linalg.norm(r2, axis=1))
+    return np.degrees(np.arccos(np.clip(cos, -1.0, 1.0)))
+
+
+def auto_sources(model, ref_id, num, min_triangulation_angle):
+    """`__auto__, num`: the images sharing points with the reference, by number of shared points (descending; ties by
+    ascending image id), keeping those whose 75th-percentile triangulation angle over the shared points is at least
+    `min_triangulation_angle` degrees, the first `num` of them."""
+    shared = {}
+    for pid, (_, track) in model.points.items():
+        ids = set(track)
+        if ref_id in ids:
+            for i in ids - {ref_id}:
+                shared.setdefault(i, []).append(pid)
+    order = sorted(shared, key=lambda i: (-len(shared[i]), i))
+    out = []
+    for i in order:
+        if np.percentile(_tri_angles(model, ref_id, i, shared[i]), 75) >= min_triangulation_angle:
+            out.append(i)
+        if len(out) == num:
+            break
+    return out
+
+
+def depth_range(model, image_id):
+    """(depth_min, depth_max) of an image from the camera z of its observed points: the floor(0.01 n)-th and
+    floor(0.99 n)-th smallest, times 0.75 and 1.25; None without points in front of the camera."""
+    _, _, R, t = model.images[image_id]
+    X = np.array([xyz for xyz, track in model.points.values() if image_id in track]).reshape(-1, 3)
+    d = np.sort((X @ R.T + t)[:, 2])
+    d = d[d > 0]
+    if len(d) == 0:
+        return None
+    n = len(d)
+    return float(d[min(int(0.01 * n), n - 1)]) * 0.75, float(d[min(int(0.99 * n), n - 1)]) * 1.25
+
+
+def read_config(path, model, min_triangulation_angle):
+    """patch-match.cfg: pairs of lines, a reference image name, then `__all__`, `__auto__, N` or a comma-separated list
+    of source names.  Returns [(ref image id, [source image ids])]."""
+    by_name = {v[0]: k for k, v in model.images.items()}
+    lines = _lines(path)
+    if len(lines) % 2:
+        raise ValueError(f"[mvs.py] Check Failed: {path} holds pairs of lines (reference, sources)")
+    problems = []
+    for k in range(0, len(lines), 2):
+        ref_name, spec = lines[k], lines[k + 1]
+        if ref_name not in by_name:
+            raise ValueError(f"[mvs.py] Check Failed: reference image {ref_name} of {path} is in the sparse model")
+        ref = by_name[ref_name]
+        if spec == "__all__":
+            src = [i for i in sorted(model.images) if i != ref]
+        elif spec.startswith("__auto__"):
+            parts = [p.strip() for p in spec.split(",")]
+            if len(parts) != 2 or not parts[1].isdigit():
+                raise ValueError(f"[mvs.py] Check Failed: `__auto__, N` in {path}, got `{spec}`")
+            src = auto_sources(model, ref, int(parts[1]), min_triangulation_angle)
+        else:
+            names = [p.strip() for p in spec.split(",") if p.strip()]
+            missing = [n for n in names if n not in by_name]
+            if missing:
+                raise ValueError(f"[mvs.py] Check Failed: source images {missing} of {path} are in the sparse model")
+            src = [by_name[n] for n in names]
+        problems.append((ref, src))
+    return problems
+
+
+# ---- map files -------------------------------------------------------------------------------------------------------
+
+def write_array(path, array):
+    """COLMAP's Mat<float> file: `W&H&C&`, then float32 channel after channel, each row-major."""
+    a = np.asarray(array, np.float32)
+    a3 = a[:, :, None] if a.ndim == 2 else a
+    h, w, c = a3.shape
+    os.makedirs(os.path.dirname(path), exist_ok=True)
+    tmp = path + ".tmp"
+    with open(tmp, "wb") as f:
+        f.write(f"{w}&{h}&{c}&".encode())
+        f.write(np.ascontiguousarray(np.transpose(a3, (2, 0, 1))).tobytes())
+    os.replace(tmp, path)
+
+
+def read_array(path):
+    """The inverse of write_array, as upstream's scripts/python/read_write_dense.py reads it: (H, W) or (H, W, C)."""
+    with open(path, "rb") as f:
+        data = f.read()
+    pos = 0
+    dims = []
+    for _ in range(3):
+        end = data.index(b"&", pos)
+        dims.append(int(data[pos:end]))
+        pos = end + 1
+    w, h, c = dims
+    a = np.frombuffer(data[pos:], np.float32).reshape((w, h, c), order="F")
+    return np.transpose(a, (1, 0, 2)).squeeze()
+
+
+def map_paths(workspace, name, kind):
+    return (os.path.join(workspace, "stereo", "depth_maps", f"{name}.{kind}.bin"),
+            os.path.join(workspace, "stereo", "normal_maps", f"{name}.{kind}.bin"))
+
+
+# ---- images ------------------------------------------------------------------------------------------------------------
+
+def _decode(path, max_image_size, device):
+    """Grey image of a workspace file as K7 makes it: decode (nvJPEG / host PNG), Rec709 grey, FreeImage bilinear
+    rescale when larger than max_image_size."""
+    with open(path, "rb") as f:
+        data = f.read()
+    return _core.debug_decode_grey(data, max_image_size if max_image_size > 0 else 1 << 30, device)
+
+
+def scaled_K(K, orig_wh, new_wh):
+    """K of an image rescaled from orig_wh to new_wh, per axis."""
+    fx, fy, cx, cy = K
+    sx, sy = new_wh[0] / orig_wh[0], new_wh[1] / orig_wh[1]
+    return fx * sx, fy * sy, cx * sx, cy * sy
+
+
+def _run(images, cameras, depth_maps, problems, options, geom, filt):
+    return _core._patch_match_run(images, cameras, depth_maps, problems, options, geom, filt)
+
+
+# ---- controller ----------------------------------------------------------------------------------------------------------
+
+def patch_match_stereo(workspace_path, workspace_format="COLMAP", pmvs_option_name="option-all", options=None,
+                       config_path=""):
+    """Compute depth and normal maps of every reference image listed in the workspace's patch-match.cfg (or
+    `config_path`), with geometric consistency when `options.geom_consistency`: first a photometric pass over every
+    problem (no filter), then the geometric pass, which starts from the reference's photometric maps and reads the
+    sources' photometric depth maps.  Problems whose output files exist are skipped (resume)."""
+    workspace_path = os.fspath(workspace_path)
+    if not os.path.isdir(workspace_path):
+        raise ValueError(f"[mvs.h:20] Check Failed: ExistsDir(workspace_path) : Directory {workspace_path} does not exist.")
+    fmt = workspace_format.lower()
+    if fmt not in ("colmap", "pmvs"):
+        raise ValueError("Invalid `workspace_format` - supported values are 'COLMAP' or 'PMVS'.")
+    if fmt == "pmvs":
+        raise ValueError("[mvs.py] Check Failed: workspace_format == 'COLMAP' (the PMVS workspace format is not supported)")
+    if options is None:
+        options = _core.PatchMatchOptions()
+    elif isinstance(options, dict):
+        options = _core.PatchMatchOptions(options)
+    device = _core._check_patch_match_options(options)
+    if options.write_consistency_graph:
+        raise ValueError("[mvs.py] Check Failed: write_consistency_graph is not supported")
+
+    model = read_sparse(os.path.join(workspace_path, "sparse"))
+    cfg = config_path or os.path.join(workspace_path, "stereo", "patch-match.cfg")
+    problems = read_config(cfg, model, options.min_triangulation_angle)
+    passes = [("photometric", False, False), ("geometric", True, options.filter)] if options.geom_consistency else \
+        [("photometric", False, options.filter)]
+
+    grey = {}  # image id -> (grey uint8, (fx, fy, cx, cy) of the rescaled image); decoded once per call
+
+    def load(iid):
+        if iid not in grey:
+            name, cid, _, _ = model.images[iid]
+            path = os.path.join(workspace_path, "images", name)
+            K = pinhole_K(model.cameras[cid])
+            if not os.path.isfile(path):
+                grey[iid] = None
+            else:
+                img = _decode(path, options.max_image_size, device)
+                cam = model.cameras[cid]
+                grey[iid] = (np.ascontiguousarray(img), scaled_K(K, (cam[1], cam[2]), (img.shape[1], img.shape[0])))
+        return grey[iid]
+
+    for kind, geom, filt in passes:
+        todo = []
+        for ref, src in problems:
+            name = model.images[ref][0]
+            if all(os.path.isfile(p) for p in map_paths(workspace_path, name, kind)):
+                continue
+            if not src:
+                _warn(f"{name}: no source images, skipped")
+                continue
+            if options.depth_min != -1.0 or options.depth_max != -1.0:
+                rng = (options.depth_min, options.depth_max)
+            else:
+                rng = depth_range(model, ref)
+                if rng is None:
+                    _warn(f"{name}: no sparse points in front of the camera to take a depth range from, skipped")
+                    continue
+            ids = [ref] + src
+            missing = [model.images[i][0] for i in ids if load(i) is None]
+            if geom:
+                missing += [p for i in ids for p in map_paths(workspace_path, model.images[i][0], "photometric")[:1]
+                            if not os.path.isfile(p)]
+                missing += [p for p in map_paths(workspace_path, name, "photometric")[1:] if not os.path.isfile(p)]
+            if missing:
+                if not options.allow_missing_files:
+                    raise ValueError(f"[mvs.py] Check Failed: the files of problem {name} exist: missing {missing}")
+                _warn(f"{name}: missing {missing}, skipped")
+                continue
+            todo.append((ref, src, rng))
+        if not todo:
+            continue
+        used = sorted({i for ref, src, _ in todo for i in [ref] + src})
+        slot = {iid: k for k, iid in enumerate(used)}
+        images = [grey[i][0] for i in used]
+        cameras = np.zeros((len(used), 16))
+        for k, i in enumerate(used):
+            _, _, R, t = model.images[i]
+            cameras[k, :4] = grey[i][1]
+            cameras[k, 4:13] = R.ravel()
+            cameras[k, 13:] = t
+        depth_maps = None
+        probs = []
+        for ref, src, (dmin, dmax) in todo:
+            p = dict(ref=slot[ref], image_id=ref, src=[slot[s] for s in src], depth_min=dmin, depth_max=dmax)
+            if geom:
+                dpath, npath = map_paths(workspace_path, model.images[ref][0], "photometric")
+                p["init_depth"] = read_array(dpath)
+                p["init_normal"] = read_array(npath)
+            probs.append(p)
+        if geom:
+            depth_maps = [None] * len(used)
+            for ref, src, _ in todo:
+                for s in src:
+                    if depth_maps[slot[s]] is None:
+                        depth_maps[slot[s]] = read_array(map_paths(workspace_path, model.images[s][0], "photometric")[0])
+        maps = _run(images, cameras, depth_maps, probs, options, geom, filt)
+        for (ref, _, _), (depth, normal) in zip(todo, maps):
+            dpath, npath = map_paths(workspace_path, model.images[ref][0], kind)
+            write_array(dpath, depth)
+            write_array(npath, normal)

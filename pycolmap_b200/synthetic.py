@@ -182,3 +182,154 @@ def homography_pair(rng, width, height, size=1024):
     H12 = c @ P @ R @ np.linalg.inv(c)
     H2 = H12 @ H1
     return render_view(tex, H1, width, height), render_view(tex, H2, width, height), H12
+
+
+# ---------------------------------------------------------------------------------------------
+# Piecewise-planar dense scene (PatchMatch stereo tests and tools/bench_patch_match.py).
+# ---------------------------------------------------------------------------------------------
+
+def planar_scene(rng, n_views, width, height, focal=None, texture_size=512):
+    """A textured back wall and two textured, tilted rectangles in front of it (they occlude the wall and, from some
+    views, each other), seen by `n_views` PINHOLE cameras on a grid near z = 0 looking towards +z.
+
+    Returns dict(planes, cameras [dict(K=(fx, fy, cx, cy), R, t) with x_cam = R x_world + t], width, height)."""
+    focal = focal or 0.9 * width
+    planes = []
+    for centre, normal, half, period in (((0.0, 0.0, 12.0), (0.15, -0.1, -1.0), 12.0, 2),
+                                         ((-1.2, -0.3, 7.0), (0.35, 0.1, -1.0), 1.6, 2),
+                                         ((1.3, 0.6, 8.5), (-0.3, -0.25, -1.0), 1.4, 2)):
+        n = np.asarray(normal, float)
+        n /= np.linalg.norm(n)
+        a1 = np.cross(n, [0.0, 1.0, 0.0])
+        a1 /= np.linalg.norm(a1)
+        a2 = np.cross(n, a1)
+        tex = textured_plane(rng, texture_size, octaves=(period, 2 * period, 4 * period, 8 * period, 16 * period))
+        planes.append(dict(c=np.asarray(centre, float), n=n, a1=a1, a2=a2, half=half, tex=tex))
+    cams = []
+    side = int(np.ceil(np.sqrt(n_views)))
+    for i in range(n_views):
+        gx, gy = i % side, i // side
+        C = np.array([(gx - (side - 1) / 2) * 0.8, (gy - (side - 1) / 2) * 0.6, 0.0]) + rng.normal(0, 0.05, 3)
+        z = np.array([0.0, 0.0, 9.0]) - C
+        z /= np.linalg.norm(z)
+        x = np.cross([0.0, 1.0, 0.0], z)
+        x /= np.linalg.norm(x)
+        y = np.cross(z, x)
+        R = np.stack([x, y, z])
+        cams.append(dict(K=(focal, focal, width / 2.0, height / 2.0), R=R, t=-R @ C))
+    return dict(planes=planes, cameras=cams, width=width, height=height)
+
+
+def render_planar(scene, i):
+    """View i of a planar_scene by ray casting: (grey uint8 [H, W], depth [H, W] (camera z), normal [H, W, 3] (camera
+    frame, facing the camera), plane index [H, W]).  Pixel centres at +0.5."""
+    cam = scene["cameras"][i]
+    W, H = scene["width"], scene["height"]
+    fx, fy, cx, cy = cam["K"]
+    ys, xs = np.mgrid[0:H, 0:W]
+    rays = np.stack([(xs + 0.5 - cx) / fx, (ys + 0.5 - cy) / fy, np.ones((H, W))], -1)  # camera frame, z = 1
+    R, t = cam["R"], cam["t"]
+    C = -R.T @ t
+    rw = rays @ R  # world directions (R^T r)
+    best = np.full((H, W), np.inf)
+    label = np.full((H, W), -1)
+    for k, p in enumerate(scene["planes"]):
+        den = rw @ p["n"]
+        s = ((p["c"] - C) @ p["n"]) / np.where(np.abs(den) > 1e-12, den, np.nan)
+        X = C + s[..., None] * rw
+        u, v = (X - p["c"]) @ p["a1"], (X - p["c"]) @ p["a2"]
+        hit = (s > 0) & (np.abs(u) <= p["half"]) & (np.abs(v) <= p["half"]) & (s < best)
+        best = np.where(hit, s, best)
+        label = np.where(hit, k, label)
+    grey = np.zeros((H, W))
+    normal = np.zeros((H, W, 3))
+    for k, p in enumerate(scene["planes"]):
+        m = label == k
+        X = C + best[m][:, None] * rw[m]
+        size = p["tex"].shape[0]
+        u = np.clip(((X - p["c"]) @ p["a1"] / (2 * p["half"]) + 0.5) * size - 0.5, 0, size - 1.000001)
+        v = np.clip(((X - p["c"]) @ p["a2"] / (2 * p["half"]) + 0.5) * size - 0.5, 0, size - 1.000001)
+        i0, j0 = np.floor(v).astype(np.int64), np.floor(u).astype(np.int64)
+        fv, fu = v - i0, u - j0
+        tex = p["tex"]
+        grey[m] = (tex[i0, j0] * (1 - fu) * (1 - fv) + tex[i0, j0 + 1] * fu * (1 - fv) + tex[i0 + 1, j0] * (1 - fu) * fv
+                   + tex[i0 + 1, j0 + 1] * fu * fv)
+        nc = R @ p["n"]
+        if nc @ np.array([0.0, 0.0, 1.0]) > 0:  # face the camera
+            nc = -nc
+        normal[m] = nc
+    depth = np.where(label >= 0, best, 0.0)  # s is the camera z, since the rays have z = 1 in the camera frame
+    return (np.clip(np.round(255.0 * grey), 0, 255).astype(np.uint8), depth.astype(np.float32),
+            normal.astype(np.float32), label)
+
+
+def write_dense_workspace(path, scene, sources="__auto__, 5", points_per_view=300, seed=0):
+    """A COLMAP dense workspace of a planar_scene under `path`: images/view_XXX.png, sparse/{cameras,images,
+    points3D}.bin (one PINHOLE camera per view; points sampled from the views' true depths, tracked into every view
+    that sees them unoccluded) and stereo/patch-match.cfg with `sources` for every view.  Returns the renders."""
+    import os
+    import struct
+    from PIL import Image
+
+    rng = np.random.default_rng(seed)
+    os.makedirs(os.path.join(path, "images"), exist_ok=True)
+    os.makedirs(os.path.join(path, "sparse"), exist_ok=True)
+    os.makedirs(os.path.join(path, "stereo"), exist_ok=True)
+    n = len(scene["cameras"])
+    renders = [render_planar(scene, i) for i in range(n)]
+    names = [f"view_{i:03d}.png" for i in range(n)]
+    for i in range(n):
+        Image.fromarray(renders[i][0]).save(os.path.join(path, "images", names[i]))
+    W, H = scene["width"], scene["height"]
+    points = []
+    for i in range(n):
+        cam = scene["cameras"][i]
+        d = renders[i][1]
+        ys, xs = rng.integers(0, H, points_per_view), rng.integers(0, W, points_per_view)
+        ok = d[ys, xs] > 0
+        fx, fy, cx, cy = cam["K"]
+        Xc = np.stack([(xs + 0.5 - cx) / fx, (ys + 0.5 - cy) / fy, np.ones(len(xs))], 1) * d[ys, xs][:, None]
+        Xw = (Xc - cam["t"]) @ cam["R"]
+        for X in Xw[ok]:
+            track = []
+            for j in range(n):
+                cj = scene["cameras"][j]
+                y = cj["R"] @ X + cj["t"]
+                u, v = cj["K"][0] * y[0] / y[2] + cj["K"][2], cj["K"][1] * y[1] / y[2] + cj["K"][3]
+                if y[2] > 0 and 0 <= u < W and 0 <= v < H and abs(renders[j][1][int(v), int(u)] - y[2]) < 0.01 * y[2]:
+                    track.append(j + 1)
+            if len(track) >= 2:
+                points.append((X, track))
+    with open(os.path.join(path, "sparse", "cameras.bin"), "wb") as f:
+        f.write(struct.pack("<Q", n))
+        for i, c in enumerate(scene["cameras"]):
+            f.write(struct.pack("<iiQQ4d", i + 1, 1, W, H, *c["K"]))
+    with open(os.path.join(path, "sparse", "images.bin"), "wb") as f:
+        f.write(struct.pack("<Q", n))
+        for i, c in enumerate(scene["cameras"]):
+            f.write(struct.pack("<i4d3di", i + 1, *_rot_to_quat(c["R"]), *c["t"], i + 1))
+            f.write(names[i].encode() + b"\0")
+            f.write(struct.pack("<Q", 0))
+    with open(os.path.join(path, "sparse", "points3D.bin"), "wb") as f:
+        f.write(struct.pack("<Q", len(points)))
+        for k, (X, track) in enumerate(points):
+            f.write(struct.pack("<Q3d3Bd", k + 1, *X, 128, 128, 128, 0.5))
+            f.write(struct.pack("<Q", len(track)))
+            for j in track:
+                f.write(struct.pack("<ii", j, 0))
+    with open(os.path.join(path, "stereo", "patch-match.cfg"), "w") as f:
+        for i in range(n):
+            f.write(f"{names[i]}\n{sources}\n")
+    return renders
+
+
+def _rot_to_quat(R):
+    """(w, x, y, z) of a rotation matrix, w >= 0."""
+    w = np.sqrt(max(0.0, 1.0 + R[0, 0] + R[1, 1] + R[2, 2])) / 2
+    x = np.sqrt(max(0.0, 1.0 + R[0, 0] - R[1, 1] - R[2, 2])) / 2
+    y = np.sqrt(max(0.0, 1.0 - R[0, 0] + R[1, 1] - R[2, 2])) / 2
+    z = np.sqrt(max(0.0, 1.0 - R[0, 0] - R[1, 1] + R[2, 2])) / 2
+    x = np.copysign(x, R[2, 1] - R[1, 2])
+    y = np.copysign(y, R[0, 2] - R[2, 0])
+    z = np.copysign(z, R[1, 0] - R[0, 1])
+    return w, x, y, z
