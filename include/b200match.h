@@ -26,11 +26,11 @@
 extern "C" {
 #endif
 
-#define B2M_ABI_VERSION 8   /* 2: b2m_camera carries 12 parameters, batch estimator; 3: multi-GPU entry points (NCCL);
+#define B2M_ABI_VERSION 9   /* 2: b2m_camera carries 12 parameters, batch estimator; 3: multi-GPU entry points (NCCL);
                              * 4: absolute pose estimation / refinement, b2m_stats.abs_pose_*;
                              * 5: triangulation, b2m_stats.tri_*; 6: SIFT feature extraction, b2m_stats.sift_*;
                              * 7: extraction from encoded / RGB sources, b2m_stats.sift_decode*;
-                             * 8: PatchMatch stereo, b2m_stats.pm_* */
+                             * 8: PatchMatch stereo, b2m_stats.pm_*; 9: stereo fusion, b2m_stats.fusion_* */
 
 /* error codes */
 #define B2M_OK 0
@@ -589,6 +589,66 @@ void b2m_depth_maps_free(b2m_depth_maps* m);
 int b2m_debug_patch_match_cost(b2m_ctx* ctx, const b2m_patch_match_problem* problem, const b2m_patch_match_opts* opts,
                                const float* queries, int32_t n, float* out);
 
+/* ---- stereo fusion (ABI 9) ------------------------------------------------------------------------------------------
+ * What COLMAP's StereoFusion (U:mvs/fusion.cc, recalled) computes from a workspace's depth and normal maps: from every
+ * seed pixel a depth-first traversal through the overlapping images gathers the pixels whose depth, reprojection and
+ * normal agree with the seed's point, and a cluster of at least min_num_pixels pixels becomes one point (per-channel
+ * medians of position, normal and colour; visibility = the images that contributed).  K9 (csrc/fusion.cu): seeds run in
+ * rounds over a 16 x 16 lattice of each image; a round's seeds traverse speculatively and commit by a fixed rule, so that
+ * the result equals the sequential traversal over the committed-seed order it reports (DESIGN.md section 4, K9) and is
+ * a function of the inputs alone.  oracle/fusion.cpp restates it. */
+typedef struct b2m_fusion_image {
+  uint32_t struct_size;
+  int32_t width, height;           /* depth-map size */
+  const float* depth;              /* [height x width], or NULL: the image has no maps (neither a seed nor a target) */
+  const float* normal;             /* [height x width x 3] (camera frame), with depth */
+  const uint8_t* mask;             /* NULL, or [height x width]: pixels where it is 0 are never fused */
+  float P[12];                     /* K [R | t], K scaled per axis by bitmap_scale, row-major 3 x 4 */
+  float inv_P[12];                 /* the top 3 rows of [P; 0 0 0 1]^-1 */
+  float inv_R[9];                  /* R^T */
+  float bitmap_scale[2];           /* depth-map width / camera width, depth-map height / camera height */
+  const int32_t* overlap;          /* n_overlap image indices, in the order the traversal pushes them */
+  int32_t n_overlap;
+  int32_t reserved;
+  b2m_image_source color;          /* the image at camera size: JPEG (decoded by nvJPEG) or host pixels of 1, 3 or 4
+                                    * channels; data NULL = black (allowed for images without maps) */
+} b2m_fusion_image;
+
+typedef struct b2m_fusion_opts {
+  uint32_t struct_size;
+  int32_t min_num_pixels;          /* 5 */
+  int32_t max_num_pixels;          /* 10000 */
+  int32_t max_traversal_depth;     /* 100 */
+  float max_reproj_error;          /* 2, pixels */
+  float max_depth_error;           /* 0.01, relative */
+  float max_normal_error;          /* 10, degrees */
+  float bounding_box[6];           /* min x, y, z, max x, y, z: -FLT_MAX .. FLT_MAX */
+} b2m_fusion_opts;
+void b2m_fusion_opts_default(b2m_fusion_opts* o);
+
+typedef struct b2m_fused_points b2m_fused_points;
+typedef struct b2m_fused_points_view {
+  uint32_t struct_size;
+  int32_t reserved;
+  int64_t n_points;
+  const float* xyz;                /* [n_points x 3] */
+  const float* normals;            /* [n_points x 3] */
+  const uint8_t* colors;           /* [n_points x 3] */
+  const int64_t* vis_off;          /* [n_points + 1]: point k is seen by vis[vis_off[k] .. vis_off[k + 1]) */
+  const int32_t* vis;              /* image indices, ascending per point */
+  const int32_t* seeds;            /* [n_points x 3]: (image, row, col) of the seed that made the point */
+  int64_t n_order;
+  const int32_t* order;            /* [n_order x 4]: every committed seed (image, row, col, round), in commit order,
+                                    * including those whose cluster made no point */
+} b2m_fused_points_view;
+
+/* Fuses n images in one call (nothing stays resident).  A workspace that does not fit in device memory is B2M_ENOMEM
+ * with its size in the message; b2m_request_stop is honoured between rounds. */
+int b2m_stereo_fusion(b2m_ctx* ctx, const b2m_fusion_image* images, int32_t n, const b2m_fusion_opts* opts,
+                      b2m_fused_points** out);
+int b2m_fused_points_get(const b2m_fused_points* p, b2m_fused_points_view* out);
+void b2m_fused_points_free(b2m_fused_points* p);
+
 /* ---- instrumentation ---------------------------------------------------------------- */
 
 /* The cross-check consults m21 only at the columns some row matched (m21[m12[i]]): the column-direction GEMM is run
@@ -650,6 +710,12 @@ typedef struct b2m_stats {
   uint64_t pm_problems;               /* PatchMatch: reference images processed since reset */
   uint64_t pm_pixel_updates;          /* PatchMatch: pixel x sweep steps */
   uint64_t pm_window_samples;         /* PatchMatch: window samples evaluated (one reference / source pixel pair each) */
+  uint64_t fusion_seeds;              /* stereo fusion: committed seeds since reset */
+  uint64_t fusion_traversals;         /* stereo fusion: traversals run (speculative and committing) */
+  uint64_t fusion_pops;               /* stereo fusion: pixels popped by those traversals */
+  uint64_t fusion_rounds;             /* stereo fusion: rounds */
+  uint64_t fusion_deferred;           /* stereo fusion: candidates deferred to a later round */
+  uint64_t fusion_points;             /* stereo fusion: points emitted */
 } b2m_stats;
 int b2m_get_stats(b2m_ctx* ctx, b2m_stats* out);
 int b2m_reset_stats(b2m_ctx* ctx);

@@ -472,6 +472,24 @@ int prepare(b2m_ctx* ctx, ImageIoState** S) {
 
 }  // namespace
 
+namespace b2m {
+int image_io_decode_jpeg(b2m_ctx* ctx, const b2m_image_source& src, const uint8_t** pixels, int* W, int* H,
+                         int* channels) {
+  ImageIoState* S = nullptr;
+  if (int rc = prepare(ctx, &S)) return rc;
+  DecodeCounts c;
+  std::string why;
+  const int rc = decode_jpeg(S->jpeg, S->slot[0], S->side, src, W, H, channels, &c, &why);
+  c.images += rc == B2M_OK;
+  add_counts(ctx, c);
+  if (rc == B2M_EINVAL && !why.empty()) return fail(ctx, rc, "[image_io.cu] source does not decode: " + why);
+  if (rc) return fail(ctx, rc, g_noctx_err);
+  B2M_CUDA_TRY(ctx, cudaStreamSynchronize(S->side));
+  *pixels = S->slot[0].src;
+  return B2M_OK;
+}
+}  // namespace b2m
+
 extern "C" {
 
 int b2m_extract_features_sources(b2m_ctx* ctx, const b2m_image_source* sources, int32_t n, const b2m_extract_opts* opts,

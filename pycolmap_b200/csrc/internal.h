@@ -161,6 +161,10 @@ int sift_extract(b2m_ctx* ctx, const SiftPlan& plan, const uint8_t* img, int64_t
                  b2m_features* F, const float** d_kout);
 // image_io.cu
 void image_io_release(b2m_ctx* ctx);
+// Decodes a B2M_SOURCE_JPEG source with nvJPEG: *pixels = W x H x channels (1 or 3) bytes in device memory, valid until
+// the next decode on this context.
+int image_io_decode_jpeg(b2m_ctx* ctx, const b2m_image_source& src, const uint8_t** pixels, int* W, int* H,
+                         int* channels);
 // patch_match.cu
 void pm_release(b2m_ctx* ctx);
 }  // namespace b2m

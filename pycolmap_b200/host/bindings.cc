@@ -21,6 +21,7 @@
 #include <dlfcn.h>
 
 #include <array>
+#include <cfloat>
 #include <atomic>
 #include <chrono>
 #include <cstring>
@@ -1142,6 +1143,171 @@ py::list PatchMatchRun(b2m_ctx* ctx, const py::list& images, const ArrD& cameras
   return out;
 }
 
+// ---- stereo fusion (R:pipeline/mvs.h:43-90, 193-254; U:mvs/fusion.h StereoFusionOptions) ----------------------------
+// The workspace I/O lives in pycolmap_b200/mvs.py; this is the option class and the device call.
+struct StereoFusionOptions {
+  std::string mask_path = "";
+  int num_threads = -1;
+  int max_image_size = -1;
+  int min_num_pixels = 5;
+  int max_num_pixels = 10000;
+  int max_traversal_depth = 100;
+  double max_reproj_error = 2.0;
+  double max_depth_error = 0.01;
+  double max_normal_error = 10.0;
+  int check_num_images = 50;
+  bool use_cache = false;
+  double cache_size = 32.0;
+  std::pair<std::array<float, 3>, std::array<float, 3>> bounding_box{{-FLT_MAX, -FLT_MAX, -FLT_MAX},
+                                                                      {FLT_MAX, FLT_MAX, FLT_MAX}};
+};
+
+// StereoFusionOptions::Check (U:mvs/fusion.cc), in its order; num_threads, use_cache and cache_size have no effect.
+void CheckStereoFusionOptions(const StereoFusionOptions& o) {
+  auto check = [](bool ok, const char* expr) {
+    if (!ok) throw std::invalid_argument(std::string("[fusion.cc] Check Failed: ") + expr);
+  };
+  check(o.min_num_pixels >= 0, "min_num_pixels >= 0");
+  check(o.min_num_pixels <= o.max_num_pixels, "min_num_pixels <= max_num_pixels");
+  check(o.max_traversal_depth > 0, "max_traversal_depth > 0");
+  check(o.max_reproj_error >= 0.0, "max_reproj_error >= 0");
+  check(o.max_depth_error >= 0.0, "max_depth_error >= 0");
+  check(o.max_normal_error >= 0.0, "max_normal_error >= 0");
+  check(o.check_num_images > 0, "check_num_images > 0");
+  check(o.cache_size > 0.0, "cache_size > 0");
+  check(o.num_threads == -1 || o.num_threads > 0, "num_threads == -1 || num_threads > 0");
+}
+
+// One device call: images [dict(depth, normal, mask, P, inv_P, inv_R, bitmap_scale, overlap, color)] -> dict.
+// color: a JPEG / PNG file's bytes, an (H, W[, C]) uint8 array, or None.
+py::dict StereoFusionRun(b2m_ctx* ctx, const py::list& images, const StereoFusionOptions& options) {
+  CheckStereoFusionOptions(options);
+  const size_t n = images.size();
+  std::vector<b2m_fusion_image> im(n);
+  std::vector<ArrF32> keep_f;
+  std::vector<ArrU8> keep_u;
+  std::vector<std::vector<int32_t>> ov(n);
+  std::vector<std::vector<uint8_t>> bytes(n);
+  std::vector<Pixels> px(n);
+  auto f32 = [&](const py::handle& o, size_t count, float* dst, const char* what) {
+    ArrF32 a = ArrF32::ensure(o);
+    if (!a || static_cast<size_t>(a.size()) != count)
+      throw std::invalid_argument(std::string("[bindings.cc] Check Failed: ") + what + " has " + std::to_string(count) + " values");
+    std::memcpy(dst, a.data(), sizeof(float) * count);
+  };
+  for (size_t i = 0; i < n; ++i) {
+    const py::dict d = images[i];
+    b2m_fusion_image& m = im[i];
+    std::memset(&m, 0, sizeof(m));
+    m.struct_size = sizeof(m);
+    if (d.contains("depth") && !d["depth"].is_none()) {
+      ArrF32 dep = ArrF32::ensure(d["depth"]), nor = ArrF32::ensure(d["normal"]);
+      if (!dep || dep.ndim() != 2 || !nor || nor.ndim() != 3 || nor.shape(0) != dep.shape(0) || nor.shape(1) != dep.shape(1) ||
+          nor.shape(2) != 3)
+        throw std::invalid_argument("[bindings.cc] Check Failed: depth (H, W) and normal (H, W, 3) float32 maps");
+      m.width = static_cast<int32_t>(dep.shape(1));
+      m.height = static_cast<int32_t>(dep.shape(0));
+      m.depth = dep.data();
+      m.normal = nor.data();
+      keep_f.push_back(std::move(dep));
+      keep_f.push_back(std::move(nor));
+      if (d.contains("mask") && !d["mask"].is_none()) {
+        ArrU8 mk = ArrU8::ensure(d["mask"]);
+        if (!mk || mk.ndim() != 2 || mk.shape(0) != m.height || mk.shape(1) != m.width)
+          throw std::invalid_argument("[bindings.cc] Check Failed: a mask has its depth map's size");
+        m.mask = mk.data();
+        keep_u.push_back(std::move(mk));
+      }
+    }
+    f32(d["P"], 12, m.P, "P");
+    f32(d["inv_P"], 12, m.inv_P, "inv_P");
+    f32(d["inv_R"], 9, m.inv_R, "inv_R");
+    f32(d["bitmap_scale"], 2, m.bitmap_scale, "bitmap_scale");
+    ov[i] = d["overlap"].cast<std::vector<int32_t>>();
+    m.overlap = ov[i].data();
+    m.n_overlap = static_cast<int32_t>(ov[i].size());
+    b2m_image_source& s = m.color;
+    const py::object c = d.contains("color") ? py::object(d["color"]) : py::object(py::none());
+    if (py::isinstance<py::bytes>(c)) {
+      const std::string buf = c.cast<std::string>();
+      bytes[i].assign(buf.begin(), buf.end());
+      ImageHeader h;
+      std::string why;
+      if (!ReadImageHeader(bytes[i], &h, &why)) throw std::invalid_argument("[bindings.cc] image " + std::to_string(i) + ": " + why);
+      if (h.format == ImageFormat::PNG) {
+        if (!DecodePng(bytes[i], &px[i], &why)) throw std::invalid_argument("[bindings.cc] image " + std::to_string(i) + ": " + why);
+        s.kind = B2M_SOURCE_PIXELS;
+        s.channels = px[i].channels;
+        s.width = px[i].width;
+        s.height = px[i].height;
+        s.stride = static_cast<int64_t>(px[i].width) * px[i].channels;
+        s.data = px[i].data.data();
+      } else {
+        s.kind = B2M_SOURCE_JPEG;
+        s.data = bytes[i].data();
+        s.size = static_cast<int64_t>(bytes[i].size());
+      }
+    } else if (!c.is_none()) {
+      ArrU8 a = ArrU8::ensure(c);
+      if (!a || (a.ndim() != 2 && a.ndim() != 3) || (a.ndim() == 3 && a.shape(2) != 1 && a.shape(2) != 3 && a.shape(2) != 4))
+        throw std::invalid_argument("[bindings.cc] Check Failed: a color array is (H, W) or (H, W, 1 | 3 | 4) uint8");
+      s.kind = B2M_SOURCE_PIXELS;
+      s.channels = a.ndim() == 3 ? static_cast<int32_t>(a.shape(2)) : 1;
+      s.width = static_cast<int32_t>(a.shape(1));
+      s.height = static_cast<int32_t>(a.shape(0));
+      s.stride = static_cast<int64_t>(s.width) * s.channels;
+      s.data = a.data();
+      keep_u.push_back(std::move(a));
+    }
+  }
+  b2m_fusion_opts o;  // every field set below: no link-time reference to an ABI 9 symbol
+  std::memset(&o, 0, sizeof(o));
+  o.struct_size = sizeof(o);
+  o.min_num_pixels = options.min_num_pixels;
+  o.max_num_pixels = options.max_num_pixels;
+  o.max_traversal_depth = options.max_traversal_depth;
+  o.max_reproj_error = static_cast<float>(options.max_reproj_error);
+  o.max_depth_error = static_cast<float>(options.max_depth_error);
+  o.max_normal_error = static_cast<float>(options.max_normal_error);
+  for (int k = 0; k < 3; ++k) {
+    o.bounding_box[k] = options.bounding_box.first[k];
+    o.bounding_box[3 + k] = options.bounding_box.second[k];
+  }
+  const auto fuse = SiftSymbol<decltype(&b2m_stereo_fusion)>("b2m_stereo_fusion");
+  const auto get = SiftSymbol<decltype(&b2m_fused_points_get)>("b2m_fused_points_get");
+  const auto release = SiftSymbol<decltype(&b2m_fused_points_free)>("b2m_fused_points_free");
+  b2m_fused_points* pts = nullptr;
+  RunInterruptible([&] { ThrowOnError(ctx, fuse(ctx, im.data(), static_cast<int32_t>(n), &o, &pts)); });
+  std::unique_ptr<b2m_fused_points, decltype(release)> guard(pts, release);
+  b2m_fused_points_view v;
+  std::memset(&v, 0, sizeof(v));
+  ThrowOnError(ctx, get(pts, &v));
+  const py::ssize_t N = v.n_points, M = v.n_order;
+  py::array_t<float> xyz(std::vector<py::ssize_t>{N, 3}), nrm(std::vector<py::ssize_t>{N, 3});
+  py::array_t<uint8_t> col(std::vector<py::ssize_t>{N, 3});
+  py::array_t<int32_t> seeds(std::vector<py::ssize_t>{N, 3}), order(std::vector<py::ssize_t>{M, 4});
+  py::array_t<int64_t> voff(N + 1);
+  py::array_t<int32_t> vis(static_cast<py::ssize_t>(N ? v.vis_off[N] : 0));
+  if (N) {
+    std::memcpy(xyz.mutable_data(), v.xyz, sizeof(float) * 3 * N);
+    std::memcpy(nrm.mutable_data(), v.normals, sizeof(float) * 3 * N);
+    std::memcpy(col.mutable_data(), v.colors, 3 * N);
+    std::memcpy(seeds.mutable_data(), v.seeds, sizeof(int32_t) * 3 * N);
+    std::memcpy(vis.mutable_data(), v.vis, sizeof(int32_t) * v.vis_off[N]);
+  }
+  std::memcpy(voff.mutable_data(), v.vis_off, sizeof(int64_t) * (N + 1));
+  if (M) std::memcpy(order.mutable_data(), v.order, sizeof(int32_t) * 4 * M);
+  py::dict out;
+  out["xyz"] = xyz;
+  out["normals"] = nrm;
+  out["colors"] = col;
+  out["vis_off"] = voff;
+  out["vis"] = vis;
+  out["seeds"] = seeds;
+  out["order"] = order;
+  return out;
+}
+
 void CheckCameraMode(const ImageReaderOptions& o, const char* where) {
   if (CameraModelId(o.camera_model) < 0)
     throw std::invalid_argument(std::string("[") + where + "] Invalid camera model: " + o.camera_model);
@@ -1863,6 +2029,45 @@ PYBIND11_MODULE(_core, m) {
         "images"_a, "cameras"_a, "depth_maps"_a, "problem"_a, "queries"_a, "options"_a,
         "Instrumentation: K8's cost arithmetic, [n x 3] = (photometric cost, geometric cost, depth of the plane at "
         "(x, y + 1)) for queries [n x 7] = (x, y, depth, nx, ny, nz, source slot)");
+  OptionsClass<StereoFusionOptions>(m, "StereoFusionOptions")
+      .field("mask_path", &StereoFusionOptions::mask_path,
+             "Path for PNG masks. Same format expected as ImageReaderOptions.")
+      .field("num_threads", &StereoFusionOptions::num_threads, "The number of threads to use during fusion (no effect).")
+      .field("max_image_size", &StereoFusionOptions::max_image_size,
+             "Maximum image size in either dimension (images larger than it are refused).")
+      .field("min_num_pixels", &StereoFusionOptions::min_num_pixels, "Minimum number of fused pixels to produce a point.")
+      .field("max_num_pixels", &StereoFusionOptions::max_num_pixels,
+             "Maximum number of pixels to fuse into a single point.")
+      .field("max_traversal_depth", &StereoFusionOptions::max_traversal_depth,
+             "Maximum depth in consistency graph traversal.")
+      .field("max_reproj_error", &StereoFusionOptions::max_reproj_error, "Maximum relative difference between measured and projected pixel.")
+      .field("max_depth_error", &StereoFusionOptions::max_depth_error, "Maximum relative difference between measured and projected depth.")
+      .field("max_normal_error", &StereoFusionOptions::max_normal_error, "Maximum angular difference in degrees of normals of pixels to be fused.")
+      .field("check_num_images", &StereoFusionOptions::check_num_images,
+             "Number of overlapping images to transitively check for fusing points.")
+      .field("use_cache", &StereoFusionOptions::use_cache, "Flag indicating whether to use LRU cache or pre-load all data (no effect).")
+      .field("cache_size", &StereoFusionOptions::cache_size, "Maximum cache size in gigabytes (no effect).")
+      .field("bounding_box", &StereoFusionOptions::bounding_box, "Bounding box Tuple[min, max]")
+      .Finish();
+  m.def("_check_stereo_fusion_options", [](const StereoFusionOptions& o) { CheckStereoFusionOptions(o); });
+  m.def("_stereo_fusion_run",
+        [](const py::list& images, const StereoFusionOptions& options, int device) {
+          return StereoFusionRun(Engine::Get(device), images, options);
+        },
+        "images"_a, "options"_a, "device"_a = 0, "One stereo fusion device call (pycolmap_b200.mvs)");
+  m.def("_stereo_fusion_stats",
+        [](int device) {
+          b2m_stats st;
+          std::memset(&st, 0, sizeof(st));
+          st.struct_size = sizeof(st);
+          b2m_ctx* ctx = Engine::Get(device);
+          ThrowOnError(ctx, b2m_get_stats(ctx, &st));
+          return py::dict("fusion_seeds"_a = st.fusion_seeds, "fusion_traversals"_a = st.fusion_traversals,
+                          "fusion_pops"_a = st.fusion_pops, "fusion_rounds"_a = st.fusion_rounds,
+                          "fusion_deferred"_a = st.fusion_deferred, "fusion_points"_a = st.fusion_points,
+                          "kernel_launches"_a = st.kernel_launches);
+        },
+        "device"_a = 0, "The stereo fusion counters of the context stereo_fusion uses on this device (since it was created)");
   m.def("debug_decode_grey",
         [](const py::bytes& file, int max_image_size, int device) { return DebugDecodeGrey(Engine::Get(device), file, max_image_size); },
         "file"_a, "max_image_size"_a = 3200, "device"_a = 0,

@@ -356,3 +356,195 @@ def patch_match_stereo(workspace_path, workspace_format="COLMAP", pmvs_option_na
             dpath, npath = map_paths(workspace_path, model.images[ref][0], kind)
             write_array(dpath, depth)
             write_array(npath, normal)
+
+
+# ---- stereo fusion (R:pipeline/mvs.h:43-90; U:mvs/fusion.cc) ----------------------------------------------------------
+
+def fusion_camera(K, R, t, camera_wh, map_wh):
+    """The per-image arrays of stereo fusion, computed in fp64 and rounded to fp32 once: P = K [R | t] with K scaled
+    per axis by bitmap_scale = map size / camera size, inv_P = the top 3 rows of [P; 0 0 0 1]^-1, inv_R = R^T."""
+    sx, sy = map_wh[0] / camera_wh[0], map_wh[1] / camera_wh[1]
+    fx, fy, cx, cy = K
+    Km = np.array([[fx * sx, 0.0, cx * sx], [0.0, fy * sy, cy * sy], [0.0, 0.0, 1.0]])
+    P = Km @ np.c_[np.asarray(R, float), np.asarray(t, float)]
+    inv_P = np.linalg.inv(np.r_[P, [[0.0, 0.0, 0.0, 1.0]]])[:3]
+    return dict(P=P.astype(np.float32), inv_P=inv_P.astype(np.float32), inv_R=np.asarray(R, float).T.astype(np.float32),
+                bitmap_scale=np.array([sx, sy], np.float32))
+
+
+def overlapping_images(model, check_num_images):
+    """Per image index (sparse model order), the indices of the images that share sparse points with it, by number of
+    shared points (descending; ties by ascending index), the first `check_num_images` of them
+    (Model::GetMaxOverlappingImages(check_num_images, 0))."""
+    index = {iid: k for k, iid in enumerate(model.images)}
+    n = len(index)
+    shared = np.zeros((n, n), np.int64)
+    for _, track in model.points.values():
+        ids = sorted({index[i] for i in track if i in index})
+        for a in ids:
+            for b in ids:
+                if a != b:
+                    shared[a, b] += 1
+    out = []
+    for a in range(n):
+        cand = [b for b in range(n) if shared[a, b] > 0]
+        cand.sort(key=lambda b: (-shared[a, b], b))
+        out.append(cand[:check_num_images])
+    return out
+
+
+def read_fusion_config(path):
+    """stereo/fusion.cfg: one image name per line."""
+    return _lines(path)
+
+
+def write_ply(path, xyz, normals, colors):
+    """Binary little-endian PLY: float x y z nx ny nz, uchar red green blue (WriteBinaryPlyPoints)."""
+    n = len(xyz)
+    head = ("ply\nformat binary_little_endian 1.0\nelement vertex %d\nproperty float x\nproperty float y\n"
+            "property float z\nproperty float nx\nproperty float ny\nproperty float nz\nproperty uchar red\n"
+            "property uchar green\nproperty uchar blue\nend_header\n" % n)
+    rec = np.zeros(n, np.dtype([("p", "<f4", 6), ("c", "u1", 3)]))
+    rec["p"][:, :3] = xyz
+    rec["p"][:, 3:] = normals
+    rec["c"] = colors
+    with open(path, "wb") as f:
+        f.write(head.encode())
+        f.write(rec.tobytes())
+
+
+def read_ply(path):
+    """The points of a PLY written by write_ply: (xyz (N, 3) f32, normals (N, 3) f32, colors (N, 3) u8)."""
+    with open(path, "rb") as f:
+        data = f.read()
+    end = data.index(b"end_header\n") + len(b"end_header\n")
+    n = int(next(ln.split()[2] for ln in data[:end].decode().splitlines() if ln.startswith("element vertex")))
+    rec = np.frombuffer(data[end:], np.dtype([("p", "<f4", 6), ("c", "u1", 3)]), count=n)
+    return rec["p"][:, :3].copy(), rec["p"][:, 3:].copy(), rec["c"].copy()
+
+
+def write_points_visibility(path, visibility):
+    """WritePointsVisibility: uint64 count, then per point a uint32 count and its uint32 image indices."""
+    with open(path, "wb") as f:
+        f.write(struct.pack("<Q", len(visibility)))
+        for v in visibility:
+            f.write(struct.pack("<I", len(v)))
+            f.write(np.asarray(v, "<u4").tobytes())
+
+
+def read_points_visibility(path):
+    with open(path, "rb") as f:
+        data = f.read()
+    n = struct.unpack_from("<Q", data, 0)[0]
+    pos, out = 8, []
+    for _ in range(n):
+        m = struct.unpack_from("<I", data, pos)[0]
+        out.append(np.frombuffer(data, "<u4", m, pos + 4).astype(np.int32))
+        pos += 4 + 4 * m
+    return out
+
+
+def _write_points3D(path, xyz, colors, first_id):
+    """points3D.bin of fused points: empty tracks, error -1, ids from first_id."""
+    with open(path, "wb") as f:
+        f.write(struct.pack("<Q", len(xyz)))
+        for k in range(len(xyz)):
+            f.write(struct.pack("<Q3d3Bd", first_id + k, *map(float, xyz[k]), *map(int, colors[k]), -1.0))
+            f.write(struct.pack("<Q", 0))
+
+
+def _fusion_run(images, options, device):
+    return _core._stereo_fusion_run(images, options, device)
+
+
+def stereo_fusion(output_path, workspace_path, workspace_format="COLMAP", pmvs_option_name="option-all",
+                  input_type="geometric", options=None):
+    """Fuse the `input_type` depth and normal maps of the images listed in the workspace's stereo/fusion.cfg into a
+    point cloud (K9, csrc/fusion.cu).  `output_path` is a directory (cameras.bin, images.bin of the workspace and a
+    points3D.bin of the fused points) or a .ply file (plus `<output_path>.vis`).  Returns dict(xyz, normals, colors,
+    visibility [int32 arrays of image indices])."""
+    output_path = os.fspath(output_path)
+    workspace_path = os.fspath(workspace_path)
+    if not os.path.isdir(workspace_path):
+        raise ValueError(f"[mvs.h:56] Check Failed: ExistsDir(workspace_path) : Directory {workspace_path} does not exist.")
+    fmt = workspace_format.lower()
+    if fmt not in ("colmap", "pmvs"):
+        raise ValueError("Invalid `workspace_format` - supported values are 'COLMAP' or 'PMVS'.")
+    if input_type not in ("photometric", "geometric"):
+        raise ValueError("Invalid input type - supported values are 'photometric' and 'geometric'.")
+    if fmt == "pmvs":
+        raise ValueError("[mvs.py] Check Failed: workspace_format == 'COLMAP' (the PMVS workspace format is not supported)")
+    if options is None:
+        options = _core.StereoFusionOptions()
+    elif isinstance(options, dict):
+        options = _core.StereoFusionOptions(options)
+    _core._check_stereo_fusion_options(options)
+    to_dir = os.path.isdir(output_path)
+    if not to_dir and not output_path.lower().endswith(".ply"):
+        raise ValueError(f"[mvs.h:66] Check Failed: HasFileExtension(output_path, \".ply\") : Path {output_path} "
+                         "does not have extension .ply")
+
+    sparse = os.path.join(workspace_path, "sparse")
+    model = read_sparse(sparse)
+    ids = list(model.images)
+    index = {iid: k for k, iid in enumerate(ids)}
+    by_name = {v[0]: k for k, v in model.images.items()}
+    names = read_fusion_config(os.path.join(workspace_path, "stereo", "fusion.cfg"))
+    used = set()
+    for name in names:
+        if name not in by_name:
+            raise ValueError(f"[mvs.py] Check Failed: image {name} of fusion.cfg is in the sparse model")
+        dpath, npath = map_paths(workspace_path, name, input_type)
+        if not (os.path.isfile(dpath) and os.path.isfile(npath)):
+            _warn(f"{name}: no {input_type} depth and normal maps, skipped")
+            continue
+        used.add(index[by_name[name]])
+    overlap = overlapping_images(model, options.check_num_images)
+    images = []
+    for k, iid in enumerate(ids):
+        name, cid, R, t = model.images[iid]
+        cam = model.cameras[cid]
+        K = pinhole_K(cam)
+        entry = dict(overlap=overlap[k], depth=None, normal=None, mask=None, color=None)
+        map_wh = (cam[1], cam[2])
+        if k in used:
+            if options.max_image_size > 0 and max(cam[1], cam[2]) > options.max_image_size:
+                raise ValueError(f"[mvs.py] Check Failed: max_image_size <= 0 or >= the image size ({name}: "
+                                 f"{cam[1]} x {cam[2]}); downsized maps are not supported")
+            dpath, npath = map_paths(workspace_path, name, input_type)
+            depth = np.ascontiguousarray(read_array(dpath), np.float32)
+            normal = np.ascontiguousarray(read_array(npath), np.float32)
+            map_wh = (depth.shape[1], depth.shape[0])
+            entry.update(depth=depth, normal=normal)
+            if options.mask_path:
+                mpath = os.path.join(options.mask_path, name + ".png")
+                if os.path.isfile(mpath):
+                    with open(mpath, "rb") as f:
+                        mk = _core.debug_decode_png(f.read())[:, :, 0]
+                    if mk.shape != depth.shape:
+                        raise ValueError(f"[mvs.py] Check Failed: mask {mpath} ({mk.shape[1]} x {mk.shape[0]}) has the "
+                                         f"depth map's size ({depth.shape[1]} x {depth.shape[0]})")
+                    entry["mask"] = np.ascontiguousarray(mk)
+            ipath = os.path.join(workspace_path, "images", name)
+            if os.path.isfile(ipath):
+                with open(ipath, "rb") as f:
+                    entry["color"] = f.read()
+        entry.update(fusion_camera(K, R, t, (cam[1], cam[2]), map_wh))
+        images.append(entry)
+    r = _fusion_run(images, options, 0)
+    voff = r["vis_off"]
+    vis = [r["vis"][voff[k]:voff[k + 1]] for k in range(len(r["xyz"]))]
+    if to_dir:
+        import shutil
+        for f in ("cameras", "images"):
+            for ext in (".bin", ".txt"):
+                src = os.path.join(sparse, f + ext)
+                if os.path.isfile(src):
+                    shutil.copyfile(src, os.path.join(output_path, f + ext))
+                    break
+        _write_points3D(os.path.join(output_path, "points3D.bin"), r["xyz"], r["colors"],
+                        max(model.points, default=0) + 1)
+    else:
+        write_ply(output_path, r["xyz"], r["normals"], r["colors"])
+        write_points_visibility(output_path + ".vis", vis)
+    return dict(xyz=r["xyz"], normals=r["normals"], colors=r["colors"], visibility=vis)

@@ -220,14 +220,15 @@ def planar_scene(rng, n_views, width, height, focal=None, texture_size=512):
     return dict(planes=planes, cameras=cams, width=width, height=height)
 
 
-def render_planar(scene, i):
+def render_planar(scene, i, offset=0.5):
     """View i of a planar_scene by ray casting: (grey uint8 [H, W], depth [H, W] (camera z), normal [H, W, 3] (camera
-    frame, facing the camera), plane index [H, W]).  Pixel centres at +0.5."""
+    frame, facing the camera), plane index [H, W]).  Rays through pixel (x + offset, y + offset): pixel centres at +0.5
+    by default, integer pixel coordinates (stereo fusion's convention) with offset=0."""
     cam = scene["cameras"][i]
     W, H = scene["width"], scene["height"]
     fx, fy, cx, cy = cam["K"]
     ys, xs = np.mgrid[0:H, 0:W]
-    rays = np.stack([(xs + 0.5 - cx) / fx, (ys + 0.5 - cy) / fy, np.ones((H, W))], -1)  # camera frame, z = 1
+    rays = np.stack([(xs + offset - cx) / fx, (ys + offset - cy) / fy, np.ones((H, W))], -1)  # camera frame, z = 1
     R, t = cam["R"], cam["t"]
     C = -R.T @ t
     rw = rays @ R  # world directions (R^T r)
@@ -320,7 +321,24 @@ def write_dense_workspace(path, scene, sources="__auto__, 5", points_per_view=30
     with open(os.path.join(path, "stereo", "patch-match.cfg"), "w") as f:
         for i in range(n):
             f.write(f"{names[i]}\n{sources}\n")
+    with open(os.path.join(path, "stereo", "fusion.cfg"), "w") as f:
+        for i in range(n):
+            f.write(f"{names[i]}\n")
     return renders
+
+
+def fusion_maps(scene, i, rng=None, noise=0.0, outliers=0.0):
+    """Exact depth and normal maps of view i of a planar_scene in stereo fusion's pixel convention (rays through
+    integer pixel coordinates), as float32 (depth [H, W], normal [H, W, 3]).  With `rng`: depths times (1 + N(0,
+    noise)), and a fraction `outliers` of the valid pixels replaced by depths uniform in [0.5, 2] x the true one."""
+    _, depth, normal, _ = render_planar(scene, i, offset=0.0)
+    depth = depth.astype(np.float64)
+    if rng is not None:
+        valid = depth > 0
+        depth = np.where(valid, depth * (1.0 + rng.normal(0.0, noise, depth.shape)), 0.0)
+        out = valid & (rng.random(depth.shape) < outliers)
+        depth[out] *= rng.uniform(0.5, 2.0, out.sum())
+    return depth.astype(np.float32), np.ascontiguousarray(normal, np.float32)
 
 
 def _rot_to_quat(R):
