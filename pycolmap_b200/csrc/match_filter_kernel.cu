@@ -9,11 +9,17 @@
 //     128-column half of every 256-column tile of image B and each block, a warpgroup issues four
 //     wgmma.mma_async m64n128k32 (u8 x u8 -> s32, A from registers) into one 64-register accumulator bank, waits
 //     and folds it into the slot maxima of that block.  Halves rather than one m64n256 keep the 64 accumulators,
-//     32 A registers and 64 slot maxima of a thread within the 232 registers a consumer thread gets (setmaxnreg).
+//     32 A registers and 64 slot maxima of a thread within the 224 registers a consumer thread gets (setmaxnreg).
 //   * One lane of a producer warpgroup streams B through a 4-stage ring of 32 KiB tiles (TMA, SWIZZLE_128B) and the 32 KiB A
 //     strips through two buffers, so the pipeline runs straight across unit boundaries; barriers are set up
-//     once per launch.  Each B tile serves 256 rows, and A costs shared-memory bandwidth once per unit.
+//     once per launch.  Each B tile serves 256 rows, and A costs shared-memory bandwidth once per unit.  The same
+//     lane decodes the work units: it publishes each unit's tile count beside its A strip, so the consumers read no
+//     global memory.
 //   * While one warpgroup folds its accumulators the other one can use the tensor cores.
+//   * At the end of a unit the consumers only reduce their slot maxima to (best, S1, slot) per row and hand these to
+//     shared memory (two buffers); two more warps of the producer warpgroup take the distance and ratio tests and
+//     write the outputs, while the consumers already issue the next unit's MMAs.  Both consumer warpgroups reach
+//     a unit's end together (they share every B tile), so whatever they do there leaves the tensor cores idle.
 //
 // Filter: instead of an exact running top-2 (4 ALU ops per accumulator) each row keeps 64 "slot maxima".
 // Thread lane l of a quad (q = l % 4) holds the columns 8 j + 2 q + e (j = 0..31, e = 0, 1) of its rows; its
@@ -45,19 +51,22 @@ constexpr int kStripRows = 128;                    // the launchers' max_strips 
 constexpr int kTileN = 256;                        // columns per B tile (the N of one wgmma)
 constexpr int kStages = 4;                         // B-tile ring depth
 constexpr int kABufs = 2;                          // A strips double-buffered across work units
+constexpr int kDecBufs = kABufs;                   // row decisions too (both indexed by the unit count)
 constexpr int kBytesA = kRowsPerItem * kDim;       // 32 KiB per strip
 constexpr int kBytesB = kTileN * kDim;             // 32 KiB per B tile
 constexpr int kBytesBox = kBoxRows * kDim;         // 16 KiB per TMA box
 constexpr int kConsumerWarps = 8;
 constexpr int kOwnSlots = 16;                      // slot maxima per row kept in one thread's registers
 constexpr int kSlots = kOwnSlots * 4;              // 64 slot maxima per row (four lanes of a quad)
-// + a producer warpgroup (one lane issues the TMA loads).  Warps are spread over the SM's four sub-partitions of 16 384
-// registers each: with 288 threads one of them holds three warps, so a thread could use no more than 168 registers, as
-// with 384.  A whole producer warpgroup can hand its registers to the consumers (setmaxnreg): 128 x 40 + 256 x 232 =
-// 64 512 of the SM's 65 536.
+// + a producer warpgroup (one lane issues the TMA loads, two warps finish the row decisions).  Warps are spread over the
+// SM's four sub-partitions of 16 384 registers each: with 288 threads one of them holds three warps, so a thread could
+// use no more than 168 registers, as with 384.  A whole producer warpgroup can hand its registers to the consumers
+// (setmaxnreg): 128 x 56 + 256 x 224 = 64 512 of the SM's 65 536.  The finishing warps need more than 40.
 constexpr int kThreads = (kConsumerWarps + 4) * 32;
-constexpr int kProducerRegs = 40;
-constexpr int kConsumerRegs = 232;
+constexpr int kFinishWarps = 2;                    // warps kConsumerWarps + 1 .. of the producer warpgroup
+constexpr int kFinishRows = kRowsPerItem / (32 * kFinishWarps);   // rows per finishing lane and unit
+constexpr int kProducerRegs = 56;
+constexpr int kConsumerRegs = 224;
 static_assert(kRowsPerItem == kRowPad && kTileN == kRowPad, "images are padded to whole items / column tiles");
 
 struct __align__(8) Barriers {
@@ -65,9 +74,20 @@ struct __align__(8) Barriers {
   uint64_t empty_a[kABufs];
   uint64_t full_b[kStages];
   uint64_t empty_b[kStages];
+  uint64_t full_dec[kDecBufs];
+  uint64_t empty_dec[kDecBufs];
+  int32_t unit_tiles[kABufs];   // n_tiles of the unit whose strip full_a publishes; -1: no unit left
 };
 
-constexpr size_t kSmemBytes = 1024 + kABufs * kBytesA + kStages * kBytesB + sizeof(Barriers);
+// A unit's filter outcome per row, from the consumers to the finishing warps
+struct Decisions {
+  uint32_t best[kRowsPerItem];
+  uint32_t s1[kRowsPerItem];
+  int32_t slot[kRowsPerItem];
+};
+
+constexpr size_t kSmemBytes =
+    1024 + kABufs * kBytesA + kStages * kBytesB + kDecBufs * sizeof(Decisions) + sizeof(Barriers);
 
 // A work unit and the data every warp role derives from its index (pure function of `w`).
 struct Item {
@@ -116,10 +136,12 @@ b2m_k1_filter_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_cons
   // tmap: the resident descriptor set (column tiles; row strips too unless the rows are gathered), tmap_a: the row
   // strips (== tmap except for the gathered column direction, where it covers the gather scratch)
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  // aligned by an offset, so that the compiler still sees a shared-memory pointer (LDS / STS rather than generic)
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint8_t* smA = smem;                                     // [kABufs][32 KiB]
   uint8_t* smB = smem + kABufs * kBytesA;                  // [kStages][32 KiB]
-  Barriers* bars = reinterpret_cast<Barriers*>(smB + kStages * kBytesB);
+  Decisions* decs = reinterpret_cast<Decisions*>(smB + kStages * kBytesB);   // [kDecBufs]
+  Barriers* bars = reinterpret_cast<Barriers*>(decs + kDecBufs);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -137,21 +159,32 @@ b2m_k1_filter_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_cons
       mbar_init(&bars->full_b[s], 1);
       mbar_init(&bars->empty_b[s], kConsumerWarps);
     }
+    for (int s = 0; s < kDecBufs; ++s) {
+      mbar_init(&bars->full_dec[s], kConsumerWarps);
+      mbar_init(&bars->empty_dec[s], kFinishWarps);
+    }
     fence_mbar_init();
   }
   __syncthreads();
 
+  // Every valid unit, in the order of u, takes one A buffer and one decision buffer: unit k of the CTA uses buffer
+  // k % 2 of both, in phase (k / 2) % 2.
   if (warp >= kConsumerWarps) {
-    // ===== TMA producer (one lane) =====
     setmaxnreg_dec<kProducerRegs>();
     if (warp == kConsumerWarps && lane == 0) {
+      // ===== TMA producer (one lane) =====
       uint32_t stage = 0, phase = 0, n_done = 0;
       for (int u = blockIdx.x; u < n_units; u += gridDim.x) {
         const Item it = decode_item(p, u);
-        if (!it.valid || it.n_tiles == 0) continue;
+        if (!it.valid) continue;
         const uint32_t ab = n_done & 1, aph = (n_done >> 1) & 1;
         ++n_done;
         mbar_wait(&bars->empty_a[ab], aph ^ 1);  // the consumers of the unit that used this A buffer hold it in registers
+        bars->unit_tiles[ab] = it.n_tiles;
+        if (it.n_tiles == 0) {   // an empty image B: nothing to load, the consumers still hand its rows on as "no match"
+          mbar_arrive(&bars->full_a[ab]);
+          continue;
+        }
         mbar_arrive_expect_tx(&bars->full_a[ab], kBytesA);
         tma_load_2d(smA + ab * kBytesA, &tmap_a, &bars->full_a[ab], 0, it.rowA);
         tma_load_2d(smA + ab * kBytesA + kBytesBox, &tmap_a, &bars->full_a[ab], 0, it.rowA + kBoxRows);
@@ -167,6 +200,50 @@ b2m_k1_filter_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_cons
           }
         }
       }
+      const uint32_t ab = n_done & 1, aph = (n_done >> 1) & 1;
+      mbar_wait(&bars->empty_a[ab], aph ^ 1);
+      bars->unit_tiles[ab] = -1;   // no unit left: the consumers stop
+      mbar_arrive(&bars->full_a[ab]);
+    } else if (warp > kConsumerWarps && warp <= kConsumerWarps + kFinishWarps) {
+      // ===== finishing warps: distance and ratio tests and the outputs of every row =====
+      const int fw = warp - kConsumerWarps - 1;
+      uint32_t n_done = 0;
+      for (int u = blockIdx.x; u < n_units; u += gridDim.x) {
+        const Item it = decode_item(p, u);
+        if (!it.valid) continue;
+        const uint32_t db = n_done & 1, dph = (n_done >> 1) & 1;
+        ++n_done;
+        const int64_t base = (static_cast<int64_t>(it.pair) * 2 + it.dir) * p.mstride;
+        // the lane's rows r(k) = 32 (kFinishWarps k + fw) + lane, all in flight at once: with few column tiles per
+        // unit these warps must keep up with the MMAs
+        uint32_t b[kFinishRows], s[kFinishRows];
+        int slot[kFinishRows];
+        mbar_wait(&bars->full_dec[db], dph);
+#pragma unroll
+        for (int k = 0; k < kFinishRows; ++k) {
+          const int r = 32 * (kFinishWarps * k + fw) + lane;
+          b[k] = decs[db].best[r];
+          s[k] = decs[db].s1[r];
+          slot[k] = decs[db].slot[r];
+        }
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&bars->empty_dec[db]);
+#pragma unroll
+        for (int k = 0; k < kFinishRows; ++k) {
+          const float fa = __ldg(p.acos_lut + min(b[k], 262144u));
+          const float fb = __ldg(p.acos_lut + min(s[k], 262144u));
+          int32_t out = -1;
+          if (b[k] > 0u && !(fa > p.max_distance) && !(fa >= __fmul_rn(p.max_ratio, fb)))
+            out = -2 - slot[k];  // candidate: resolve exactly
+          const int row = it.row0 + 32 * (kFinishWarps * k + fw) + lane;
+          p.mbuf[base + row] = out;
+          if (out != -1 && row < it.nA) {
+            p.aux[base + row] = make_uint2(b[k], s[k]);
+            const int c = atomicAdd(p.cand_cnt + it.pair * 2 + it.dir, 1);
+            p.cand_rows[base + c] = row | (slot[k] << 24);  // winning slot travels with the row
+          }
+        }
+      }
     }
   } else {
     // ===== consumers: MMA + filter epilogue =====
@@ -178,52 +255,51 @@ b2m_k1_filter_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_cons
     uint32_t acc[64];   // one 64-row block x 128-column half of a tile at a time
 #pragma unroll
     for (int i = 0; i < 64; ++i) acc[i] = 0u;
-    uint32_t stage = 0, phase = 0, n_done = 0;
-    for (int u = blockIdx.x; u < n_units; u += gridDim.x) {
-      const Item it = decode_item(p, u);
-      if (!it.valid) continue;
-      const int n_tiles = it.n_tiles;
+    uint32_t stage = 0, phase = 0;
+#pragma unroll 1
+    for (uint32_t n_done = 0;; ++n_done) {
+      const uint32_t ab = n_done & 1, aph = (n_done >> 1) & 1;   // A buffer and decision buffer
+      mbar_wait(&bars->full_a[ab], aph);
+      const int n_tiles = bars->unit_tiles[ab];
+      if (n_tiles < 0) break;
       uint32_t S[4][kOwnSlots];   // slot maxima of the thread's four rows, [2 blk + i]
 #pragma unroll
       for (int i = 0; i < 4; ++i)
 #pragma unroll
         for (int r = 0; r < kOwnSlots; ++r) S[i][r] = 0u;
+      uint32_t afrag[2][16];
       if (n_tiles > 0) {
-        const uint32_t ab = n_done & 1, aph = (n_done >> 1) & 1;
-        ++n_done;
-        mbar_wait(&bars->full_a[ab], aph);
-        uint32_t afrag[2][16];
 #pragma unroll
         for (int blk = 0; blk < 2; ++blk)
           load_a_frag_sw128(afrag[blk], smA + ab * kBytesA + (wg * 128 + blk * 64) * kDim, warp & 3, lane);
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&bars->empty_a[ab]);   // the strip lives in registers from here on
+      }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&bars->empty_a[ab]);   // the strip lives in registers from here on
 #pragma unroll 1
-        for (int t = 0; t < n_tiles; ++t) {
-          mbar_wait(&bars->full_b[stage], phase);
+      for (int t = 0; t < n_tiles; ++t) {
+        mbar_wait(&bars->full_b[stage], phase);
 #pragma unroll
-          for (int h = 0; h < 2; ++h)
+        for (int h = 0; h < 2; ++h)
 #pragma unroll
-            for (int blk = 0; blk < 2; ++blk) {
-              wgmma_tile_u8_rs(acc, afrag[blk], smem_u32(smB + stage * kBytesB + h * (kBytesB / 2)));
-              if (h == 1 && blk == 1) {
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&bars->empty_b[stage]);   // the MMAs reading this stage have completed
-              }
-              // column 128 h + 8 j + 2 q + e (acc[4 j + 2 i + e], j < 16) = 64 c + 8 (r >> 1) + 2 q + (r & 1) with
-              // c = 2 h + j / 8, r = 2 (j % 8) + e
-#pragma unroll
-              for (int i = 0; i < 2; ++i)
-#pragma unroll
-                for (int r = 0; r < kOwnSlots; ++r) {
-                  const int a0 = 4 * (r >> 1) + 2 * i + (r & 1);
-                  S[2 * blk + i][r] = max(S[2 * blk + i][r], max(acc[a0], acc[a0 + 32]));
-                }
+          for (int blk = 0; blk < 2; ++blk) {
+            wgmma_tile_u8_rs(acc, afrag[blk], smem_u32(smB + stage * kBytesB + h * (kBytesB / 2)));
+            if (h == 1 && blk == 1) {
+              __syncwarp();
+              if (lane == 0) mbar_arrive(&bars->empty_b[stage]);   // the MMAs reading this stage have completed
             }
-          if (++stage == kStages) {
-            stage = 0;
-            phase ^= 1;
+            // column 128 h + 8 j + 2 q + e (acc[4 j + 2 i + e], j < 16) = 64 c + 8 (r >> 1) + 2 q + (r & 1) with
+            // c = 2 h + j / 8, r = 2 (j % 8) + e
+#pragma unroll
+            for (int i = 0; i < 2; ++i)
+#pragma unroll
+              for (int r = 0; r < kOwnSlots; ++r) {
+                const int a0 = 4 * (r >> 1) + 2 * i + (r & 1);
+                S[2 * blk + i][r] = max(S[2 * blk + i][r], max(acc[a0], acc[a0 + 32]));
+              }
           }
+        if (++stage == kStages) {
+          stage = 0;
+          phase ^= 1;
         }
       }
       // (largest, second largest) over the 64 slot maxima of each row, multiset semantics, lowest slot id on ties:
@@ -269,19 +345,13 @@ b2m_k1_filter_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_cons
           s = s1[i];
           slot = sstar[i];
         }
-      const float fa = __ldg(p.acos_lut + min(b, 262144u));
-      const float fb = __ldg(p.acos_lut + min(s, 262144u));
-      int32_t out = -1;
-      if (b > 0u && !(fa > p.max_distance) && !(fa >= __fmul_rn(p.max_ratio, fb)))
-        out = -2 - slot;  // candidate: resolve exactly
-      const int64_t base = (static_cast<int64_t>(it.pair) * 2 + it.dir) * p.mstride;
-      const int row = it.row0 + row_in_unit + 64 * (q >> 1) + 8 * (q & 1);
-      p.mbuf[base + row] = out;
-      if (out != -1 && row < it.nA) {
-        p.aux[base + row] = make_uint2(b, s);
-        const int k = atomicAdd(p.cand_cnt + it.pair * 2 + it.dir, 1);
-        p.cand_rows[base + k] = row | (slot << 24);  // winning slot travels with the row
-      }
+      const int r_dec = row_in_unit + 64 * (q >> 1) + 8 * (q & 1);
+      mbar_wait(&bars->empty_dec[ab], aph ^ 1);   // the finishing warps are done with the unit before last
+      decs[ab].best[r_dec] = b;
+      decs[ab].s1[r_dec] = s;
+      decs[ab].slot[r_dec] = slot;
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&bars->full_dec[ab]);
     }
   }
 }
