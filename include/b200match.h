@@ -26,11 +26,12 @@
 extern "C" {
 #endif
 
-#define B2M_ABI_VERSION 9   /* 2: b2m_camera carries 12 parameters, batch estimator; 3: multi-GPU entry points (NCCL);
+#define B2M_ABI_VERSION 10  /* 2: b2m_camera carries 12 parameters, batch estimator; 3: multi-GPU entry points (NCCL);
                              * 4: absolute pose estimation / refinement, b2m_stats.abs_pose_*;
                              * 5: triangulation, b2m_stats.tri_*; 6: SIFT feature extraction, b2m_stats.sift_*;
                              * 7: extraction from encoded / RGB sources, b2m_stats.sift_decode*;
-                             * 8: PatchMatch stereo, b2m_stats.pm_*; 9: stereo fusion, b2m_stats.fusion_* */
+                             * 8: PatchMatch stereo, b2m_stats.pm_*; 9: stereo fusion, b2m_stats.fusion_*;
+                             * 10: image undistortion, b2m_stats.undistort_* */
 
 /* error codes */
 #define B2M_OK 0
@@ -649,6 +650,63 @@ int b2m_stereo_fusion(b2m_ctx* ctx, const b2m_fusion_image* images, int32_t n, c
 int b2m_fused_points_get(const b2m_fused_points* p, b2m_fused_points_view* out);
 void b2m_fused_points_free(b2m_fused_points* p);
 
+/* ---- image undistortion (ABI 10) ------------------------------------------------------------------------------------
+ * What COLMAP's image undistorter (U:image/undistortion.cc, U:image/warp.cc, U:sensor/bitmap.cc; recalled, DESIGN.md
+ * section 4 K10) does to one image: UndistortCamera gives a PINHOLE camera (ROI, scale from the distorted image's
+ * borders, max_image_size), and the image is warped at the source resolution (pinhole CamFromImg of each pixel centre,
+ * the distorted ImgFromCam, fp64 bilinear interpolation on FreeImage's bottom-up rows, black outside), then rescaled to
+ * the undistorted size with FreeImage's bilinear filter.  K10 (csrc/undistort.cu); oracle/undistort.py restates it. */
+typedef struct b2m_undistort_opts {
+  uint32_t struct_size;
+  int32_t max_image_size;          /* -1: no limit; > 0: the undistorted image is scaled down to fit */
+  double blank_pixels;             /* 0: no blank pixel in the output; 1: every input pixel in the output */
+  double min_scale;                /* 0.2 */
+  double max_scale;                /* 2 */
+  double roi_min_x, roi_min_y;     /* 0, 0: the region of interest as fractions of the image size */
+  double roi_max_x, roi_max_y;     /* 1, 1 */
+} b2m_undistort_opts;
+void b2m_undistort_opts_default(b2m_undistort_opts* o);
+
+/* UndistortCamera on the host (no device work; ctx may be NULL, the message then goes to b2m_last_error(NULL)).  Bad
+ * options or camera: B2M_EINVAL. */
+int b2m_undistort_camera(b2m_ctx* ctx, const b2m_undistort_opts* opts, const b2m_camera* camera, b2m_camera* out);
+
+#define B2M_UNDISTORT_JPEG 0     /* the undistorted image as a JPEG file (nvJPEG, quality 100, 4:2:0) */
+#define B2M_UNDISTORT_PIXELS 1   /* the undistorted image as width x height x 3 RGB bytes */
+typedef struct b2m_undistort_item {
+  uint32_t struct_size;
+  int32_t output;                  /* B2M_UNDISTORT_* */
+  b2m_camera camera;               /* the distorted camera; the decoded source must be its size */
+  b2m_image_source source;         /* JPEG, or host pixels of 1 (grey, replicated), 3 or 4 (alpha dropped) channels;
+                                    * the mask fields are ignored */
+} b2m_undistort_item;
+
+typedef struct b2m_undistorted b2m_undistorted;
+typedef struct b2m_undistorted_view {
+  uint32_t struct_size;
+  int32_t status;                  /* B2M_OK, or B2M_EINVAL when the source does not decode or is not its camera's size */
+  const char* error;               /* why, when status != B2M_OK */
+  int32_t width, height;           /* the undistorted size */
+  b2m_camera camera;               /* the undistorted (PINHOLE) camera */
+  int64_t size;                    /* bytes at data: the JPEG file, or width x height x 3 */
+  const uint8_t* data;
+} b2m_undistorted_view;
+
+/* Undistorts n items in order, one after the other on the device.  An item whose source does not decode or has not its
+ * camera's size gets an error status and the others go on; a bad argument fails the call.  A call whose largest image
+ * does not fit in device memory is B2M_ENOMEM with its size in the message.  Read with b2m_undistorted_get, release with
+ * b2m_undistorted_free. */
+int b2m_undistort_images(b2m_ctx* ctx, const b2m_undistort_item* items, int32_t n, const b2m_undistort_opts* opts,
+                         b2m_undistorted** out);
+int b2m_undistorted_get(const b2m_undistorted* r, int32_t k, b2m_undistorted_view* out);
+void b2m_undistorted_free(b2m_undistorted* r);
+
+/* The RGB image b2m_undistort_images encodes for `item` (whatever its output kind).  With rgb == NULL only *width /
+ * *height are set; otherwise rgb holds width x height x 3 bytes.  Exists so that tests can hold K10 against
+ * oracle/undistort.py exactly. */
+int b2m_debug_undistort_pixels(b2m_ctx* ctx, const b2m_undistort_item* item, const b2m_undistort_opts* opts, uint8_t* rgb,
+                               int32_t* width, int32_t* height);
+
 /* ---- instrumentation ---------------------------------------------------------------- */
 
 /* The cross-check consults m21 only at the columns some row matched (m21[m12[i]]): the column-direction GEMM is run
@@ -716,6 +774,9 @@ typedef struct b2m_stats {
   uint64_t fusion_rounds;             /* stereo fusion: rounds */
   uint64_t fusion_deferred;           /* stereo fusion: candidates deferred to a later round */
   uint64_t fusion_points;             /* stereo fusion: points emitted */
+  uint64_t undistort_images;          /* undistortion: images undistorted since reset */
+  uint64_t undistort_pixels;          /* undistortion: output pixels */
+  uint64_t undistort_encoded_bytes;   /* undistortion: bytes of the JPEG files written by nvJPEG */
 } b2m_stats;
 int b2m_get_stats(b2m_ctx* ctx, b2m_stats* out);
 int b2m_reset_stats(b2m_ctx* ctx);

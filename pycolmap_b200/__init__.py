@@ -21,7 +21,8 @@ try:
     from ._core import Normalization, Sift, SiftExtractionOptions  # noqa: F401
     from ._core import PatchMatchOptions  # noqa: F401
     from ._core import StereoFusionOptions  # noqa: F401
-    from .mvs import patch_match_stereo, stereo_fusion  # noqa: F401
+    from ._core import CopyType, UndistortCameraOptions  # noqa: F401
+    from .mvs import patch_match_stereo, stereo_fusion, undistort_images  # noqa: F401
     from ._core import (Context, Database, DatabaseTransaction, Device, ExhaustiveMatchingOptions,  # noqa: F401
                         RANSACOptions, Results, Rigid3d, Rotation3d, SequentialMatchingOptions,
                         SiftMatchingOptions, SpatialMatchingOptions, TwoViewGeometry,

@@ -746,6 +746,7 @@ void b2m_destroy(b2m_ctx* ctx) {
   sift_release(ctx);
   image_io_release(ctx);
   pm_release(ctx);
+  undistort_release(ctx);
   verify_release(ctx);
   delete ctx;
 }

@@ -59,29 +59,34 @@ __device__ __forceinline__ uint8_t round_byte(double v) {
   return static_cast<uint8_t>(r < 0 ? 0 : (r > 255 ? 255 : r));
 }
 
-// horizontalFilter: src sw x h -> dst dw x h
-__global__ void b2m_rescale_h_kernel(const uint8_t* __restrict__ src, int sw, int h, Weights t, int dw,
+// horizontalFilter: src sw x h -> dst dw x h, `channels` interleaved bytes per pixel, each filtered on its own
+__global__ void b2m_rescale_h_kernel(const uint8_t* __restrict__ src, int sw, int h, int channels, Weights t, int dw,
                                      uint8_t* __restrict__ dst) {
   const int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
-  if (i >= static_cast<int64_t>(dw) * h) return;
-  const int y = static_cast<int>(i / dw), x = static_cast<int>(i % dw);
-  const uint8_t* row = src + static_cast<int64_t>(y) * sw + t.left[x];
+  if (i >= static_cast<int64_t>(dw) * h * channels) return;
+  const int64_t px = i / channels;
+  const int c = static_cast<int>(i % channels);
+  const int y = static_cast<int>(px / dw), x = static_cast<int>(px % dw);
+  const uint8_t* row = src + (static_cast<int64_t>(y) * sw + t.left[x]) * channels + c;
   const double* w = t.w + t.off[x];
   double v = 0.0;
-  for (int k = 0; k < t.count[x]; ++k) v = __dadd_rn(v, __dmul_rn(w[k], static_cast<double>(row[k])));
+  for (int k = 0; k < t.count[x]; ++k)
+    v = __dadd_rn(v, __dmul_rn(w[k], static_cast<double>(row[static_cast<int64_t>(k) * channels])));
   dst[i] = round_byte(v);
 }
 
-// verticalFilter: src w x sh -> dst w x dh
-__global__ void b2m_rescale_v_kernel(const uint8_t* __restrict__ src, int w, int sh, Weights t, int dh,
+// verticalFilter: src w x sh -> dst w x dh, `channels` interleaved bytes per pixel
+__global__ void b2m_rescale_v_kernel(const uint8_t* __restrict__ src, int w, int sh, int channels, Weights t, int dh,
                                      uint8_t* __restrict__ dst) {
   const int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
-  if (i >= static_cast<int64_t>(w) * dh) return;
-  const int y = static_cast<int>(i / w), x = static_cast<int>(i % w);
-  const uint8_t* col = src + static_cast<int64_t>(t.left[y]) * w + x;
+  const int64_t rowlen = static_cast<int64_t>(w) * channels;
+  if (i >= rowlen * dh) return;
+  const int y = static_cast<int>(i / rowlen);
+  const int64_t xc = i % rowlen;
+  const uint8_t* col = src + static_cast<int64_t>(t.left[y]) * rowlen + xc;
   const double* wt = t.w + t.off[y];
   double v = 0.0;
-  for (int k = 0; k < t.count[y]; ++k) v = __dadd_rn(v, __dmul_rn(wt[k], static_cast<double>(col[static_cast<int64_t>(k) * w])));
+  for (int k = 0; k < t.count[y]; ++k) v = __dadd_rn(v, __dmul_rn(wt[k], static_cast<double>(col[static_cast<int64_t>(k) * rowlen])));
   dst[i] = round_byte(v);
 }
 
@@ -123,6 +128,8 @@ struct Nvjpeg {
   nvjpegHandle_t hybrid = nullptr, hw = nullptr;
   nvjpegJpegState_t hybrid_state = nullptr, hw_rgb = nullptr, hw_y = nullptr;
   nvjpegJpegStream_t hw_stream = nullptr;
+  nvjpegEncoderState_t enc_state = nullptr;  // K10's JPEG output, on the hybrid handle
+  nvjpegEncoderParams_t enc_params = nullptr;
   bool hw_tried = false;
   void drop_hw() {
     if (hw_stream) nvjpegJpegStreamDestroy(hw_stream);
@@ -135,6 +142,8 @@ struct Nvjpeg {
   }
   ~Nvjpeg() {
     drop_hw();
+    if (enc_params) nvjpegEncoderParamsDestroy(enc_params);
+    if (enc_state) nvjpegEncoderStateDestroy(enc_state);
     if (hybrid_state) nvjpegJpegStateDestroy(hybrid_state);
     if (hybrid) nvjpegDestroy(hybrid);
   }
@@ -142,9 +151,8 @@ struct Nvjpeg {
 
 // The buffers one image goes through between decode and SIFT.
 struct Slot {
-  DeviceArray<uint8_t> src, grey, tmp, small;
-  DeviceArray<int> tab_i;
-  DeviceArray<double> tab_w;
+  DeviceArray<uint8_t> src, grey, small;
+  RescaleBufs rs;
 };
 
 constexpr int kSlots = 3;  // images decoded ahead of K6, plus the one K6 reads
@@ -200,6 +208,46 @@ AxisTable bilinear_table(int dst, int src) {
   return t;
 }
 
+}  // namespace
+
+int rescale_bilinear(b2m_ctx* ctx, const uint8_t* src, int W, int H, int channels, int w, int h, RescaleBufs& b,
+                     uint8_t* dst, cudaStream_t st) {
+  const AxisTable tx = bilinear_table(w, W), ty = bilinear_table(h, H);
+  // one upload: [left | count | off] of x, then of y; weights of x then of y
+  std::vector<int> ti;
+  for (const AxisTable* t : {&tx, &ty}) {
+    ti.insert(ti.end(), t->left.begin(), t->left.end());
+    ti.insert(ti.end(), t->count.begin(), t->count.end());
+    ti.insert(ti.end(), t->off.begin(), t->off.end());
+  }
+  std::vector<double> tw(tx.w);
+  tw.insert(tw.end(), ty.w.begin(), ty.w.end());
+  B2M_CUDA_TRY(ctx, b.tab_i.ensure(ti.size()));
+  B2M_CUDA_TRY(ctx, b.tab_w.ensure(tw.size()));
+  B2M_CUDA_TRY(ctx, cudaMemcpyAsync(b.tab_i, ti.data(), sizeof(int) * ti.size(), cudaMemcpyHostToDevice, st));
+  B2M_CUDA_TRY(ctx, cudaMemcpyAsync(b.tab_w, tw.data(), sizeof(double) * tw.size(), cudaMemcpyHostToDevice, st));
+  const int* di = b.tab_i;
+  const Weights wx{di, di + w, di + 2 * w, b.tab_w};
+  const int* dy = di + 3 * w;
+  const Weights wy{dy, dy + h, dy + 2 * h, b.tab_w + tx.w.size()};
+  const int c = channels;
+  if (static_cast<int64_t>(w) * H <= static_cast<int64_t>(h) * W) {  // xy filtering: horizontal pass first
+    B2M_CUDA_TRY(ctx, b.tmp.ensure(static_cast<size_t>(w) * H * c));
+    b2m_rescale_h_kernel<<<blocks_for(static_cast<int64_t>(w) * H * c, 256), 256, 0, st>>>(src, W, H, c, wx, w, b.tmp);
+    b2m_rescale_v_kernel<<<blocks_for(static_cast<int64_t>(w) * h * c, 256), 256, 0, st>>>(b.tmp, w, H, c, wy, h, dst);
+  } else {  // yx filtering
+    B2M_CUDA_TRY(ctx, b.tmp.ensure(static_cast<size_t>(W) * h * c));
+    b2m_rescale_v_kernel<<<blocks_for(static_cast<int64_t>(W) * h * c, 256), 256, 0, st>>>(src, W, H, c, wy, h, b.tmp);
+    b2m_rescale_h_kernel<<<blocks_for(static_cast<int64_t>(w) * h * c, 256), 256, 0, st>>>(b.tmp, W, h, c, wx, w, dst);
+  }
+  B2M_CUDA_TRY(ctx, cudaGetLastError());
+  // the weight tables are pageable host memory read by the copies above: they live until the stream is done
+  B2M_CUDA_TRY(ctx, cudaStreamSynchronize(st));
+  return B2M_OK;
+}
+
+namespace {
+
 ImageIoState* state_of(b2m_ctx* ctx) {
   if (!ctx->image_io_state) ctx->image_io_state = new ImageIoState();
   return static_cast<ImageIoState*>(ctx->image_io_state);
@@ -231,14 +279,19 @@ struct Decoded {
 
 // JPEG -> RGB interleaved (or the Y plane of a one-component file) in s.src on `st`.  B2M_EINVAL with *why when the
 // file does not decode.  Errors of the CUDA runtime go to the calling thread's error (fail with a null context).
-int decode_jpeg(Nvjpeg& J, Slot& s, cudaStream_t st, const b2m_image_source& src, int* W, int* H, int* channels,
-                DecodeCounts* cnt, std::string* why) {
+int ensure_hybrid(Nvjpeg& J) {
   if (!J.hybrid) {
     if (nvjpegCreateSimple(&J.hybrid) != NVJPEG_STATUS_SUCCESS)
       return fail(nullptr, B2M_ECUDA, "[image_io.cu] nvjpegCreateSimple failed");
     if (nvjpegJpegStateCreate(J.hybrid, &J.hybrid_state) != NVJPEG_STATUS_SUCCESS)
       return fail(nullptr, B2M_ECUDA, "[image_io.cu] nvjpegJpegStateCreate failed");
   }
+  return B2M_OK;
+}
+
+int decode_jpeg(Nvjpeg& J, Slot& s, cudaStream_t st, const b2m_image_source& src, int* W, int* H, int* channels,
+                DecodeCounts* cnt, std::string* why) {
+  if (int rc = ensure_hybrid(J)) return rc;
   if (!J.hw_tried) {  // a GPU or driver without JPEG engines refuses the backend: the hybrid one does every file
     J.hw_tried = true;
     const bool ok = nvjpegCreateEx(NVJPEG_BACKEND_HARDWARE, nullptr, nullptr, 0, &J.hw) == NVJPEG_STATUS_SUCCESS &&
@@ -316,38 +369,10 @@ int decode_grey(Nvjpeg& J, Slot& s, cudaStream_t st, const b2m_image_source& src
     return B2M_EINVAL;
   }
   if (w != W || h != H) {
-    const AxisTable tx = bilinear_table(w, W), ty = bilinear_table(h, H);
-    // one upload: [left | count | off] of x, then of y; weights of x then of y
-    std::vector<int> ti;
-    for (const AxisTable* t : {&tx, &ty}) {
-      ti.insert(ti.end(), t->left.begin(), t->left.end());
-      ti.insert(ti.end(), t->count.begin(), t->count.end());
-      ti.insert(ti.end(), t->off.begin(), t->off.end());
-    }
-    std::vector<double> tw(tx.w);
-    tw.insert(tw.end(), ty.w.begin(), ty.w.end());
-    B2M_CUDA_TRY(nullptr, s.tab_i.ensure(ti.size()));
-    B2M_CUDA_TRY(nullptr, s.tab_w.ensure(tw.size()));
-    B2M_CUDA_TRY(nullptr, cudaMemcpyAsync(s.tab_i, ti.data(), sizeof(int) * ti.size(), cudaMemcpyHostToDevice, st));
-    B2M_CUDA_TRY(nullptr, cudaMemcpyAsync(s.tab_w, tw.data(), sizeof(double) * tw.size(), cudaMemcpyHostToDevice, st));
-    const int* di = s.tab_i;
-    const Weights wx{di, di + w, di + 2 * w, s.tab_w};
-    const int* dy = di + 3 * w;
-    const Weights wy{dy, dy + h, dy + 2 * h, s.tab_w + tx.w.size()};
     B2M_CUDA_TRY(nullptr, s.small.ensure(static_cast<size_t>(w) * h));
-    if (static_cast<int64_t>(w) * H <= static_cast<int64_t>(h) * W) {  // xy filtering: horizontal pass first
-      B2M_CUDA_TRY(nullptr, s.tmp.ensure(static_cast<size_t>(w) * H));
-      b2m_rescale_h_kernel<<<blocks_for(static_cast<int64_t>(w) * H, 256), 256, 0, st>>>(s.grey, W, H, wx, w, s.tmp);
-      b2m_rescale_v_kernel<<<blocks_for(static_cast<int64_t>(w) * h, 256), 256, 0, st>>>(s.tmp, w, H, wy, h, s.small);
-    } else {  // yx filtering
-      B2M_CUDA_TRY(nullptr, s.tmp.ensure(static_cast<size_t>(W) * h));
-      b2m_rescale_v_kernel<<<blocks_for(static_cast<int64_t>(W) * h, 256), 256, 0, st>>>(s.grey, W, H, wy, h, s.tmp);
-      b2m_rescale_h_kernel<<<blocks_for(static_cast<int64_t>(w) * h, 256), 256, 0, st>>>(s.tmp, W, h, wx, w, s.small);
-    }
+    if (int rc = rescale_bilinear(nullptr, s.grey, W, H, 1, w, h, s.rs, s.small, st)) return rc;
     cnt->launches += 2;
-    B2M_CUDA_TRY(nullptr, cudaGetLastError());
     d->grey = s.small;
-    // the weight tables are pageable host memory read by the copies above: they live until the stream is done
   }
   B2M_CUDA_TRY(nullptr, cudaStreamSynchronize(st));
   return B2M_OK;
@@ -486,6 +511,50 @@ int image_io_decode_jpeg(b2m_ctx* ctx, const b2m_image_source& src, const uint8_
   if (rc) return fail(ctx, rc, g_noctx_err);
   B2M_CUDA_TRY(ctx, cudaStreamSynchronize(S->side));
   *pixels = S->slot[0].src;
+  return B2M_OK;
+}
+
+int image_io_encode_jpeg(b2m_ctx* ctx, const uint8_t* rgb, int W, int H, cudaStream_t st, std::vector<uint8_t>* out) {
+  ImageIoState* S = nullptr;
+  if (int rc = prepare(ctx, &S)) return rc;
+  Nvjpeg& J = S->jpeg;
+  if (int rc = ensure_hybrid(J)) return fail(ctx, rc, g_noctx_err);
+  auto check = [&](nvjpegStatus_t e, const char* what) {
+    return e == NVJPEG_STATUS_SUCCESS ? B2M_OK
+                                      : fail(ctx, B2M_ECUDA, std::string("[image_io.cu] ") + what + " failed (status " +
+                                                                 std::to_string(static_cast<int>(e)) + ")");
+  };
+  if (!J.enc_state) {  // FreeImage's JPEG_QUALITYSUPERB with its default 4:2:0 subsampling
+    nvjpegEncoderParams_t p = nullptr;
+    nvjpegEncoderState_t e = nullptr;
+    int rc = check(nvjpegEncoderParamsCreate(J.hybrid, &p, st), "nvjpegEncoderParamsCreate");
+    if (!rc) rc = check(nvjpegEncoderParamsSetQuality(p, 100, st), "nvjpegEncoderParamsSetQuality");
+    if (!rc) rc = check(nvjpegEncoderParamsSetSamplingFactors(p, NVJPEG_CSS_420, st), "nvjpegEncoderParamsSetSamplingFactors");
+    if (!rc) rc = check(nvjpegEncoderStateCreate(J.hybrid, &e, st), "nvjpegEncoderStateCreate");
+    if (rc) {  // nothing half-built is kept: the next call starts over
+      if (e) nvjpegEncoderStateDestroy(e);
+      if (p) nvjpegEncoderParamsDestroy(p);
+      return rc;
+    }
+    J.enc_params = p;
+    J.enc_state = e;
+  }
+  nvjpegImage_t img;
+  memset(&img, 0, sizeof(img));
+  img.channel[0] = const_cast<uint8_t*>(rgb);
+  img.pitch[0] = static_cast<size_t>(W) * 3;
+  if (int rc = check(nvjpegEncodeImage(J.hybrid, J.enc_state, J.enc_params, &img, NVJPEG_INPUT_RGBI, W, H, st),
+                     "nvjpegEncodeImage"))
+    return rc;
+  size_t n = 0;
+  if (int rc = check(nvjpegEncodeRetrieveBitstream(J.hybrid, J.enc_state, nullptr, &n, st), "nvjpegEncodeRetrieveBitstream"))
+    return rc;
+  B2M_CUDA_TRY(ctx, cudaStreamSynchronize(st));
+  out->resize(n);
+  if (int rc = check(nvjpegEncodeRetrieveBitstream(J.hybrid, J.enc_state, out->data(), &n, st), "nvjpegEncodeRetrieveBitstream"))
+    return rc;
+  B2M_CUDA_TRY(ctx, cudaStreamSynchronize(st));
+  out->resize(n);
   return B2M_OK;
 }
 }  // namespace b2m

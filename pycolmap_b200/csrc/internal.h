@@ -134,6 +134,7 @@ struct b2m_ctx {
   void* sift_state = nullptr;    // b2m::SiftState (sift.cu): pyramid, gradient and keypoint buffers
   void* image_io_state = nullptr;  // b2m::ImageIoState (image_io.cu): nvJPEG handles, decode and rescale buffers
   void* pm_state = nullptr;        // b2m::PmState (patch_match.cu): the resident images, depth maps and map buffers
+  void* undistort_state = nullptr; // b2m::UndistortState (undistort.cu): source, warp and rescale buffers
 };
 
 namespace b2m {
@@ -165,8 +166,22 @@ void image_io_release(b2m_ctx* ctx);
 // the next decode on this context.
 int image_io_decode_jpeg(b2m_ctx* ctx, const b2m_image_source& src, const uint8_t** pixels, int* W, int* H,
                          int* channels);
+// FreeImage's bilinear Rescale (FILTER_BILINEAR) of a W x H image of `channels` interleaved bytes per pixel into dst
+// (w x h x channels) on `st`: fp64 weight tables per axis, two separable passes through an 8-bit intermediate, the
+// pass order chosen from the aspect ratio as CResizeEngine::scale does.  Returns once the result is on the device.
+struct RescaleBufs {
+  DeviceArray<uint8_t> tmp;
+  DeviceArray<int> tab_i;
+  DeviceArray<double> tab_w;
+};
+int rescale_bilinear(b2m_ctx* ctx, const uint8_t* src, int W, int H, int channels, int w, int h, RescaleBufs& b,
+                     uint8_t* dst, cudaStream_t st);
+// nvJPEG's encoder on a W x H RGB interleaved device image, quality 100, 4:2:0: the file's bytes in *out.
+int image_io_encode_jpeg(b2m_ctx* ctx, const uint8_t* rgb, int W, int H, cudaStream_t st, std::vector<uint8_t>* out);
 // patch_match.cu
 void pm_release(b2m_ctx* ctx);
+// undistort.cu
+void undistort_release(b2m_ctx* ctx);
 }  // namespace b2m
 
 struct b2m_features {

@@ -1308,6 +1308,154 @@ py::dict StereoFusionRun(b2m_ctx* ctx, const py::list& images, const StereoFusio
   return out;
 }
 
+// ---- image undistortion (R:pipeline/images.h:96-261; U:image/undistortion.h UndistortCameraOptions) ----------------
+// The workspace I/O lives in pycolmap_b200/mvs.py; this is the option class, the camera and the device call.
+struct UndistortCameraOptions {
+  double blank_pixels = 0.0;
+  double min_scale = 0.2;
+  double max_scale = 2.0;
+  int max_image_size = -1;
+  double roi_min_x = 0.0;
+  double roi_min_y = 0.0;
+  double roi_max_x = 1.0;
+  double roi_max_y = 1.0;
+};
+
+enum class CopyType { COPY = 0, SOFT_LINK = 1, HARD_LINK = 2 };  // U:util/misc.h FileCopyType
+
+// UndistortCameraOptions' checks (UndistortCamera's CHECKs, U:image/undistortion.cc), in their order.
+void CheckUndistortOptions(const UndistortCameraOptions& o) {
+  auto check = [](bool ok, const char* expr) {
+    if (!ok) throw std::invalid_argument(std::string("[undistortion.cc] Check Failed: ") + expr);
+  };
+  check(o.blank_pixels >= 0, "blank_pixels >= 0");
+  check(o.blank_pixels <= 1, "blank_pixels <= 1");
+  check(o.min_scale > 0.0, "min_scale > 0");
+  check(o.min_scale <= o.max_scale, "min_scale <= max_scale");
+  check(o.max_image_size != 0, "max_image_size != 0");
+  check(o.roi_min_x >= 0.0, "roi_min_x >= 0");
+  check(o.roi_min_y >= 0.0, "roi_min_y >= 0");
+  check(o.roi_max_x <= 1.0, "roi_max_x <= 1");
+  check(o.roi_max_y <= 1.0, "roi_max_y <= 1");
+  check(o.roi_min_x < o.roi_max_x, "roi_min_x < roi_max_x");
+  check(o.roi_min_y < o.roi_max_y, "roi_min_y < roi_max_y");
+}
+
+b2m_undistort_opts ToAbi(const UndistortCameraOptions& o) {
+  b2m_undistort_opts a;  // every field set here: no link-time reference to an ABI 10 symbol
+  std::memset(&a, 0, sizeof(a));
+  a.struct_size = sizeof(a);
+  a.max_image_size = o.max_image_size;
+  a.blank_pixels = o.blank_pixels;
+  a.min_scale = o.min_scale;
+  a.max_scale = o.max_scale;
+  a.roi_min_x = o.roi_min_x;
+  a.roi_min_y = o.roi_min_y;
+  a.roi_max_x = o.roi_max_x;
+  a.roi_max_y = o.roi_max_y;
+  return a;
+}
+
+py::dict AbiCameraToDict(const b2m_camera& c) {
+  const int n = b2m::cam::num_params(c.model);
+  return py::dict("model"_a = c.model, "width"_a = c.width, "height"_a = c.height,
+                  "params"_a = std::vector<double>(c.params, c.params + std::max(n, 0)));
+}
+
+py::dict UndistortCameraPy(const UndistortCameraOptions& options, const py::object& camera) {
+  CheckUndistortOptions(options);
+  const b2m_camera c = CameraFromPython(camera);
+  const b2m_undistort_opts o = ToAbi(options);
+  const auto und = SiftSymbol<decltype(&b2m_undistort_camera)>("b2m_undistort_camera");
+  b2m_camera out;
+  std::memset(&out, 0, sizeof(out));
+  if (und(nullptr, &o, &c, &out) != B2M_OK) throw std::invalid_argument(b2m_last_error(nullptr));
+  return AbiCameraToDict(out);
+}
+
+// The device source of a JPEG / PNG file's bytes: JPEG goes whole to the device, PNG is decoded here into *px (which
+// must outlive the source).  False with *why for a file that is neither, or a PNG this reader does not decode.
+bool SourceFromFile(const std::vector<uint8_t>& bytes, Pixels* px, b2m_image_source* s, std::string* why) {
+  ImageHeader h;
+  if (!ReadImageHeader(bytes, &h, why)) return false;
+  if (h.format == ImageFormat::PNG) {
+    if (!DecodePng(bytes, px, why)) return false;
+    s->kind = B2M_SOURCE_PIXELS;
+    s->channels = px->channels;
+    s->width = px->width;
+    s->height = px->height;
+    s->stride = static_cast<int64_t>(px->width) * px->channels;
+    s->data = px->data.data();
+  } else {
+    s->kind = B2M_SOURCE_JPEG;
+    s->data = bytes.data();
+    s->size = static_cast<int64_t>(bytes.size());
+  }
+  return true;
+}
+
+// One device call over items [(file bytes, camera, "jpeg" | "pixels")]: per item dict(status, error, camera, data), data
+// = the JPEG file's bytes or an (H, W, 3) uint8 array.  PNG files are decoded here; a file that is neither JPEG nor a
+// PNG this reader decodes gets an error status, like one the device cannot decode.
+py::list UndistortRun(b2m_ctx* ctx, const py::list& items, const UndistortCameraOptions& options) {
+  CheckUndistortOptions(options);
+  const size_t n = items.size();
+  std::vector<std::vector<uint8_t>> bytes(n);
+  std::vector<Pixels> px(n);
+  std::vector<std::string> host_error(n);
+  std::vector<b2m_undistort_item> it;
+  std::vector<size_t> which;
+  for (size_t i = 0; i < n; ++i) {
+    const py::tuple t = items[i];
+    const std::string buf = t[0].cast<std::string>();
+    bytes[i].assign(buf.begin(), buf.end());
+    const std::string kind = t[2].cast<std::string>();
+    if (kind != "jpeg" && kind != "pixels")
+      throw std::invalid_argument("[bindings.cc] Check Failed: output is \"jpeg\" or \"pixels\", got \"" + kind + "\"");
+    b2m_undistort_item m;
+    std::memset(&m, 0, sizeof(m));
+    m.struct_size = sizeof(m);
+    m.output = kind == "jpeg" ? B2M_UNDISTORT_JPEG : B2M_UNDISTORT_PIXELS;
+    m.camera = CameraFromPython(t[1]);
+    if (!SourceFromFile(bytes[i], &px[i], &m.source, &host_error[i])) continue;
+    it.push_back(m);
+    which.push_back(i);
+  }
+  const b2m_undistort_opts o = ToAbi(options);
+  const auto run = SiftSymbol<decltype(&b2m_undistort_images)>("b2m_undistort_images");
+  const auto get = SiftSymbol<decltype(&b2m_undistorted_get)>("b2m_undistorted_get");
+  const auto release = SiftSymbol<decltype(&b2m_undistorted_free)>("b2m_undistorted_free");
+  b2m_undistorted* r = nullptr;
+  RunInterruptible([&] { ThrowOnError(ctx, run(ctx, it.data(), static_cast<int32_t>(it.size()), &o, &r)); });
+  std::unique_ptr<b2m_undistorted, decltype(release)> guard(r, release);
+  std::vector<py::object> out(n, py::none());
+  for (size_t j = 0; j < which.size(); ++j) {
+    b2m_undistorted_view v;
+    std::memset(&v, 0, sizeof(v));
+    ThrowOnError(ctx, get(r, static_cast<int32_t>(j), &v));
+    py::object data = py::none();
+    if (v.status == B2M_OK) {
+      if (it[j].output == B2M_UNDISTORT_JPEG) {
+        data = py::bytes(reinterpret_cast<const char*>(v.data), static_cast<size_t>(v.size));
+      } else {
+        py::array_t<uint8_t> a(std::vector<py::ssize_t>{v.height, v.width, 3});
+        std::memcpy(a.mutable_data(), v.data, static_cast<size_t>(v.size));
+        data = a;
+      }
+    }
+    out[which[j]] = py::dict("status"_a = v.status, "error"_a = std::string(v.error ? v.error : ""),
+                             "camera"_a = AbiCameraToDict(v.camera), "data"_a = data);
+  }
+  py::list res;
+  for (size_t i = 0; i < n; ++i) {
+    if (out[i].is_none())
+      out[i] = py::dict("status"_a = static_cast<int>(B2M_EINVAL), "error"_a = host_error[i], "camera"_a = py::none(),
+                        "data"_a = py::none());
+    res.append(out[i]);
+  }
+  return res;
+}
+
 void CheckCameraMode(const ImageReaderOptions& o, const char* where) {
   if (CameraModelId(o.camera_model) < 0)
     throw std::invalid_argument(std::string("[") + where + "] Invalid camera model: " + o.camera_model);
@@ -2068,6 +2216,86 @@ PYBIND11_MODULE(_core, m) {
                           "kernel_launches"_a = st.kernel_launches);
         },
         "device"_a = 0, "The stereo fusion counters of the context stereo_fusion uses on this device (since it was created)");
+  OptionsClass<UndistortCameraOptions>(m, "UndistortCameraOptions")
+      .field("blank_pixels", &UndistortCameraOptions::blank_pixels,
+             "The amount of blank pixels in the undistorted image in the range [0, 1].")
+      .field("min_scale", &UndistortCameraOptions::min_scale, "Minimum scale change of camera used to satisfy the blank pixel constraint.")
+      .field("max_scale", &UndistortCameraOptions::max_scale, "Maximum scale change of camera used to satisfy the blank pixel constraint.")
+      .field("max_image_size", &UndistortCameraOptions::max_image_size,
+             "Maximum image size in terms of width or height of the undistorted camera.")
+      .field("roi_min_x", &UndistortCameraOptions::roi_min_x, "The 4 factors in the range [0, 1] that define the ROI (region of interest) in original image. The bounding box pixel coordinates are calculated as (roi_min_x * Width, roi_min_y * Height) and (roi_max_x * Width, roi_max_y * Height).")
+      .field("roi_min_y", &UndistortCameraOptions::roi_min_y)
+      .field("roi_max_x", &UndistortCameraOptions::roi_max_x)
+      .field("roi_max_y", &UndistortCameraOptions::roi_max_y)
+      .Finish();
+  auto copy_type = py::enum_<CopyType>(m, "CopyType")
+                       .value("copy", CopyType::COPY)
+                       .value("soft-link", CopyType::SOFT_LINK)
+                       .value("hard-link", CopyType::HARD_LINK);
+  copy_type.def(py::init([](const std::string& name) {
+                  if (name == "copy") return CopyType::COPY;
+                  if (name == "soft-link") return CopyType::SOFT_LINK;
+                  if (name == "hard-link") return CopyType::HARD_LINK;
+                  throw std::invalid_argument("Invalid string value " + name + " for enum CopyType");
+                }),
+                "name"_a);
+  py::implicitly_convertible<std::string, CopyType>();
+  m.def("_check_undistort_options", [](const UndistortCameraOptions& o) { CheckUndistortOptions(o); });
+  m.def("_undistort_camera", &UndistortCameraPy, "options"_a, "camera"_a,
+        "UndistortCamera on the host: the PINHOLE camera (dict) of the undistorted image");
+  m.def("_undistort_run",
+        [](const py::list& items, const UndistortCameraOptions& options, int device) {
+          return UndistortRun(Engine::Get(device), items, options);
+        },
+        "items"_a, "options"_a, "device"_a = 0, "One undistortion device call (pycolmap_b200.mvs)");
+  m.def("_undistort_stats",
+        [](int device) {
+          b2m_stats st;
+          std::memset(&st, 0, sizeof(st));
+          st.struct_size = sizeof(st);
+          b2m_ctx* ctx = Engine::Get(device);
+          ThrowOnError(ctx, b2m_get_stats(ctx, &st));
+          return py::dict("undistort_images"_a = st.undistort_images, "undistort_pixels"_a = st.undistort_pixels,
+                          "undistort_encoded_bytes"_a = st.undistort_encoded_bytes, "kernel_launches"_a = st.kernel_launches);
+        },
+        "device"_a = 0, "The undistortion counters of the context undistort_images uses on this device");
+  m.def("debug_undistort_pixels",
+        [](const py::bytes& file, const py::object& camera, const UndistortCameraOptions& options, int device) {
+          CheckUndistortOptions(options);
+          const std::string buf = file;
+          const std::vector<uint8_t> bytes(buf.begin(), buf.end());
+          Pixels px;
+          std::string why;
+          b2m_undistort_item it;
+          std::memset(&it, 0, sizeof(it));
+          it.struct_size = sizeof(it);
+          it.output = B2M_UNDISTORT_PIXELS;
+          it.camera = CameraFromPython(camera);
+          if (!SourceFromFile(bytes, &px, &it.source, &why)) throw std::invalid_argument("[bindings.cc] " + why);
+          const b2m_undistort_opts o = ToAbi(options);
+          const auto dbg = SiftSymbol<decltype(&b2m_debug_undistort_pixels)>("b2m_debug_undistort_pixels");
+          b2m_ctx* ctx = Engine::Get(device);
+          int32_t w = 0, h = 0;
+          ThrowOnError(ctx, dbg(ctx, &it, &o, nullptr, &w, &h));
+          py::array_t<uint8_t> out(std::vector<py::ssize_t>{h, w, 3});
+          ThrowOnError(ctx, dbg(ctx, &it, &o, out.mutable_data(), &w, &h));
+          return out;
+        },
+        "file"_a, "camera"_a, "options"_a, "device"_a = 0,
+        "Instrumentation: b2m_debug_undistort_pixels, the RGB image undistort_images encodes for this JPEG / PNG "
+        "file's bytes under `camera`");
+  m.def("_encode_png",
+        [](const py::array_t<uint8_t, py::array::c_style | py::array::forcecast>& a) {
+          if (a.ndim() != 2 && a.ndim() != 3) throw std::invalid_argument("[bindings.cc] Check Failed: an (H, W[, C]) image");
+          const int c = a.ndim() == 3 ? static_cast<int>(a.shape(2)) : 1;
+          std::vector<uint8_t> png;
+          {
+            py::gil_scoped_release release;
+            png = EncodePng(a.data(), static_cast<int>(a.shape(1)), static_cast<int>(a.shape(0)), c);
+          }
+          return py::bytes(reinterpret_cast<const char*>(png.data()), png.size());
+        },
+        "image"_a, "An 8-bit PNG file of an (H, W), (H, W, 3) or (H, W, 4) uint8 image");
   m.def("debug_decode_grey",
         [](const py::bytes& file, int max_image_size, int device) { return DebugDecodeGrey(Engine::Get(device), file, max_image_size); },
         "file"_a, "max_image_size"_a = 3200, "device"_a = 0,

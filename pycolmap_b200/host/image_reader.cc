@@ -50,6 +50,8 @@ std::vector<double> CsvToDoubles(const std::string& csv) {
 struct Zlib {
   int (*uncompress)(unsigned char*, unsigned long*, const unsigned char*, unsigned long) = nullptr;
   unsigned long (*crc32)(unsigned long, const unsigned char*, unsigned int) = nullptr;
+  unsigned long (*compress_bound)(unsigned long) = nullptr;
+  int (*compress2)(unsigned char*, unsigned long*, const unsigned char*, unsigned long, int) = nullptr;
 };
 
 const Zlib& zlib() {
@@ -63,7 +65,10 @@ const Zlib& zlib() {
     if (!lib) throw std::runtime_error("[image_reader.cc] cannot load libz.so.1 (needed to decode PNG files)");
     r.uncompress = reinterpret_cast<decltype(r.uncompress)>(dlsym(lib, "uncompress"));
     r.crc32 = reinterpret_cast<decltype(r.crc32)>(dlsym(lib, "crc32"));
-    if (!r.uncompress || !r.crc32) throw std::runtime_error("[image_reader.cc] libz.so.1 lacks uncompress / crc32");
+    r.compress_bound = reinterpret_cast<decltype(r.compress_bound)>(dlsym(lib, "compressBound"));
+    r.compress2 = reinterpret_cast<decltype(r.compress2)>(dlsym(lib, "compress2"));
+    if (!r.uncompress || !r.crc32 || !r.compress_bound || !r.compress2)
+      throw std::runtime_error("[image_reader.cc] libz.so.1 lacks uncompress / crc32 / compressBound / compress2");
     return r;
   }();
   return z;
@@ -385,6 +390,41 @@ bool DecodePng(const std::vector<uint8_t>& bytes, Pixels* out, std::string* why)
     }
   }
   return true;
+}
+
+std::vector<uint8_t> EncodePng(const uint8_t* pixels, int width, int height, int channels) {
+  if (width <= 0 || height <= 0 || (channels != 1 && channels != 3 && channels != 4))
+    throw std::invalid_argument("[image_reader.cc] Check Failed: a PNG is non-empty with 1, 3 or 4 channels");
+  const size_t row = static_cast<size_t>(width) * channels;
+  std::vector<uint8_t> raw((row + 1) * height);
+  for (int y = 0; y < height; ++y) {  // filter type 0 on every row
+    raw[(row + 1) * y] = 0;
+    std::memcpy(&raw[(row + 1) * y + 1], pixels + row * y, row);
+  }
+  unsigned long n = zlib().compress_bound(raw.size());
+  std::vector<uint8_t> idat(n);
+  if (zlib().compress2(idat.data(), &n, raw.data(), raw.size(), 6) != 0)
+    throw std::runtime_error("[image_reader.cc] compress2 failed");
+  idat.resize(n);
+  std::vector<uint8_t> out = {0x89, 'P', 'N', 'G', '\r', '\n', 0x1a, '\n'};
+  auto chunk = [&out](const char* type, const uint8_t* body, size_t len) {
+    const uint8_t be[4] = {uint8_t(len >> 24), uint8_t(len >> 16), uint8_t(len >> 8), uint8_t(len)};
+    out.insert(out.end(), be, be + 4);
+    const size_t at = out.size();
+    out.insert(out.end(), type, type + 4);
+    out.insert(out.end(), body, body + len);
+    const uint32_t crc = static_cast<uint32_t>(zlib().crc32(0, &out[at], static_cast<unsigned>(4 + len)));
+    const uint8_t bc[4] = {uint8_t(crc >> 24), uint8_t(crc >> 16), uint8_t(crc >> 8), uint8_t(crc)};
+    out.insert(out.end(), bc, bc + 4);
+  };
+  const uint32_t w = static_cast<uint32_t>(width), h = static_cast<uint32_t>(height);
+  const uint8_t color_type = channels == 1 ? 0 : (channels == 3 ? 2 : 6);
+  const uint8_t ihdr[13] = {uint8_t(w >> 24), uint8_t(w >> 16), uint8_t(w >> 8), uint8_t(w), uint8_t(h >> 24),
+                            uint8_t(h >> 16), uint8_t(h >> 8), uint8_t(h), 8, color_type, 0, 0, 0};
+  chunk("IHDR", ihdr, 13);
+  chunk("IDAT", idat.data(), idat.size());
+  chunk("IEND", nullptr, 0);
+  return out;
 }
 
 std::vector<uint8_t> ToGrey(const Pixels& p) {

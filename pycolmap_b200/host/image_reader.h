@@ -58,6 +58,9 @@ struct Pixels {
   std::vector<uint8_t> data;  // packed rows
 };
 bool DecodePng(const std::vector<uint8_t>& bytes, Pixels* out, std::string* why);
+// An 8-bit PNG of packed rows (1 grey, 3 RGB or 4 RGBA channels), compressed with zlib's compress2 (level 6), every
+// row with filter type 0.
+std::vector<uint8_t> EncodePng(const uint8_t* pixels, int width, int height, int channels);
 // FreeImage's ConvertToGreyscale on host pixels (the same Rec709 rule as the device kernel); 1 channel passes through
 std::vector<uint8_t> ToGrey(const Pixels& p);
 

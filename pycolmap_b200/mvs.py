@@ -37,10 +37,13 @@ def _quat_to_R(q):
 
 class SparseModel:
     """cameras {id: (model_id, width, height, params)}, images {id: (name, camera_id, R, t)}, points {id: (xyz,
-    [image ids of the track])}."""
+    [image ids of the track])}.  What a writer needs besides: image_raw {id: (qvec, tvec as read, xy (n, 2) float64,
+    point3D ids (n,) int64)}, point_raw {id: (rgb (3,) uint8, error, track (n, 2) int64 of (image id, point2D
+    index))}."""
 
     def __init__(self):
         self.cameras, self.images, self.points = {}, {}, {}
+        self.image_raw, self.point_raw = {}, {}
 
 
 def _read_bin(path):
@@ -60,16 +63,19 @@ def _read_bin(path):
             while (c := f.read(1)) != b"\0":
                 name += c
             n2d = struct.unpack("<Q", f.read(8))[0]
-            f.seek(24 * n2d, 1)
+            p2d = np.frombuffer(f.read(24 * n2d), np.dtype([("xy", "<f8", 2), ("id", "<i8")]))
             m.images[iid] = (name.decode(), cid, _quat_to_R(q), t)
+            m.image_raw[iid] = (q, t, p2d["xy"].astype(np.float64).reshape(-1, 2), p2d["id"].astype(np.int64))
     with open(os.path.join(path, "points3D.bin"), "rb") as f:
         for _ in range(struct.unpack("<Q", f.read(8))[0]):
             pid = struct.unpack("<Q", f.read(8))[0]
             xyz = np.array(struct.unpack("<3d", f.read(24)))
-            f.seek(3 + 8, 1)
+            rgb = np.frombuffer(f.read(3), np.uint8).copy()
+            err = struct.unpack("<d", f.read(8))[0]
             n = struct.unpack("<Q", f.read(8))[0]
-            track = np.frombuffer(f.read(8 * n), np.int32).reshape(n, 2)[:, 0]
-            m.points[pid] = (xyz, [int(i) for i in track])
+            full = np.frombuffer(f.read(8 * n), np.int32).reshape(n, 2).astype(np.int64)
+            m.points[pid] = (xyz, [int(i) for i in full[:, 0]])
+            m.point_raw[pid] = (rgb, err, full)
     return m
 
 
@@ -93,10 +99,15 @@ def _read_txt(path):
         q = np.array([float(v) for v in e[1:5]])
         t = np.array([float(v) for v in e[5:8]])
         m.images[int(e[0])] = (" ".join(e[9:]), int(e[8]), _quat_to_R(q), t)
+        p2d = rows[k + 1].split()
+        xy = np.array([[float(p2d[j]), float(p2d[j + 1])] for j in range(0, len(p2d), 3)], np.float64).reshape(-1, 2)
+        m.image_raw[int(e[0])] = (q, t, xy, np.array([int(p2d[j + 2]) for j in range(0, len(p2d), 3)], np.int64))
     for ln in _lines(os.path.join(path, "points3D.txt")):
         e = ln.split()
         track = [int(v) for v in e[8::2]]
         m.points[int(e[0])] = (np.array([float(v) for v in e[1:4]]), track)
+        m.point_raw[int(e[0])] = (np.array([int(v) for v in e[4:7]], np.uint8), float(e[7]),
+                                  np.array([int(v) for v in e[8:]], np.int64).reshape(-1, 2))
     return m
 
 
@@ -548,3 +559,209 @@ def stereo_fusion(output_path, workspace_path, workspace_format="COLMAP", pmvs_o
         write_ply(output_path, r["xyz"], r["normals"], r["colors"])
         write_points_visibility(output_path + ".vis", vis)
     return dict(xyz=r["xyz"], normals=r["normals"], colors=r["colors"], visibility=vis)
+
+
+# ---- image undistortion (R:pipeline/images.h:96-261; U:image/undistortion.cc COLMAPUndistorter, recalled) -----------
+
+def write_sparse_bin(path, model):
+    """cameras.bin, images.bin and points3D.bin of `model` (a read_sparse model with its raw fields) under `path`, in
+    the model's order.  Poses are written from the raw qvec / tvec, so they carry the input's values bit for bit."""
+    os.makedirs(path, exist_ok=True)
+    with open(os.path.join(path, "cameras.bin"), "wb") as f:
+        f.write(struct.pack("<Q", len(model.cameras)))
+        for cid, (mid, w, h, p) in model.cameras.items():
+            f.write(struct.pack("<iiQQ", cid, mid, w, h) + np.asarray(p, "<f8").tobytes())
+    with open(os.path.join(path, "images.bin"), "wb") as f:
+        f.write(struct.pack("<Q", len(model.images)))
+        for iid, (name, cid, _, _) in model.images.items():
+            q, t, xy, ids = model.image_raw[iid]
+            f.write(struct.pack("<i4d3di", iid, *map(float, q), *map(float, t), cid) + name.encode() + b"\0")
+            rec = np.zeros(len(xy), np.dtype([("xy", "<f8", 2), ("id", "<i8")]))
+            rec["xy"], rec["id"] = xy, ids
+            f.write(struct.pack("<Q", len(xy)) + rec.tobytes())
+    with open(os.path.join(path, "points3D.bin"), "wb") as f:
+        f.write(struct.pack("<Q", len(model.points)))
+        for pid, (xyz, _) in model.points.items():
+            rgb, err, track = model.point_raw[pid]
+            f.write(struct.pack("<Q3d3Bd", pid, *map(float, xyz), *map(int, rgb), float(err)))
+            f.write(struct.pack("<Q", len(track)) + np.asarray(track, "<i4").tobytes())
+
+
+def _camera_dict(camera):
+    model, w, h, p = camera
+    return dict(model=int(model), width=int(w), height=int(h), params=[float(v) for v in p])
+
+
+def _same_pinhole(camera, undistorted):
+    """True when the undistorted camera describes the input image as it is: a pinhole input whose size, focal lengths
+    and principal point UndistortCamera left unchanged.  Only such an image is copied instead of warped, so that every
+    file in images/ has its camera's size and model."""
+    model, w, h, p = camera
+    if model not in (0, 1) or (w, h) != (undistorted["width"], undistorted["height"]):
+        return False
+    fx, fy, cx, cy = (p[0], p[0], p[1], p[2]) if model == 0 else tuple(p)
+    return [float(fx), float(fy), float(cx), float(cy)] == [float(v) for v in undistorted["params"]]
+
+
+def _write_file(path, data):
+    with open(path, "wb") as f:
+        f.write(data)
+
+
+def _undistort_points(camera, undistorted, xy):
+    """undistorted.ImgFromCam(camera.CamFromImg(xy)): the pinhole models in closed form, the others through
+    b2m_cam_from_img on the device."""
+    model, _, _, p = camera
+    if len(xy) == 0:
+        return xy
+    if model in (0, 1):
+        fx, fy, cx, cy = (p[0], p[0], p[1], p[2]) if model == 0 else tuple(p)
+        uv = np.stack([(xy[:, 0] - cx) / fx, (xy[:, 1] - cy) / fy], 1)
+    else:
+        uv = _core.cam_from_img(_camera_dict(camera), np.ascontiguousarray(xy, np.float64))
+    fx, fy, cx, cy = undistorted["params"]
+    return np.stack([fx * uv[:, 0] + cx, fy * uv[:, 1] + cy], 1)
+
+
+def _link_or_copy(src, dst, policy):
+    """FileCopy(src, dst, policy): a copy, a symbolic link or a hard link."""
+    import shutil
+    if os.path.lexists(dst):
+        os.remove(dst)
+    if policy == _core.CopyType.copy:
+        shutil.copyfile(src, dst)
+    elif policy == getattr(_core.CopyType, "soft-link"):
+        os.symlink(os.path.abspath(src), dst)
+    else:
+        os.link(src, dst)
+
+
+_CHUNK_IMAGES = 32
+_CHUNK_BYTES = 256 << 20
+
+
+def _undistort_run(items, options, device):
+    return _core._undistort_run(items, options, device)
+
+
+def undistort_images(output_path, input_path, image_path, image_list=[], output_type="COLMAP",
+                     copy_policy=None, num_patch_match_src_images=20, undistort_options=None):
+    """Undistort the images of the sparse model at `input_path` (files under `image_path`) into a COLMAP dense workspace
+    at `output_path`: images/ (K10, csrc/undistort.cu), sparse/ (every camera replaced by its undistorted PINHOLE
+    camera, the 2-D points mapped through it; poses, points and tracks unchanged) and stereo/ (patch-match.cfg,
+    fusion.cfg and the empty map directories), which patch_match_stereo and stereo_fusion read."""
+    from concurrent.futures import ThreadPoolExecutor
+
+    output_path, input_path, image_path = map(os.fspath, (output_path, input_path, image_path))
+    if not os.path.isdir(input_path):
+        raise ValueError(f"[images.h:105] Check Failed: ExistsDir(input_path) : Directory {input_path} does not exist.")
+    if not os.path.isdir(image_path):
+        raise ValueError(f"[images.h:106] Check Failed: ExistsDir(image_path) : Directory {image_path} does not exist.")
+    fmt = output_type.lower()
+    if fmt not in ("colmap", "pmvs", "cmp-mvs"):
+        raise ValueError("Invalid `output_type` - supported values are 'COLMAP', 'PMVS' or 'CMP-MVS'.")
+    if fmt != "colmap":
+        raise ValueError(f"[mvs.py] Check Failed: output_type == 'COLMAP' (the {output_type} format is not supported)")
+    if copy_policy is None:
+        copy_policy = _core.CopyType.copy
+    elif isinstance(copy_policy, str):
+        copy_policy = _core.CopyType(copy_policy)
+    if undistort_options is None:
+        undistort_options = _core.UndistortCameraOptions()
+    elif isinstance(undistort_options, dict):
+        undistort_options = _core.UndistortCameraOptions(undistort_options)
+    _core._check_undistort_options(undistort_options)
+
+    model = read_sparse(input_path)
+    by_name = {v[0]: k for k, v in model.images.items()}
+    if image_list:
+        ids = []
+        for name in image_list:
+            if name in by_name:
+                ids.append(by_name[name])
+            else:
+                _warn(f"Cannot find image {name}")
+    else:
+        ids = list(model.images)
+    for d in ("images", "sparse", "stereo/depth_maps", "stereo/normal_maps", "stereo/consistency_graphs"):
+        os.makedirs(os.path.join(output_path, d), exist_ok=True)
+    undistorted = {cid: _core._undistort_camera(undistort_options, _camera_dict(c)) for cid, c in model.cameras.items()}
+
+    todo = []  # (image id, input file, output file, "jpeg" | "pixels")
+    written = set()  # the images whose file is in images/
+    for iid in ids:
+        name, cid, _, _ = model.images[iid]
+        src, dst = os.path.join(image_path, name), os.path.join(output_path, "images", name)
+        os.makedirs(os.path.dirname(dst), exist_ok=True)
+        if _same_pinhole(model.cameras[cid], undistorted[cid]) and os.path.isfile(src):
+            _link_or_copy(src, dst, copy_policy)
+            written.add(iid)
+            continue
+        ext = os.path.splitext(name)[1].lower()
+        if ext not in (".jpg", ".jpeg", ".png"):
+            _warn(f"{name}: only JPEG and PNG images are written, skipped")
+            continue
+        if not os.path.isfile(src):
+            _warn(f"Cannot read image at path {src}")
+            continue
+        todo.append((iid, src, dst, "pixels" if ext == ".png" else "jpeg"))
+
+    chunks, cur, size = [], [], 0
+    for t in todo:
+        b = os.path.getsize(t[1])
+        if cur and (len(cur) == _CHUNK_IMAGES or size + b > _CHUNK_BYTES):
+            chunks.append(cur)
+            cur, size = [], 0
+        cur.append(t)
+        size += b
+    if cur:
+        chunks.append(cur)
+
+    def read(chunk):
+        out = []
+        for iid, src, _, kind in chunk:
+            with open(src, "rb") as f:
+                out.append((f.read(), _camera_dict(model.cameras[model.images[iid][1]]), kind))
+        return out
+
+    def write(chunk, results):
+        for (iid, _, dst, kind), r in zip(chunk, results):
+            if r["status"] != 0:
+                _warn(f"{model.images[iid][0]}: {r['error'] or 'does not undistort'}, skipped")
+                continue
+            _write_file(dst, r["data"] if kind == "jpeg" else _core._encode_png(r["data"]))
+            written.add(iid)
+
+    # the files of chunk k + 1 are read and those of chunk k - 1 written while chunk k runs on the device
+    with ThreadPoolExecutor(1) as reader, ThreadPoolExecutor(1) as writer:
+        pending = reader.submit(read, chunks[0]) if chunks else None
+        writing = None
+        for k, chunk in enumerate(chunks):
+            items = pending.result()
+            if k + 1 < len(chunks):
+                pending = reader.submit(read, chunks[k + 1])
+            results = _undistort_run(items, undistort_options, 0)
+            if writing is not None:
+                writing.result()
+            writing = writer.submit(write, chunk, results)
+        if writing is not None:
+            writing.result()
+
+    distorted = dict(model.cameras)
+    for cid in model.cameras:
+        u = undistorted[cid]
+        model.cameras[cid] = (u["model"], u["width"], u["height"], np.array(u["params"], np.float64))
+    for iid in model.images:
+        cid = model.images[iid][1]
+        q, t, xy, pids = model.image_raw[iid]
+        model.image_raw[iid] = (q, t, _undistort_points(distorted[cid], undistorted[cid], xy), pids)
+    write_sparse_bin(os.path.join(output_path, "sparse"), model)
+    # the configurations name the images that were written; a skipped image stays in sparse/ only
+    done = [iid for iid in ids if iid in written]
+    with open(os.path.join(output_path, "stereo", "patch-match.cfg"), "w") as f:
+        for iid in done:
+            f.write(model.images[iid][0] + "\n")
+            f.write(f"__auto__, {num_patch_match_src_images}\n" if num_patch_match_src_images > 0 else "__all__\n")
+    with open(os.path.join(output_path, "stereo", "fusion.cfg"), "w") as f:
+        for iid in done:
+            f.write(model.images[iid][0] + "\n")

@@ -188,9 +188,11 @@ def homography_pair(rng, width, height, size=1024):
 # Piecewise-planar dense scene (PatchMatch stereo tests and tools/bench_patch_match.py).
 # ---------------------------------------------------------------------------------------------
 
-def planar_scene(rng, n_views, width, height, focal=None, texture_size=512):
+def planar_scene(rng, n_views, width, height, focal=None, texture_size=512, distorted=None):
     """A textured back wall and two textured, tilted rectangles in front of it (they occlude the wall and, from some
-    views, each other), seen by `n_views` PINHOLE cameras on a grid near z = 0 looking towards +z.
+    views, each other), seen by `n_views` PINHOLE cameras on a grid near z = 0 looking towards +z.  `distorted`: None,
+    or per view a COLMAP camera dict(model, params) of the width x height image that view is rendered through instead
+    (stored as the camera's "camera"; K stays the pinhole one).
 
     Returns dict(planes, cameras [dict(K=(fx, fy, cx, cy), R, t) with x_cam = R x_world + t], width, height)."""
     focal = focal or 0.9 * width
@@ -217,18 +219,27 @@ def planar_scene(rng, n_views, width, height, focal=None, texture_size=512):
         y = np.cross(z, x)
         R = np.stack([x, y, z])
         cams.append(dict(K=(focal, focal, width / 2.0, height / 2.0), R=R, t=-R @ C))
+        if distorted is not None:
+            cams[-1]["camera"] = dict(model=distorted[i]["model"], width=width, height=height,
+                                      params=list(distorted[i]["params"]))
     return dict(planes=planes, cameras=cams, width=width, height=height)
 
 
 def render_planar(scene, i, offset=0.5):
     """View i of a planar_scene by ray casting: (grey uint8 [H, W], depth [H, W] (camera z), normal [H, W, 3] (camera
     frame, facing the camera), plane index [H, W]).  Rays through pixel (x + offset, y + offset): pixel centres at +0.5
-    by default, integer pixel coordinates (stereo fusion's convention) with offset=0."""
+    by default, integer pixel coordinates (stereo fusion's convention) with offset=0.  A view with a distorted camera
+    casts its rays through CamFromImg of those pixels (oracle/ransac.py)."""
     cam = scene["cameras"][i]
     W, H = scene["width"], scene["height"]
     fx, fy, cx, cy = cam["K"]
     ys, xs = np.mgrid[0:H, 0:W]
-    rays = np.stack([(xs + offset - cx) / fx, (ys + offset - cy) / fy, np.ones((H, W))], -1)  # camera frame, z = 1
+    if "camera" in cam:
+        from oracle import ransac as R
+        uv = R.cam_from_img(cam["camera"], np.stack([xs.ravel() + offset, ys.ravel() + offset], 1)).reshape(H, W, 2)
+        rays = np.concatenate([uv, np.ones((H, W, 1))], -1)
+    else:
+        rays = np.stack([(xs + offset - cx) / fx, (ys + offset - cy) / fy, np.ones((H, W))], -1)  # camera frame, z = 1
     R, t = cam["R"], cam["t"]
     C = -R.T @ t
     rw = rays @ R  # world directions (R^T r)
@@ -324,6 +335,62 @@ def write_dense_workspace(path, scene, sources="__auto__, 5", points_per_view=30
     with open(os.path.join(path, "stereo", "fusion.cfg"), "w") as f:
         for i in range(n):
             f.write(f"{names[i]}\n")
+    return renders
+
+
+def write_input_workspace(path, scene, points_per_view=300, seed=0, ext=".png"):
+    """The input of undistort_images for a planar_scene rendered through distorted cameras: images/view_XXX<ext> and
+    sparse/{cameras,images,points3D}.bin with one camera per view (its "camera", else PINHOLE K) and the 2-D
+    observations of the points (sampled from the views' true depths, tracked into every view that sees them
+    unoccluded).  Returns the renders."""
+    import os
+    from PIL import Image
+    from oracle import ransac as R
+    from . import mvs
+
+    rng = np.random.default_rng(seed)
+    os.makedirs(os.path.join(path, "images"), exist_ok=True)
+    n = len(scene["cameras"])
+    W, H = scene["width"], scene["height"]
+    renders = [render_planar(scene, i) for i in range(n)]
+    names = [f"view_{i:03d}{ext}" for i in range(n)]
+    for i in range(n):
+        Image.fromarray(renders[i][0]).save(os.path.join(path, "images", names[i]), quality=95)
+    cams = [c.get("camera", dict(model=1, width=W, height=H, params=list(c["K"]))) for c in scene["cameras"]]
+    m = mvs.SparseModel()
+    obs = [([], []) for _ in range(n)]
+    for i in range(n):
+        c = scene["cameras"][i]
+        d = renders[i][1]
+        ys, xs = rng.integers(0, H, points_per_view), rng.integers(0, W, points_per_view)
+        ok = d[ys, xs] > 0
+        uv = R.cam_from_img(cams[i], np.stack([xs + 0.5, ys + 0.5], 1))
+        Xc = np.c_[uv, np.ones(len(xs))] * d[ys, xs][:, None]
+        for X in ((Xc - c["t"]) @ c["R"])[ok]:
+            track = []
+            for j in range(n):
+                cj = scene["cameras"][j]
+                y = cj["R"] @ X + cj["t"]
+                if y[2] <= 0:
+                    continue
+                u, v = R.img_from_cam(cams[j], (y[:2] / y[2])[None])[0]
+                if 0 <= u < W and 0 <= v < H and abs(renders[j][1][int(v), int(u)] - y[2]) < 0.01 * y[2]:
+                    track.append((j, u, v))
+            if len(track) >= 2:
+                pid = len(m.points) + 1
+                full = []
+                for j, u, v in track:
+                    full.append((j + 1, len(obs[j][0])))
+                    obs[j][0].append((u, v))
+                    obs[j][1].append(pid)
+                m.points[pid] = (X, [j + 1 for j, _, _ in track])
+                m.point_raw[pid] = (np.array([128, 128, 128], np.uint8), 0.5, np.array(full, np.int64))
+    for i, c in enumerate(scene["cameras"]):
+        m.cameras[i + 1] = (cams[i]["model"], W, H, np.array(cams[i]["params"], np.float64))
+        m.images[i + 1] = (names[i], i + 1, c["R"], c["t"])
+        m.image_raw[i + 1] = (np.array(_rot_to_quat(c["R"])), np.asarray(c["t"], np.float64),
+                              np.array(obs[i][0], np.float64).reshape(-1, 2), np.array(obs[i][1], np.int64))
+    mvs.write_sparse_bin(os.path.join(path, "sparse"), m)
     return renders
 
 
